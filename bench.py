@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""bench.py — images/sec of the BYOL training step (ResNet-50 @224, synthetic data) on N B200s of one node.
+"""bench.py — images/sec of the BYOL training step (ResNet-50 @224, synthetic data) on N H100s of one node.
 
     python bench.py --gpus 1 --steps 10 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus 8 --steps 10 --warmup 3
     python bench.py --impl reference --steps 2 --warmup 1     # the reference algorithm on the host CPU cores
+    python bench.py --steps 10 --warmup 3 --dump-outputs out/  # + what the last timed step computed, as .npy
 
 One "step" = one pass of the hot path (/root/reference/main.py:579-624) over one synthetic batch: 4 encoder
 passes (online x2 with grad, EMA target x2), loss, backward, gradient all-reduce, LARS+SGD, EMA update.  One
@@ -56,7 +57,27 @@ def parse():
     ap.add_argument("--no-layers", action="store_true", help="skip the per-layer kernel roofline pass")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--layers-out", default=None, help="write the per-layer kernel table (JSON) to this path")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps write what the last timed step computed to DIR/<name>.npy (float32)")
     return ap.parse_args()
+
+
+DUMP_SAMPLE = 1 << 20   # parameter vectors are dumped as a fixed, seeded sample of this many entries (4 MB each)
+
+
+def dump_outputs(path, stats, model):
+    """The step's results as a caller receives them: the returned losses / accuracies and the parameters the step
+    updated (online weights after LARS, EMA target), the latter as the same seeded sample in every run."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    arrays = dict(stats)
+    theta, mean = model._engine.theta.detach(), model.target_network.mean.detach()
+    idx = torch.randperm(theta.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_SAMPLE].to(theta.device)
+    arrays["params_sample"] = theta[idx]
+    arrays["ema_params_sample"] = mean[idx]
+    for name, t in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 # ------------------------------------------------------------------------------------------------
@@ -121,11 +142,11 @@ def _host_threads():
 
 
 def _run_reference_main(arch, image_size, batch, steps, warmup):
-    """The UNMODIFIED reference (baseline/_ref/main.py, shipped by tools/ship_reference.py) on the host cores: its
+    """The UNMODIFIED reference (oracle/_ref, byte-compiled by build()) on the host cores: its
     BYOL / loss_function / LARS(SGD) driven by its own main.execute_graph, --no-cuda, synthetic batches."""
     import torch
-    ref = os.path.join(ROOT, "baseline", "_ref")
-    if not os.path.exists(os.path.join(ref, "main.py")):
+    ref = os.path.join(ROOT, "oracle", "_ref")
+    if not os.path.exists(os.path.join(ref, "main.pyc")):
         return None
     rep = REP_DIM.get(arch, 2048)
     argv, path = sys.argv, list(sys.path)
@@ -161,7 +182,7 @@ def run_cpu_reference(arch, image_size, batch, steps, warmup):
     import io
     import torch
     cores = _host_threads()
-    kind, what = "reference", "unmodified /root/reference main.execute_graph (baseline/_ref)"
+    kind, what = "reference", "unmodified reference main.execute_graph (oracle/_ref)"
     with contextlib.redirect_stdout(io.StringIO()):        # the reference prints a log line per call
         dt = _run_reference_main(arch, image_size, batch, steps, warmup)
     if dt is None:
@@ -202,7 +223,7 @@ def main_reference(args):
 
 
 # ------------------------------------------------------------------------------------------------
-# per-layer kernel roofline (dominant kernel = tcgen05 implicit-GEMM conv, fprop + dgrad + wgrad)
+# per-layer kernel roofline (dominant kernel = wgmma implicit-GEMM conv, fprop + dgrad + wgrad)
 # ------------------------------------------------------------------------------------------------
 def layer_table(model, batch, image_size, reps=5):
     """Time every distinct conv shape of the encoder in isolation (CUDA events on the launching stream, L2
@@ -317,9 +338,10 @@ def main_b200(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_sustained = peaks.get("bf16_tflops_sustained", 1400.0)
-    peak_burst = peaks.get("bf16_tflops", 1590.0)
-    peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)"
+    # without a measured peak: NVIDIA's H100 SXM data sheet, dense bf16 at 700 W (a rate, not one reached here)
+    peak_sustained = peaks.get("bf16_tflops_sustained", 989.4)
+    peak_burst = peaks.get("bf16_tflops", 989.4)
+    peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "H100 SXM data sheet, dense bf16"
 
     torch.manual_seed(0)
     rep = REP_DIM.get(args.arch, 2048)
@@ -366,6 +388,8 @@ def main_b200(args):
     host_ms = 1000.0 * (time.perf_counter() - t_host0) / args.steps   # Python time to ENQUEUE one step
     e1.record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, stats, model)
     ms = max_over_ranks(e0.elapsed_time(e1))
     launches = (_lib.launch_count[0] - l0) // args.steps
     ms1 = torch.cuda.memory_stats()
@@ -427,33 +451,16 @@ def main_b200(args):
                 "frac": (step_tflops / peak_sustained) if step_tflops else None, "traffic": None,
                 "what": "whole step: images/s/GPU x %.4f algorithmic GFLOP/image vs sustained bf16 peak, %s"
                         % (alg or 0.0, peak_src)}
-    # DRAM traffic of one step from the committed ncu launch list (profiles/traffic_r02.json: dram__bytes_read.sum +
-    # dram__bytes_write.sum per launch, summed over one eager step of this same command) - only for the workload it
-    # was captured on
-    traffic = None
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "traffic_r02.json")))
-        if (args.arch, R, b, args.precision) == ("resnet50", 224, 512, "bf16"):
-            traffic = tr
-    except Exception:
-        pass
-    if traffic is not None:
-        roofline["traffic"] = traffic["step_dram_bytes"]
-        hbm_peak = peaks.get("hbm_gbs", 6485.8)
-        gbs = traffic["step_dram_bytes"] / (ms / args.steps / 1000.0) / 1e9
-        roofline["hbm_view"] = {"achieved": gbs, "peak": hbm_peak, "unit": "GB/s", "frac": gbs / hbm_peak,
-                                "what": "DRAM bytes of one step (ncu, profiles/traffic_r02.json) / measured step time: "
-                                        "in aggregate the step is bound by HBM traffic, not by the tensor pipe"}
     if rank == 0 and world == 1 and not args.no_layers:
         rows, agg = layer_table(model, b, R)
         conv_flops = sum(v["launch_gflop"] for v in agg.values())
         conv_ms = sum(v["ms_per_step"] for v in agg.values())
         roofline["dominant_kernel"] = {
-            "name": "conv_igemm_kernel / conv_wgrad_kernel (tcgen05 implicit GEMM)",
+            "name": "conv_igemm_kernel / conv_wgrad_kernel (wgmma implicit GEMM)",
             "achieved": conv_flops / conv_ms, "peak": peak_burst, "unit": "TFLOP/s",
             "frac": conv_flops / conv_ms / peak_burst, "isolated_ms_per_step": conv_ms,
             "share_of_step": conv_ms / (ms / args.steps), "by_kind": agg,
-            "traffic": traffic["tcgen05_family_dram_bytes"] if traffic is not None else None,
+            "traffic": None,
             "how": "every distinct conv shape timed alone with CUDA events, L2 flushed between launches, weighted "
                    "by its count in one step (4 fprop passes, 2 dgrad/wgrad passes); peak = burst bf16, %s" % peak_src}
         if args.layers_out:

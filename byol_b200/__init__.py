@@ -1,4 +1,4 @@
-"""byol_b200 — B200-native (sm_100a) BYOL training step behind the jramapuram/BYOL Python API.
+"""byol_b200 — H100-native (sm_90a) BYOL training step behind the jramapuram/BYOL Python API.
 
 Importing the package loads the mandatory C-ABI CUDA library (``libbyol_b200.so``); there is no fallback.
 """

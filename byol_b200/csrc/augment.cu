@@ -202,9 +202,9 @@ __device__ __forceinline__ void colour_ops(const float* q, float& r, float& g, f
 }
 
 // mean grey level per (sample, view) of the image as it stands right before adjust_contrast (sum in fp32 per block,
-// fp64 atomics); skipped (mean unused) when the jitter is off
+// blocks combined in fixed point); skipped (mean unused) when the jitter is off
 __global__ void augment_gray_mean_kernel(const float* __restrict__ src, const float* __restrict__ params,
-                                         double* __restrict__ gray_sum, int N, int Hs, int Ws, int R) {
+                                         Fix128* __restrict__ gray_sum, int N, int Hs, int Ws, int R) {
   const int sv = blockIdx.y;                      // sample * 2 + view... laid out view-major: sv = view * N + n
   const int n = sv % N;
   const float* q = params + (int64_t)sv * AP;
@@ -224,18 +224,18 @@ __global__ void augment_gray_mean_kernel(const float* __restrict__ src, const fl
   if (warp == 0) {
     float v = lane < (int)(blockDim.x >> 5) ? sh[lane] : 0.f;
     v = warp_sum(v);
-    if (lane == 0) atomicAdd(gray_sum + sv, (double)v);
+    if (lane == 0) fix_add(gray_sum + sv, v);   // fixed point: order-independent
   }
 }
 
 // out[view][n, c, y, x] (fp32 NCHW): crop / resize / flip, colour jitter, grayscale
 __global__ void augment_apply_kernel(const float* __restrict__ src, const float* __restrict__ params,
-                                     const double* __restrict__ gray_sum, float* __restrict__ out, int N, int Hs, int Ws,
+                                     const Fix128* __restrict__ gray_sum, float* __restrict__ out, int N, int Hs, int Ws,
                                      int R) {
   const int sv = blockIdx.y;
   const int n = sv % N;
   const float* q = params + (int64_t)sv * AP;
-  const float mean_gray = (float)(gray_sum[sv] / (double)(R * R));
+  const float mean_gray = (float)(fix_value(gray_sum[sv]) / (double)(R * R));
   float* o = out + (int64_t)sv * 3 * R * R;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < R * R; i += gridDim.x * blockDim.x) {
     float r, g, b;
@@ -290,21 +290,26 @@ extern "C" int byol_augment_params(float* params, int N, int Hs, int Ws, uint64_
 }
 
 // src: fp32 NCHW [N, 3, Hs, Ws] in [0, 1]; out: fp32 [2, N, 3, R, R] (view 1 | view 2); tmp: same size as out (blur);
-// gray_sum: 2N doubles of scratch; ksize: odd Gaussian kernel size (0 = no blur stage).
+// gray_sum: part of the ABI, no longer used (the per-view sums live in the stream's fix_scratch); ksize: odd Gaussian kernel size (0 = no blur stage).
 extern "C" int byol_augment_apply(const float* src, const float* params, float* out, float* tmp, double* gray_sum,
                                   int N, int Hs, int Ws, int R, int ksize, cudaStream_t stream) {
   BYOL_CHECK_ARG(src && params && out && gray_sum && N > 0 && R > 0, "byol_augment_apply: bad args");
   BYOL_CHECK_ARG(ksize == 0 || (ksize % 2 == 1 && ksize < 2 * R - 1 && tmp != nullptr), "byol_augment_apply: bad ksize %d", ksize);
-  cudaError_t e = cudaMemsetAsync(gray_sum, 0, 2 * (size_t)N * sizeof(double), stream);
-  if (e != cudaSuccess) { set_last_error("byol_augment_apply: memset failed: %s", cudaGetErrorString(e)); return -2; }
+  Fix128* gsum = fix_scratch(stream, 2 * (int64_t)N);
+  if (gsum == nullptr) return -2;
   int bx = (R * R + 255) / 256;
   if (bx > 64) bx = 64;
   dim3 grid((unsigned)bx, (unsigned)(2 * N));
-  augment_gray_mean_kernel<<<grid, 256, 0, stream>>>(src, params, gray_sum, N, Hs, Ws, R);
-  augment_apply_kernel<<<grid, 256, 0, stream>>>(src, params, gray_sum, out, N, Hs, Ws, R);
+  augment_gray_mean_kernel<<<grid, 256, 0, stream>>>(src, params, gsum, N, Hs, Ws, R);
+  augment_apply_kernel<<<grid, 256, 0, stream>>>(src, params, gsum, out, N, Hs, Ws, R);
+  // every block of augment_apply_kernel read the sums: leave the scratch zeroed (fix_scratch)
+  if (cudaMemsetAsync(gsum, 0, 2 * (size_t)N * sizeof(Fix128), stream) != cudaSuccess) {
+    set_last_error("byol_augment_apply: memset failed");
+    return -2;
+  }
   if (ksize > 0) {
     augment_blur_kernel<<<grid, 256, 0, stream>>>(out, tmp, params, R, ksize, 1);
     augment_blur_kernel<<<grid, 256, 0, stream>>>(tmp, out, params, R, ksize, 0);
   }
-  return check_launch("augment kernels");
+  return fix_done(stream, check_launch("augment kernels"));
 }

@@ -21,10 +21,10 @@ namespace byol {
 // column statistics: x [M, C] bf16 (C % 8 == 0).  Each thread owns one 8-channel group and strides
 // over rows; a block covers ROWS_PER_BLOCK rows.  Partial sums are combined with fp32 atomics.
 // ---------------------------------------------------------------------------------------------
-__global__ void bn_stats_kernel(const bf16* __restrict__ x, float* __restrict__ sum, float* __restrict__ sqsum,
+__global__ void bn_stats_kernel(const bf16* __restrict__ x, Fix128* __restrict__ sum, Fix128* __restrict__ sqsum,
                                 int M, int C, int rows_per_block) {
-  extern __shared__ float red[];                   // [2][C] block-level partial sums
-  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) red[c] = 0.f;
+  extern __shared__ Fix128 red[];               // [2][C] block-level partial sums (fixed point)
+  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) red[c] = Fix128{0ull, 0ll, 0.0};
   __syncthreads();
   const int groups = C >> 3;                       // 8-channel groups per row
   const int tpr = groups < (int)blockDim.x ? groups : (int)blockDim.x;  // threads used per row pass
@@ -51,15 +51,15 @@ __global__ void bn_stats_kernel(const bf16* __restrict__ x, float* __restrict__ 
       }
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
-        atomicAdd(red + g * 8 + e, s[e]);
-        atomicAdd(red + C + g * 8 + e, q[e]);
+        fix_add(red + g * 8 + e, s[e]);
+        fix_add(red + C + g * 8 + e, q[e]);
       }
     }
   }
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    atomicAdd(sum + c, red[c]);
-    atomicAdd(sqsum + c, red[C + c]);
+    fix_add_raw(sum + c, red[c]);
+    fix_add_raw(sqsum + c, red[C + c]);
   }
 }
 
@@ -234,7 +234,9 @@ bn_bwd_apply_fixed_kernel(const bf16* __restrict__ g, const bf16* __restrict__ x
                           float* __restrict__ dbeta) {
   const int groups = C >> 3;
   if (blockIdx.x == 0 && dgamma != nullptr) {
-    for (int c = threadIdx.x; c < C; c += blockDim.x) {   // atomics: the two online views may run concurrently
+    // atomics: the two online views may run concurrently; each adds once per element to the zeroed gradient, and two
+    // additions onto zero give the same bits in either order
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
       atomicAdd(dgamma + c, s2_local[c]);
       atomicAdd(dbeta + c, s1_local[c]);
     }
@@ -284,10 +286,10 @@ template <int MASK>
 __global__ void bn_bwd_reduce_kernel(const bf16* __restrict__ g, const bf16* __restrict__ x,
                                      const bf16* __restrict__ act, const float* __restrict__ scale,
                                      const float* __restrict__ shift, const float* __restrict__ mean,
-                                     const float* __restrict__ invstd, float* __restrict__ s1,
-                                     float* __restrict__ s2, int M, int C, int rows_per_block) {
-  extern __shared__ float red[];                   // [2][C]
-  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) red[c] = 0.f;
+                                     const float* __restrict__ invstd, Fix128* __restrict__ s1,
+                                     Fix128* __restrict__ s2, int M, int C, int rows_per_block) {
+  extern __shared__ Fix128 red[];                   // [2][C]
+  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) red[c] = Fix128{0ull, 0ll, 0.0};
   __syncthreads();
   const int groups = C >> 3;
   const int tpr = groups < (int)blockDim.x ? groups : (int)blockDim.x;
@@ -348,29 +350,29 @@ __global__ void bn_bwd_reduce_kernel(const bf16* __restrict__ g, const bf16* __r
     }
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
-      atomicAdd(red + gi * 8 + e, a1[e]);
-      atomicAdd(red + C + gi * 8 + e, a2[e]);
+      fix_add(red + gi * 8 + e, a1[e]);
+      fix_add(red + C + gi * 8 + e, a2[e]);
     }
   }
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    atomicAdd(s1 + c, red[c]);
-    atomicAdd(s2 + c, red[C + c]);
+    fix_add_raw(s1 + c, red[c]);
+    fix_add_raw(s2 + c, red[C + c]);
   }
 }
 
 // Same reduction with the access pattern of the "fixed" elementwise kernels: the whole grid sweeps the tensor front to
 // back (grid-stride over 8-channel vectors; (gridDim.x * blockDim.x) % (C/8) == 0 pins every thread to ONE channel
 // group), instead of one private row range per block.  1184 private sequential streams per operand cost DRAM row
-// locality: the row-range kernel reads at ~3.7 TB/s where the sweeping kernels reach ~5.4 TB/s (ncu, round 2).
+// locality: the row-range kernel reads more slowly than the sweeping kernels.
 template <int MASK>
 __global__ void __launch_bounds__(256)
 bn_bwd_reduce_fixed_kernel(const bf16* __restrict__ g, const bf16* __restrict__ x, const bf16* __restrict__ act,
                            const float* __restrict__ scale, const float* __restrict__ shift,
-                           const float* __restrict__ mean, const float* __restrict__ invstd, float* __restrict__ s1,
-                           float* __restrict__ s2, int64_t nvec, int C) {
-  extern __shared__ float red[];                   // [2][C]
-  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) red[c] = 0.f;
+                           const float* __restrict__ mean, const float* __restrict__ invstd, Fix128* __restrict__ s1,
+                           Fix128* __restrict__ s2, int64_t nvec, int C) {
+  extern __shared__ Fix128 red[];                   // [2][C]
+  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) red[c] = Fix128{0ull, 0ll, 0.0};
   __syncthreads();
   const int groups = C >> 3;
   const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -424,13 +426,13 @@ bn_bwd_reduce_fixed_kernel(const bf16* __restrict__ g, const bf16* __restrict__ 
   }
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
-    atomicAdd(red + gi * 8 + e, a1[e]);
-    atomicAdd(red + C + gi * 8 + e, a2[e]);
+    fix_add(red + gi * 8 + e, a1[e]);
+    fix_add(red + C + gi * 8 + e, a2[e]);
   }
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    atomicAdd(s1 + c, red[c]);
-    atomicAdd(s2 + c, red[C + c]);
+    fix_add_raw(s1 + c, red[c]);
+    fix_add_raw(s2 + c, red[C + c]);
   }
 }
 
@@ -447,7 +449,9 @@ __global__ void bn_bwd_apply_kernel(const bf16* __restrict__ g, const bf16* __re
   const int groups = C >> 3;
   if (blockIdx.x == 0 && dgamma != nullptr) {
     // parameter gradients come from the rank-LOCAL sums (SyncBatchNorm.backward, _functions.py:122-170)
-    for (int c = threadIdx.x; c < C; c += blockDim.x) {   // atomics: the two online views may run concurrently
+    // atomics: the two online views may run concurrently; each adds once per element to the zeroed gradient, and two
+    // additions onto zero give the same bits in either order
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
       atomicAdd(dgamma + c, s2_local[c]);
       atomicAdd(dbeta + c, s1_local[c]);
     }
@@ -516,7 +520,7 @@ __global__ void bn_bwd_coeffs_kernel(const float* __restrict__ s12, const float*
 
 // column sum of a bf16 or fp32 [M, C] matrix (bias gradients): out[c] += sum_r x[r, c]
 template <typename T>
-__global__ void col_sum_kernel(const T* __restrict__ x, float* __restrict__ out, int M, int C, int ld,
+__global__ void col_sum_kernel(const T* __restrict__ x, Fix128* __restrict__ out, int M, int C, int ld,
                                int rows_per_block) {
   const int c = blockIdx.y * blockDim.x + threadIdx.x;
   if (c >= C) return;
@@ -525,7 +529,7 @@ __global__ void col_sum_kernel(const T* __restrict__ x, float* __restrict__ out,
   if (row_end > M) row_end = M;
   float s = 0.f;
   for (int r = row_begin; r < row_end; ++r) s += (float)x[(int64_t)r * ld + c];
-  atomicAdd(out + c, s);
+  fix_add(out + c, s);
 }
 
 // grid for the "fixed channel group" elementwise kernels: (grid*256) % groups == 0, or 0 if impossible
@@ -533,14 +537,14 @@ static inline int fixed_grid(int64_t nvec, int groups) {
   int unit = groups > 256 ? groups / 256 : 1;          // blocks per channel period
   if (groups > 256 ? (groups % 256 != 0) : (256 % groups != 0)) return 0;
   int64_t b = (nvec + 255) / 256;
-  int64_t cap = 148 * 8;
+  int64_t cap = 132 * 8;
   if (b > cap) b = cap;
   b = (b + unit - 1) / unit * unit;
   if (b < unit) b = unit;
   return (int)b;
 }
 
-static inline int grid_for(int64_t n, int block, int max_blocks = 148 * 16) {
+static inline int grid_for(int64_t n, int block, int max_blocks = 132 * 16) {
   int64_t b = (n + block - 1) / block;
   if (b > max_blocks) b = max_blocks;
   if (b < 1) b = 1;
@@ -553,12 +557,20 @@ using namespace byol;
 
 // stats must be zeroed by the caller; accumulates sum into stats[0:C], sqsum into stats[C:2C]
 extern "C" int byol_bn_stats(const void* x, float* stats, int M, int C, cudaStream_t stream) {
-  BYOL_CHECK_ARG(x && stats && M > 0 && C % 8 == 0 && C <= 5120, "byol_bn_stats: bad args (M=%d C=%d)", M, C);
-  int rows_per_block = (M + 148 * 8 - 1) / (148 * 8);
+  BYOL_CHECK_ARG(x && stats && M > 0 && C % 8 == 0 && C <= 4800, "byol_bn_stats: bad args (M=%d C=%d)", M, C);
+  int rows_per_block = (M + 132 * 8 - 1) / (132 * 8);
   if (rows_per_block < 32) rows_per_block = 32;
   const int blocks = (M + rows_per_block - 1) / rows_per_block;
-  bn_stats_kernel<<<blocks, 256, 2 * C * sizeof(float), stream>>>((const bf16*)x, stats, stats + C, M, C, rows_per_block);
-  return check_launch("bn_stats_kernel");
+  const size_t red_bytes = 2 * (size_t)C * sizeof(Fix128);
+  if (red_bytes > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(bn_stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
+    if (e != cudaSuccess) { set_last_error("byol_bn_stats: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e)); return -2; }
+  }
+  Fix128* fx = fix_scratch(stream, 2 * (int64_t)C);
+  if (fx == nullptr) return -2;
+  bn_stats_kernel<<<blocks, 256, red_bytes, stream>>>((const bf16*)x, fx, fx + C, M, C, rows_per_block);
+  if (check_launch("bn_stats_kernel") != 0) return -100;
+  return fix_done(stream, fix_flush(fx, stats, 2 * (int64_t)C, stream));
 }
 
 // stats: [L][2C]; coeffs: [L][4][C]; gamma_l / beta_l for l < L (L <= 4)
@@ -617,26 +629,37 @@ extern "C" int byol_bn_bwd_reduce(const void* g, const void* x, const void* act,
   BYOL_CHECK_ARG(mask_mode >= 0 && mask_mode <= 3, "byol_bn_bwd_reduce: bad mask_mode %d", mask_mode);
   BYOL_CHECK_ARG(mask_mode < 2 || act, "byol_bn_bwd_reduce: mask_mode 2/3 needs act");
   BYOL_CHECK_ARG(mask_mode != 1 || (scale && shift), "byol_bn_bwd_reduce: mask_mode 1 needs scale/shift");
-  int rows_per_block = (M + 148 * 8 - 1) / (148 * 8);
+  int rows_per_block = (M + 132 * 8 - 1) / (132 * 8);
   if (rows_per_block < 32) rows_per_block = 32;
   const int blocks = (M + rows_per_block - 1) / rows_per_block;
   const bf16 *gp = (const bf16*)g, *xp = (const bf16*)x, *ap = (const bf16*)act;
-  const size_t red_bytes = 2 * (size_t)C * sizeof(float);
+  const size_t red_bytes = 2 * (size_t)C * sizeof(Fix128);
   const int64_t nvec = (int64_t)M * C / 8;
-  const int fg = red_bytes <= 48 * 1024 ? fixed_grid(nvec, C / 8) : 0;
+  Fix128* fx = fix_scratch(stream, 2 * (int64_t)C);
+  if (fx == nullptr) return -2;
+  BYOL_CHECK_ARG(red_bytes <= 226 * 1024, "byol_bn_bwd_reduce: C=%d too wide (at most 4800 channels)", C);
+  const int fg = fixed_grid(nvec, C / 8);
   if (fg > 0) {
+    if (red_bytes > 48 * 1024) {   // wide layers: opt in to > 48 KB of dynamic smem for the per-block accumulators
+      cudaError_t e = cudaSuccess;
+      if (mask_mode == 0) e = cudaFuncSetAttribute(bn_bwd_reduce_fixed_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
+      else if (mask_mode == 1) e = cudaFuncSetAttribute(bn_bwd_reduce_fixed_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
+      else if (mask_mode == 2) e = cudaFuncSetAttribute(bn_bwd_reduce_fixed_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
+      else e = cudaFuncSetAttribute(bn_bwd_reduce_fixed_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
+      if (e != cudaSuccess) { set_last_error("byol_bn_bwd_reduce: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e)); return -2; }
+    }
     if (mask_mode == 0)
-      bn_bwd_reduce_fixed_kernel<0><<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, s12, s12 + C, nvec, C);
+      bn_bwd_reduce_fixed_kernel<0><<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, nvec, C);
     else if (mask_mode == 1)
-      bn_bwd_reduce_fixed_kernel<1><<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, s12, s12 + C, nvec, C);
+      bn_bwd_reduce_fixed_kernel<1><<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, nvec, C);
     else if (mask_mode == 2)
-      bn_bwd_reduce_fixed_kernel<2><<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, s12, s12 + C, nvec, C);
+      bn_bwd_reduce_fixed_kernel<2><<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, nvec, C);
     else
-      bn_bwd_reduce_fixed_kernel<3><<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, s12, s12 + C, nvec, C);
-    return check_launch("bn_bwd_reduce_fixed_kernel");
+      bn_bwd_reduce_fixed_kernel<3><<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, nvec, C);
+    if (check_launch("bn_bwd_reduce_fixed_kernel") != 0) return -100;
+    return fix_done(stream, fix_flush(fx, s12, 2 * (int64_t)C, stream));
   }
   if (red_bytes > 48 * 1024) {   // very wide BatchNorm1d (head_latent_size >= 6144): opt in to > 48 KB of dynamic smem
-    BYOL_CHECK_ARG(red_bytes <= 200 * 1024, "byol_bn_bwd_reduce: C=%d too wide", C);
     cudaError_t e = cudaSuccess;
     if (mask_mode == 0) e = cudaFuncSetAttribute(bn_bwd_reduce_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
     else if (mask_mode == 1) e = cudaFuncSetAttribute(bn_bwd_reduce_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
@@ -645,14 +668,15 @@ extern "C" int byol_bn_bwd_reduce(const void* g, const void* x, const void* act,
     if (e != cudaSuccess) { set_last_error("byol_bn_bwd_reduce: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e)); return -2; }
   }
   if (mask_mode == 0)
-    bn_bwd_reduce_kernel<0><<<blocks, 256, 2 * C * sizeof(float), stream>>>(gp, xp, ap, scale, shift, mean, invstd, s12, s12 + C, M, C, rows_per_block);
+    bn_bwd_reduce_kernel<0><<<blocks, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, M, C, rows_per_block);
   else if (mask_mode == 1)
-    bn_bwd_reduce_kernel<1><<<blocks, 256, 2 * C * sizeof(float), stream>>>(gp, xp, ap, scale, shift, mean, invstd, s12, s12 + C, M, C, rows_per_block);
+    bn_bwd_reduce_kernel<1><<<blocks, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, M, C, rows_per_block);
   else if (mask_mode == 2)
-    bn_bwd_reduce_kernel<2><<<blocks, 256, 2 * C * sizeof(float), stream>>>(gp, xp, ap, scale, shift, mean, invstd, s12, s12 + C, M, C, rows_per_block);
+    bn_bwd_reduce_kernel<2><<<blocks, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, M, C, rows_per_block);
   else
-    bn_bwd_reduce_kernel<3><<<blocks, 256, 2 * C * sizeof(float), stream>>>(gp, xp, ap, scale, shift, mean, invstd, s12, s12 + C, M, C, rows_per_block);
-  return check_launch("bn_bwd_reduce_kernel");
+    bn_bwd_reduce_kernel<3><<<blocks, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, M, C, rows_per_block);
+  if (check_launch("bn_bwd_reduce_kernel") != 0) return -100;
+  return fix_done(stream, fix_flush(fx, s12, 2 * (int64_t)C, stream));
 }
 
 // s12: global (cross-rank) sums used for dy; s12_local: this rank's sums accumulated into dgamma/dbeta
@@ -697,11 +721,14 @@ extern "C" int byol_col_sum(const void* x, float* out, int M, int C, int ld, int
   int rows_per_block = (M + 63) / 64;
   if (rows_per_block < 16) rows_per_block = 16;
   dim3 grid((M + rows_per_block - 1) / rows_per_block, (C + 127) / 128);
+  Fix128* fx = fix_scratch(stream, C);
+  if (fx == nullptr) return -2;
   if (is_f32)
-    col_sum_kernel<float><<<grid, 128, 0, stream>>>((const float*)x, out, M, C, ld, rows_per_block);
+    col_sum_kernel<float><<<grid, 128, 0, stream>>>((const float*)x, fx, M, C, ld, rows_per_block);
   else
-    col_sum_kernel<bf16><<<grid, 128, 0, stream>>>((const bf16*)x, out, M, C, ld, rows_per_block);
-  return check_launch("col_sum_kernel");
+    col_sum_kernel<bf16><<<grid, 128, 0, stream>>>((const bf16*)x, fx, M, C, ld, rows_per_block);
+  if (check_launch("col_sum_kernel") != 0) return -100;
+  return fix_done(stream, fix_flush(fx, out, C, stream));
 }
 
 extern "C" int byol_bn_bwd_prep(const float* mean, const float* invstd, float* out, int C, cudaStream_t stream) {

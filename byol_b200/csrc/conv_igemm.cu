@@ -1,4 +1,4 @@
-// byol_b200 — implicit-GEMM convolution / linear layers on tcgen05 tensor cores (sm_100a).
+// byol_b200 — implicit-GEMM convolution / linear layers on Hopper tensor cores (wgmma, sm_90a).
 //
 // Replaces the cuDNN conv fwd/dgrad/wgrad and cuBLAS Linear calls reached from the reference at
 // /root/reference/main.py:229-240 (BYOL.prediction: base_network -> head -> predictor).
@@ -9,13 +9,9 @@
 //   out[m, n] = sum_{tap, c} src[pix(m, tap), c] * Wt[n, tap*C + c]          (fprop and dgrad)
 //   dW[n, tap, c] += sum_m dY[m, n] * src[pix(m, tap), c]                     (wgrad)
 //
-// One CTA computes a 128 x BN tile.  Warp roles:
-//   warps 0-3 : A-operand gather (cp.async 16 B, zero-fill for padding) and, later, the epilogue
-//               (tcgen05.ld TMEM -> registers -> global)
-//   warp 4    : TMEM allocation + single-thread tcgen05.mma issue
-//   warp 5    : barrier init + TMA producer (weights always; activations when the conv is a
-//               plain GEMM, i.e. 1x1 stride 1 / Linear)
-// smem operand tiles use the 128-byte swizzle; accumulators live in TMEM.
+// One CTA computes a 128 x BN tile.  smem operand tiles use the 128-byte swizzle; two MMA warpgroups (wgmma) own
+// 64 tile rows each and keep their accumulators in registers; a finished tile is handed to the epilogue warps
+// (one tile row per lane) through an fp32 tile in shared memory.
 #include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -39,6 +35,7 @@ struct ConvGemmParams {
   const float* bias;   // optional, [Ndim]
   float* col_sum;      // optional, [Ndim] fp32: += sum over rows of the stored value
   float* col_sqsum;    // optional, [Ndim] fp32: += sum over rows of value^2
+  Fix128* fx;       // with col_sum: [2][Ndim] fixed-point accumulators of both sums (fix_scratch)
   int Nimg, Hs, Ws, C;
   int Ho, Wo;
   int KH, KW;
@@ -89,7 +86,7 @@ __device__ __forceinline__ TileInfo tile_info(const ConvGemmParams& p, int tile,
 
 // Epilogue geometry.  The TMA-operand variant (plain GEMM: 1x1 / stride 1 convolutions and the MLP layers) has no
 // gather warps and is bound by its epilogue (few k-blocks per tile, outputs up to 4x the inputs), so it runs EIGHT
-// epilogue warps: warps w and w + 4 share TMEM lane quarter w & 3 and split the tile's columns.
+// epilogue warps: warps w and w + 4 share the row quarter w & 3 of the tile and split its columns.
 // Output staging: [32 rows][32 cols] chunks with the 64-byte swizzle, NBUF staging buffers per warp.  (A variant with
 // 128-byte staging rows and a 2-stage operand ring was measured slower for every K >= 128 and removed.)
 template <int BN, int STAGES, bool A_TMA>
@@ -104,31 +101,36 @@ struct SmemLayout {
   // output staging.  The TMA swizzle patterns repeat every 512 B (64-byte mode) / 1024 B (128-byte mode), so every
   // buffer starts on such a boundary (1024-aligned base + multiples of 2048 / 4096).
   static constexpr int STAGE_OUT_OFF = B_OFF + STAGES * B_STAGE_BYTES;
-  static constexpr int BAR_OFF = STAGE_OUT_OFF + EW * STAGE_PER_WARP;
+  // finished accumulator tile [BM][ACC_LD] fp32 (MMA warpgroups -> epilogue warps)
+  static constexpr int ACC_LD = acc_ld(BN);
+  static constexpr int ACC_OFF = STAGE_OUT_OFF + EW * STAGE_PER_WARP;
+  static constexpr int BAR_OFF = ACC_OFF + BM * ACC_LD * 4;
   static constexpr int NEEDED = BAR_OFF + 256;
   static constexpr int TOTAL = NEEDED + 768;   // slack for the run-time 1024-byte alignment of the base
-  static_assert(TOTAL <= 115712, "two CTAs per SM need <= 113 KB of dynamic shared memory each");
+  static_assert(TOTAL <= 232448, "one CTA per SM: <= 227 KB of dynamic shared memory");
 };
 
 // ---------------------------------------------------------------------------------------------
 // fprop / dgrad kernel — persistent: each CTA loops over output tiles (tile = blockIdx.x + i*gridDim.x,
-// n-tile fastest so that concurrently running CTAs share the A tile through L2).  The smem operand ring and
-// the two TMEM accumulator stages run across tile boundaries, so the producers prefetch tile i+1 and the
-// tensor core works on it while the epilogue warps drain tile i.
-//   warps 0 .. EW-1     : epilogue (TMEM lanes 32*(w & 3) .. +31, column group w >> 2)
-//   next 4 (!A_TMA)     : A-operand gather producers
-//   next warp           : MMA issuer (+ TMEM alloc / dealloc)
-//   last warp           : barrier init + TMA producer
+// n-tile fastest so that concurrently running CTAs share the A tile through L2).  The smem operand ring runs across
+// tile boundaries and the accumulators of tile i+1 build up in registers while the epilogue warps drain tile i from
+// shared memory, so producers, tensor cores and epilogue overlap.
+//   warps 0 .. EW-1     : epilogue (tile rows 32*(w & 3) .. +31, column group w >> 2)
+//   warps 4-7 (!A_TMA)  : A-operand gather producers
+//   warps 8-15          : two MMA warpgroups (tile rows 0-63 / 64-127)
+//   warp 16             : barrier init + TMA producer
 // ---------------------------------------------------------------------------------------------
+static constexpr int IG_THREADS = 17 * 32;
+
 template <int BN, int STAGES, bool A_TMA>
-__global__ void __launch_bounds__(320, 2)
+__global__ void __launch_bounds__(IG_THREADS, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB,
                   const __grid_constant__ CUtensorMap tmapC, const ConvGemmParams p, const int num_tiles) {
   using L = SmemLayout<BN, STAGES, A_TMA>;
   constexpr int EW = L::EW;
   constexpr int CPW = L::CPW;
   constexpr int MMA_WARP = 8;
-  constexpr int TMA_WARP = MMA_WARP + 1;
+  constexpr int TMA_WARP = MMA_WARP + 8;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   if (smem + L::NEEDED > smem_raw + L::TOTAL) __trap();   // the dynamic smem base was less aligned than assumed
@@ -136,10 +138,10 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   uint8_t* smemB = smem + L::B_OFF;
   uint64_t* full_bar = (uint64_t*)(smem + L::BAR_OFF);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;   // [2] accumulator stage ready for the epilogue
-  uint64_t* tempty_bar = tfull_bar + 2;       // [2] accumulator stage drained
-  uint32_t* tmem_slot = (uint32_t*)(tempty_bar + 2);
+  uint64_t* tfull_bar = empty_bar + STAGES;   // accumulator tile ready for the epilogue
+  uint64_t* tempty_bar = tfull_bar + 1;       // accumulator tile drained
   uint8_t* stage_out = smem + L::STAGE_OUT_OFF;   // 1024-byte aligned
+  float* accbuf = reinterpret_cast<float*>(smem + L::ACC_OFF);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -148,34 +150,25 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   if (warp == TMA_WARP && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], A_TMA ? 1u : 129u);
-      mbar_init(&empty_bar[s], 1u);
+      mbar_init(&empty_bar[s], 2u);   // one arrival per MMA warpgroup
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull_bar[a], 1u);
-      mbar_init(&tempty_bar[a], (uint32_t)EW);   // one arrival per epilogue warp
-    }
+    mbar_init(tfull_bar, 256u);       // every MMA thread, after storing its fragment
+    mbar_init(tempty_bar, (uint32_t)EW);   // one arrival per epilogue warp
     fence_mbar_init();
     tma_prefetch_desc(&tmapB);
     if (A_TMA) tma_prefetch_desc(&tmapA);
     if (!p.out_fp32) tma_prefetch_desc(&tmapC);
   }
-  if (warp == MMA_WARP) {
-    tmem_alloc(tmem_slot, 2 * BN);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < EW) {
     // ======================= epilogue =====================================================
-    // Per 32-column chunk: TMEM -> registers -> (bias / residual / ReLU) -> bf16 -> this warp's swizzled smem
+    // Per 32-column chunk: shared-memory accumulator tile -> registers -> (bias / residual / ReLU) -> bf16 -> this warp's swizzled smem
     // staging -> TMA store (no LSU global stores).  While the TMA engine reads the staging tile, the warp sums its
     // 32 rows per column from the same tile for the fused BatchNorm statistics (packed fp32x2 arithmetic on two
     // columns per lane); the sums stay in registers across all tiles of this CTA that share a column block.
     const bool do_stats = p.col_sum != nullptr;
-    const int quarter = warp & 3;                 // TMEM lane quarter = tile rows 32*quarter ..
+    const int quarter = warp & 3;                 // tile rows 32*quarter ..
     const int col_w0 = (warp >> 2) * (CPW * 32);  // first tile column of this warp
     const uint32_t stage_base0 = smem_u32(stage_out + warp * L::STAGE_PER_WARP);
     int sbuf = 0;
@@ -197,10 +190,10 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         const int col = stat_n0 + col_w0 + i * 32 + 2 * (lane & 15);
         const bool owner = lane < 16;
         if (owner && col < p.Ndim) {   // Ndim is a multiple of 8: col + 1 is valid too
-          atomicAdd(p.col_sum + col, a.x);
-          atomicAdd(p.col_sum + col + 1, a.y);
-          atomicAdd(p.col_sqsum + col, b.x);
-          atomicAdd(p.col_sqsum + col + 1, b.y);
+          fix_add(p.fx + col, a.x);
+          fix_add(p.fx + col + 1, a.y);
+          fix_add(p.fx + p.Ndim + col, b.x);
+          fix_add(p.fx + p.Ndim + col + 1, b.y);
         }
         cs1[i] = 0ull; cs2[i] = 0ull;
       }
@@ -213,9 +206,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         if (stat_n0 >= 0) flush_stats();
         stat_n0 = n0;
       }
-      const int acc = local & 1;
-      mbar_wait(&tfull_bar[acc], (uint32_t)((local >> 1) & 1));
-      tc_fence_after_sync();
+      mbar_wait(tfull_bar, (uint32_t)(local & 1));
       const int mrow0 = m0 + quarter * 32;
       int m = mrow0 + lane;
       const bool mvalid = m < p.M;
@@ -246,13 +237,11 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       for (int cl = 0; cl < CPW; ++cl) {
         const int c0 = col_w0 + cl * 32;
         uint32_t r[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BN + c0), r);
-        tmem_ld_wait();
+        acc_load_row32(accbuf + (quarter * 32 + lane) * L::ACC_LD + c0, r);
         if (cl == CPW - 1) {
-          // last TMEM read of this tile: hand the accumulator stage back to the MMA warp
-          tc_fence_before_sync();
+          // last read of this tile: hand the accumulator tile back to the MMA warpgroups
           __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty_bar[acc]);
+          if (lane == 0) mbar_arrive(tempty_bar);
         }
         const int nbase = n0 + c0;
         if (nbase >= p.Ndim) continue;  // warp-uniform
@@ -563,37 +552,40 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     cp_async_wait<0>();
     fence_proxy_async_smem();
     for (int j = (it > GATHER_LAG ? it - GATHER_LAG : 0); j < it; ++j) mbar_arrive(&full_bar[j % STAGES]);
-  } else if (warp == MMA_WARP) {
-    // ======================= MMA issuer ===================================================
-    // whole warp, warp-uniform operands, one elected lane issues (umma_*_elect, common.cuh)
-    {
-      constexpr uint32_t idesc = make_idesc(1u, BM, BN, 0u, 0u);
-      int it = 0, local = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-        const int acc = local & 1;
-        const int nkb_tile = tile_info(p, tile, BN).nkb;
-        mbar_wait(&tempty_bar[acc], (uint32_t)(((local >> 1) & 1) ^ 1));
-        tc_fence_after_sync();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = 0; kb < nkb_tile; ++kb, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after_sync();
-          const uint64_t adesc = make_smem_desc_sw128(smem_u32(smemA + s * A_STAGE_BYTES), 16, 1024);
-          const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smemB + s * L::B_STAGE_BYTES), 16, 1024);
+  } else if (warp >= MMA_WARP && warp < TMA_WARP) {
+    // ======================= MMA warpgroups ===============================================
+    // warpgroup wg multiplies tile rows 64*wg .. +63 (A rows 8 KB further into the stage) with the whole B tile
+    const int wg = (warp - MMA_WARP) >> 2;
+    const bool leader = (threadIdx.x & 127) == 0;
+    float d[BN / 2];
+    int it = 0, local = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
+      const int nkb_tile = tile_info(p, tile, BN).nkb;
+      int prev_s = -1;
+      for (int kb = 0; kb < nkb_tile; ++kb, ++it) {
+        const int s = it % STAGES;
+        const uint32_t ph = (it / STAGES) & 1;
+        mbar_wait(&full_bar[s], ph);
+        const uint64_t adesc = make_smem_desc_sw128(smem_u32(smemA + s * A_STAGE_BYTES + wg * 8192), 16, 1024);
+        const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smemB + s * L::B_STAGE_BYTES), 16, 1024);
+        wg_fence();
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            // advance 16 bf16 = 32 bytes along K inside the swizzle row: +2 in the (addr >> 4) field
-            umma_bf16_elect(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc,
-                      (uint32_t)((kb | k) != 0));
-          }
-          umma_commit_elect(&empty_bar[s]);
+        for (int k = 0; k < BK / 16; ++k) {
+          // advance 16 bf16 = 32 bytes along K inside the swizzle row: +2 in the (addr >> 4) field
+          wgmma_bf16<BN, 0, 0>(d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)((kb | k) != 0));
         }
-        umma_commit_elect(&tfull_bar[acc]);
+        wg_commit();
+        wg_wait<1>();   // the previous k-block's MMAs are done: release its stage
+        if (leader && prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
+        prev_s = s;
       }
+      wg_wait<0>();
+      wg_fence_acc(d);
+      if (leader && prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
+      mbar_wait(tempty_bar, (uint32_t)((local & 1) ^ 1));
+      acc_store_smem<BN>(accbuf, L::ACC_LD, wg * 64, 0, d);
+      mbar_arrive(tfull_bar);
     }
-    __syncwarp();
   } else if (warp == TMA_WARP) {
     // ======================= TMA producer =================================================
     if (lane == 0) {
@@ -622,21 +614,16 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     }
     __syncwarp();
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 2 * BN);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------
 // wgrad kernel:  dW[co, tap, ci] += sum over pixels of dY[m, co] * src[pix(m, tap), ci]
 //   A = dY  (MN-major: smem rows are pixels, 64-channel chunks along M)   via TMA
 //   B = src (MN-major: smem rows are pixels, 64-channel chunks along N)   via TMA (plain GEMM) or gather
-//   D[co 128][ci BN] accumulated in TMEM over this CTA's pixel range, then atomically added to the
-//   fp32 gradient in the reference's [Cout][Cin][KH][KW] parameter layout.
+//   D[co 128][ci BN] accumulated in registers of two MMA warpgroups (co rows 0-63 / 64-127) over this CTA's pixel
+//   range, then atomically added from the registers to the fp32 gradient in the reference's [Cout][Cin][KH][KW]
+//   parameter layout.
+//   warps 0-3: B gather (when B is not loaded by TMA), warps 4-11: MMA warpgroups, warp 12: TMA producer.
 // ---------------------------------------------------------------------------------------------
 struct WgradParams {
   const bf16* src;   // NHWC [Nimg, Hs, Ws, C] forward input of the conv
@@ -652,8 +639,8 @@ struct WgradParams {
   int Cg;            // channels per column group: C, or 64 in folded (stem) mode
   int groups;        // number of column groups: KH*KW taps, or KH in folded mode
   int fold_kw;       // 1: C == 8 and the KW taps are folded into the 64-wide column group: column = kw*8 + c
-  int vec4;          // 1: 1x1 conv with 16-byte aligned gradient rows: accumulate with red.global.add.v4.f32
   int small_src;     // 1: 32-bit element offsets are safe
+  Fix128* fx;     // fixed-point accumulators over the whole dw (fix_scratch), flushed into dw after the kernel
 };
 
 static constexpr int WG_KROWS = 64;  // pixels per k-block
@@ -661,8 +648,10 @@ static constexpr int WG_A_STAGE = 2 * WG_KROWS * 128;  // two 64-channel chunks 
 
 // The GEMM N dimension is the concatenation of all taps: column = group*Cg + c (group = tap), tiled by BN, so a
 // CTA whose BN spans several taps re-uses its dY tile (A operand) for all of them.
+static constexpr int WG_THREADS = 13 * 32;
+
 template <int BN, int STAGES, bool B_TMA>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(WG_THREADS, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB,
                   const WgradParams p) {
   constexpr int NCH = BN / 64;                       // 64-channel chunks along N
@@ -673,8 +662,6 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   uint8_t* smemB = smem + STAGES * WG_A_STAGE;
   uint64_t* full_bar = (uint64_t*)(smemB + STAGES * B_STAGE);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* accum_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = (uint32_t*)(accum_bar + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -690,24 +677,16 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   const int nkb = kb_end - kb_begin;   // host guarantees nkb >= 1
   const int taps = p.KH * p.KW;
 
-  if (warp == 5 && lane == 0) {
+  if (warp == 12 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], B_TMA ? 1u : 129u);
-      mbar_init(&empty_bar[s], 1u);
+      mbar_init(&empty_bar[s], 2u);   // one arrival per MMA warpgroup
     }
-    mbar_init(accum_bar, 1u);
     fence_mbar_init();
     tma_prefetch_desc(&tmapA);
     if (B_TMA) tma_prefetch_desc(&tmapB);
   }
-  if (warp == 4) {
-    tmem_alloc(tmem_slot, BN < 32 ? 32 : BN);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < 4) {
     if (!B_TMA) {
@@ -770,72 +749,63 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       fence_proxy_async_smem();
       for (int it = (nkb > GATHER_LAG ? nkb - GATHER_LAG : 0); it < nkb; ++it) mbar_arrive(&full_bar[it % STAGES]);
     }
-    // ---------------- epilogue: TMEM -> L2 reductions into the fp32 gradient ----------------
-    mbar_wait(accum_bar, 0);
-    tc_fence_after_sync();
-    const int co = co0 + warp * 32 + lane;
-    const bool covalid = co < p.Cout;
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-      uint32_t r[32];
-      tmem_ld_32x32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, r);
-      tmem_ld_wait();
-      const int colb = n0 + c0;                // 32 columns never straddle a group (Cg is a multiple of 64)
-      const int group = colb / p.Cg;
-      const int cw0 = colb - group * p.Cg;
-      if (!covalid || group >= p.groups) continue;
-      if (p.fold_kw) {
-        // column = kw*8 + ci ; the group index is kh
-        float* gp = p.dw + ((int64_t)co * p.Cin_real) * taps + group * p.KW;
+  } else if (warp < 12) {
+    // ======================= MMA warpgroups (co rows 64*wg .. +63) ========================
+    const int wg = (warp - 4) >> 2;
+    const bool leader = (threadIdx.x & 127) == 0;
+    float d[BN / 2];
+    int prev_s = -1;
+    for (int it = 0; it < nkb; ++it) {
+      const int s = it % STAGES;
+      const uint32_t ph = (it / STAGES) & 1;
+      mbar_wait(&full_bar[s], ph);
+      // MN-major SW128: LBO = stride between 64-element MN chunks, SBO = stride between 8-row K groups; this
+      // warpgroup's 64 co are the A chunk wg
+      const uint64_t adesc =
+          make_smem_desc_sw128(smem_u32(smemA + s * WG_A_STAGE + wg * WG_KROWS * 128), WG_KROWS * 128, 1024);
+      const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smemB + s * B_STAGE), WG_KROWS * 128, 1024);
+      wg_fence();
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int cwj = cw0 + j, kwj = cwj >> 3, cj = cwj & 7;
-          if (kwj < p.KW && cj < p.Cin_real) atomicAdd(gp + (int64_t)cj * taps + kwj, __uint_as_float(r[j]));
-        }
-      } else if (p.vec4) {
-        // 1x1: the 32 columns are contiguous in memory -> 8 vector reductions instead of 32 scalar ones
-        float* gp = p.dw + (int64_t)co * p.Cin_real + cw0;
+      for (int k = 0; k < WG_KROWS / 16; ++k) {
+        // advance 16 pixel rows = 2048 bytes: +128 in the (addr >> 4) field
+        wgmma_bf16<BN, 1, 1>(d, adesc + (uint64_t)(128 * k), bdesc + (uint64_t)(128 * k), (uint32_t)((it | k) != 0));
+      }
+      wg_commit();
+      wg_wait<1>();
+      if (leader && prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
+      prev_s = s;
+    }
+    wg_wait<0>();
+    wg_fence_acc(d);
+    // ---------------- epilogue: registers -> L2 reductions into the fp32 gradient ----------------
+    const int t = threadIdx.x & 127;
+    const int r0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
+    auto add = [&](const float* q, float v) { fix_add(p.fx + (q - p.dw), v); };
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          if (cw0 + j < p.Cin_real)
-            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(gp + j), "f"(__uint_as_float(r[j])),
-                         "f"(__uint_as_float(r[j + 1])), "f"(__uint_as_float(r[j + 2])),
-                         "f"(__uint_as_float(r[j + 3]))
-                         : "memory");
-        }
-      } else {
-        float* gp = p.dw + ((int64_t)co * p.Cin_real) * taps + group;
+    for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int ci = cw0 + j;
-          if (ci < p.Cin_real) atomicAdd(gp + (int64_t)ci * taps, __uint_as_float(r[j]));
+      for (int h = 0; h < 2; ++h) {
+        const int co = co0 + r0 + 8 * h;
+        const int colb = n0 + 8 * j + 2 * (t & 3);   // columns colb, colb + 1 lie in one group (Cg % 8 == 0)
+        const int group = colb / p.Cg;
+        const int cw = colb - group * p.Cg;
+        const float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
+        if (co >= p.Cout || group >= p.groups) continue;
+        if (p.fold_kw) {
+          // column = kw*8 + ci ; the group index is kh
+          float* gp = p.dw + ((int64_t)co * p.Cin_real) * taps + group * p.KW;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int kwj = (cw + e) >> 3, cj = (cw + e) & 7;
+            if (kwj < p.KW && cj < p.Cin_real) add(gp + (int64_t)cj * taps + kwj, e ? v1 : v0);
+          }
+        } else {
+          float* gp = p.dw + ((int64_t)co * p.Cin_real) * taps + group;
+          if (cw < p.Cin_real) add(gp + (int64_t)cw * taps, v0);
+          if (cw + 1 < p.Cin_real) add(gp + (int64_t)(cw + 1) * taps, v1);
         }
       }
     }
-    tc_fence_before_sync();
-  } else if (warp == 4) {
-    // whole warp, warp-uniform operands, one elected lane issues (umma_*_elect, common.cuh)
-    {
-      constexpr uint32_t idesc = make_idesc(1u, 128, BN, 1u, 1u);  // both operands MN-major
-      for (int it = 0; it < nkb; ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after_sync();
-        // MN-major SW128: LBO = stride between 64-element MN chunks, SBO = stride between 8-row K groups
-        const uint64_t adesc = make_smem_desc_sw128(smem_u32(smemA + s * WG_A_STAGE), WG_KROWS * 128, 1024);
-        const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smemB + s * B_STAGE), WG_KROWS * 128, 1024);
-#pragma unroll
-        for (int k = 0; k < WG_KROWS / 16; ++k) {
-          // advance 16 pixel rows = 2048 bytes: +128 in the (addr >> 4) field
-          umma_bf16_elect(tmem_base, adesc + (uint64_t)(128 * k), bdesc + (uint64_t)(128 * k), idesc,
-                    (uint32_t)((it | k) != 0));
-        }
-        umma_commit_elect(&empty_bar[s]);
-      }
-      umma_commit_elect(accum_bar);
-    }
-    __syncwarp();
   } else {
     if (lane == 0) {
       constexpr uint32_t tx = (uint32_t)WG_A_STAGE + (B_TMA ? (uint32_t)B_STAGE : 0u);
@@ -857,11 +827,6 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       }
     }
     __syncwarp();
-  }
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, BN < 32 ? 32 : BN);
   }
 }
 
@@ -945,9 +910,9 @@ static int launch_igemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUte
     attr_set[dev_slot] = true;
   }
   const int num_tiles = tiles_m * p.tiles_n;
-  int grid = 2 * sm_count();           // persistent: two CTAs per SM (smem and TMEM sized for it)
+  int grid = sm_count();               // persistent: one CTA per SM (shared memory sized for it)
   if (grid > num_tiles) grid = num_tiles;
-  kern<<<grid, 320, L::TOTAL, stream>>>(ta, tb, tc, p, num_tiles);
+  kern<<<grid, IG_THREADS, L::TOTAL, stream>>>(ta, tb, tc, p, num_tiles);
   return check_launch("conv_igemm_kernel");
 }
 
@@ -970,6 +935,7 @@ extern "C" int byol_conv_igemm(const void* src, const void* wt, void* dst, const
                  "byol_conv_igemm: Ndim=%d must be a multiple of 8 (any width only for plain fp32 outputs)", Ndim);
   BYOL_CHECK_ARG(ldc >= Ndim && (ldc % 8 == 0 || out_fp32), "byol_conv_igemm: bad ldc=%d", ldc);
   BYOL_CHECK_ARG(!(out_fp32 && col_sum != nullptr), "byol_conv_igemm: fused statistics need a bf16 output");
+  BYOL_CHECK_ARG((col_sum == nullptr) == (col_sqsum == nullptr), "byol_conv_igemm: need both statistics or none");
   BYOL_CHECK_ARG(stride == 1 || stride == 2, "byol_conv_igemm: stride %d unsupported", stride);
   BYOL_CHECK_ARG(mode == 0 || mode == 1, "byol_conv_igemm: bad mode %d", mode);
   const int64_t M64 = (int64_t)Nimg * Ho * Wo;
@@ -1052,12 +1018,21 @@ extern "C" int byol_conv_igemm(const void* src, const void* wt, void* dst, const
   } else {
     ta = tb;
   }
-  if (BN == 128) {
-    return a_tma ? launch_igemm<128, 3, true>(ta, tb, tc, p, tiles_m, stream)
-                 : launch_igemm<128, 3, false>(ta, tb, tc, p, tiles_m, stream);
+  if (col_sum != nullptr) {
+    p.fx = fix_scratch(stream, 2 * (int64_t)Ndim);
+    if (p.fx == nullptr) return -2;
   }
-  return a_tma ? launch_igemm<64, 3, true>(ta, tb, tc, p, tiles_m, stream)
+  int rc;
+  if (BN == 128) {
+    rc = a_tma ? launch_igemm<128, 3, true>(ta, tb, tc, p, tiles_m, stream)
+               : launch_igemm<128, 3, false>(ta, tb, tc, p, tiles_m, stream);
+  } else {
+    rc = a_tma ? launch_igemm<64, 3, true>(ta, tb, tc, p, tiles_m, stream)
                : launch_igemm<64, 4, false>(ta, tb, tc, p, tiles_m, stream);
+  }
+  if (rc != 0 || col_sum == nullptr) return rc;
+  if ((rc = fix_flush(p.fx, col_sum, Ndim, stream)) != 0) return rc;
+  return fix_done(stream, fix_flush(p.fx + Ndim, col_sqsum, Ndim, stream));
 }
 
 template <int BN, bool B_TMA>
@@ -1076,7 +1051,7 @@ static int launch_wgrad(const CUtensorMap& ta, const CUtensorMap& tb, const Wgra
     }
     attr_set[dev_slot] = true;
   }
-  kern<<<grid, 192, SMEM, stream>>>(ta, tb, p);
+  kern<<<grid, WG_THREADS, SMEM, stream>>>(ta, tb, p);
   return check_launch("conv_wgrad_kernel");
 }
 
@@ -1110,18 +1085,18 @@ extern "C" int byol_conv_wgrad(const void* src, const void* dy, float* dw, int N
   p.Cg = p.fold_kw ? 64 : C;
   p.groups = p.fold_kw ? KH : KH * KW;
   const int ncols = p.groups * p.Cg;                       // concatenated (tap, channel) columns
-  const int BN = ncols > 128 ? 256 : (ncols > 64 ? 128 : 64);
+  // (a 128 x 256 tile would need 128 accumulator registers per MMA thread: more than the register file leaves)
+  const int BN = ncols > 64 ? 128 : 64;
   p.tiles_co = (Cout + 127) / 128;
   p.tiles_n = (ncols + BN - 1) / BN;
   p.num_kb_total = (p.M + WG_KROWS - 1) / WG_KROWS;
   p.small_src = ((int64_t)Nimg * Hs * Ws * C < (1ll << 31) - (1ll << 24)) ? 1 : 0;
   const int taps = KH * KW;
   const int base_ctas = p.tiles_co * p.tiles_n;
-  // The epilogue adds 128 x BN fp32 values per CTA to the gradient with L2 reductions, so the split count trades
-  // parallelism against reduction traffic: exactly one resident wave (2 CTAs/SM fit only for BN = 64), rounded
-  // DOWN so that no second, nearly empty wave appears.
-  p.vec4 = (taps == 1 && !p.fold_kw && Cin_real % 4 == 0 && ((uintptr_t)dw % 16 == 0)) ? 1 : 0;
-  const int target_ctas = sm_count() * (BN == 64 ? 2 : 1);
+  // The epilogue adds 128 x BN values per CTA to the gradient with L2 reductions, so the split count trades
+  // parallelism against reduction traffic: exactly one resident wave (one CTA per SM), rounded DOWN so that no
+  // second, nearly empty wave appears.
+  const int target_ctas = sm_count();
   int splits = target_ctas / base_ctas;
   int max_splits = (p.num_kb_total + 7) / 8;                // at least 8 k-blocks (512 pixels) per CTA
   if (max_splits < 1) max_splits = 1;
@@ -1140,9 +1115,10 @@ extern "C" int byol_conv_wgrad(const void* src, const void* dy, float* dw, int N
   } else {
     tb = ta;
   }
-  switch (BN) {
-    case 256: return b_tma ? launch_wgrad<256, true>(ta, tb, p, grid, stream) : launch_wgrad<256, false>(ta, tb, p, grid, stream);
-    case 128: return b_tma ? launch_wgrad<128, true>(ta, tb, p, grid, stream) : launch_wgrad<128, false>(ta, tb, p, grid, stream);
-    default:  return b_tma ? launch_wgrad<64, true>(ta, tb, p, grid, stream) : launch_wgrad<64, false>(ta, tb, p, grid, stream);
-  }
+  const int64_t ndw = (int64_t)Cout * Cin_real * taps;
+  p.fx = fix_scratch(stream, ndw);
+  if (p.fx == nullptr) return -2;
+  const int rc = BN == 128 ? (b_tma ? launch_wgrad<128, true>(ta, tb, p, grid, stream) : launch_wgrad<128, false>(ta, tb, p, grid, stream))
+                           : (b_tma ? launch_wgrad<64, true>(ta, tb, p, grid, stream) : launch_wgrad<64, false>(ta, tb, p, grid, stream));
+  return fix_done(stream, rc != 0 ? rc : fix_flush(p.fx, dw, ndw, stream));
 }

@@ -5,14 +5,15 @@
 // halo patch [(TH+2) rows][W+2 cols][64 ch] of the input (4-D tensor map; the zero padding is TMA out-of-bounds
 // fill) into a 128B-swizzled smem image with one 128-byte row per pixel.  With the GEMM rows enumerated as
 // m = orow*(W+2) + ocol (two "garbage" columns per image row, discarded in the epilogue), the A operand of tap
-// (kh, kw) is the SAME smem image shifted by (kh*(W+2) + kw) rows: the UMMA shared-memory descriptor simply starts
+// (kh, kw) is the SAME smem image shifted by (kh*(W+2) + kw) rows: the wgmma shared-memory descriptor simply starts
 // (kh*(W+2)+kw)*128 bytes later.  The 128-byte swizzle is a function of the smem address bits only, so a start
-// address that is 128-byte (not 1024-byte) aligned works with base_offset = 0 (verified on B200 by
-// tools/experiments/shift_test.cu).  Operand traffic from L2 drops from 9x to (TH+2)/TH x the input.
+// address that is 128-byte (not 1024-byte) aligned works with base_offset = 0.  Operand traffic from L2 drops from
+// 9x to (TH+2)/TH x the input.
 //
-//   warps 0-3 : epilogue (TMEM -> regs -> bf16 -> global; fused BN column statistics through a smem staging tile)
-//   warp 4    : MMA issuer (tcgen05.mma, two TMEM accumulator stages)
-//   warp 5    : TMA producer (patch ring + weight-tile ring)
+//   warps 0-3  : epilogue (smem accumulator tile -> regs -> bf16 -> global; fused BN column statistics through a
+//                smem staging tile)
+//   warps 4-11 : two MMA warpgroups (tile rows 0-63 / 64-127, accumulators of both M-tiles of a pair in registers)
+//   warp 12    : TMA producer (patch ring + weight-tile ring)
 // Replaces the cuDNN 3x3 conv fwd / dgrad calls reached from /root/reference/main.py:237 and main.py:617.
 #include <string.h>
 
@@ -25,6 +26,7 @@ struct PatchParams {
   const bf16* resid;    // optional, same shape as dst
   float* col_sum;       // optional [Ndim]
   float* col_sqsum;
+  Fix128* fx;        // with col_sum: [2][Ndim] fixed-point accumulators (fix_scratch)
   int Nimg, H, W, C;    // input == output spatial size (stride 1, pad 1)
   int Ndim, ldc;
   int Wp, TH, HB;       // W + 2, output rows per tile, tiles per image = ceil(H / TH)
@@ -38,7 +40,9 @@ struct PatchParams {
 
 static constexpr int P_PATCH_SLOT = 32768;   // bytes per patch slot (>= 128 * (128 + 2*Wp + 2))
 static constexpr int P_PSTAGES = 2;          // patch GROUP stages; a group = the patches of the (up to) 2 M-tiles of a pair
-static constexpr int P_BSTAGES = 4;
+static constexpr int P_BSTAGES = 2;
+static constexpr int P_THREADS = 13 * 32;
+static constexpr int P_ACC_LD = acc_ld(128);   // accumulator tile: [128 rows][2 M-tiles x 64 columns] fp32
 
 __device__ __forceinline__ void tma_load_4d(uint32_t dst_smem, const CUtensorMap* tmap, uint64_t* bar, int c0, int c1,
                                             int c2, int c3) {
@@ -49,14 +53,16 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst_smem, const CUtensorMap
 }
 
 template <int BN>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(P_THREADS, 1)
 conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_constant__ CUtensorMap tmapB,
                      const PatchParams p) {
   constexpr int B_STAGE = BN * 128;
   constexpr int PATCH_OFF = 0;
   constexpr int B_OFF = P_PSTAGES * 2 * P_PATCH_SLOT;
   constexpr int STAGE_OUT_OFF = B_OFF + P_BSTAGES * B_STAGE;   // 4 warps x [32 rows][64 B]
-  constexpr int BAR_OFF = STAGE_OUT_OFF + 4 * 2048;
+  constexpr int ACC_OFF = STAGE_OUT_OFF + 4 * 2048;
+  constexpr int BAR_OFF = ACC_OFF + 128 * P_ACC_LD * 4;
+  static_assert(2 * BN <= 128, "the accumulator tile holds two 64-column M-tiles");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* smemP = smem + PATCH_OFF;
@@ -66,29 +72,23 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
   uint64_t* pempty = pfull + P_PSTAGES;
   uint64_t* bfull = pempty + P_PSTAGES;
   uint64_t* bempty = bfull + P_BSTAGES;
-  uint64_t* tfull = bempty + P_BSTAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = (uint32_t*)(tempty + 2);
+  uint64_t* tfull = bempty + P_BSTAGES;   // accumulator tile ready for the epilogue
+  uint64_t* tempty = tfull + 1;           // accumulator tile drained
+  float* accbuf = reinterpret_cast<float*>(smem + ACC_OFF);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == 5 && lane == 0) {
-    for (int s = 0; s < P_PSTAGES; ++s) { mbar_init(&pfull[s], 1u); mbar_init(&pempty[s], 1u); }
-    for (int s = 0; s < P_BSTAGES; ++s) { mbar_init(&bfull[s], 1u); mbar_init(&bempty[s], 1u); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&tfull[a], 1u); mbar_init(&tempty[a], 4u); }
+  if (warp == 12 && lane == 0) {
+    for (int s = 0; s < P_PSTAGES; ++s) { mbar_init(&pfull[s], 1u); mbar_init(&pempty[s], 2u); }
+    for (int s = 0; s < P_BSTAGES; ++s) { mbar_init(&bfull[s], 1u); mbar_init(&bempty[s], 2u); }
+    mbar_init(tfull, 256u);
+    mbar_init(tempty, 4u);
     fence_mbar_init();
     tma_prefetch_desc(&tmapX);
     tma_prefetch_desc(&tmapB);
   }
-  if (warp == 4) {
-    tmem_alloc(tmem_slot, 4 * BN);     // 2 accumulator stages x 2 M-tiles of a pair
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < 4) {
     // ======================= epilogue =====================================================
@@ -109,17 +109,15 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
 #pragma unroll
           for (int i = 0; i < BN / 32; ++i) {
             if (stat_n0 + i * 32 + lane < p.Ndim) {
-              atomicAdd(p.col_sum + stat_n0 + i * 32 + lane, csum[i]);
-              atomicAdd(p.col_sqsum + stat_n0 + i * 32 + lane, csq[i]);
+              fix_add(p.fx + stat_n0 + i * 32 + lane, csum[i]);
+              fix_add(p.fx + p.Ndim + stat_n0 + i * 32 + lane, csq[i]);
             }
             csum[i] = 0.f; csq[i] = 0.f;
           }
         }
         stat_n0 = n0;
       }
-      const int acc = local & 1;
-      mbar_wait(&tfull[acc], (uint32_t)((local >> 1) & 1));
-      tc_fence_after_sync();
+      mbar_wait(tfull, (uint32_t)(local & 1));
       for (int jp = 0; jp < npair; ++jp) {
       const int mt = mt0 + jp;
       const int n = mt / p.HB;
@@ -135,12 +133,10 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
       for (int ci = 0; ci < BN / 32; ++ci) {
         const int c0 = ci * 32;
         uint32_t r[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)((acc * 2 + jp) * BN + c0), r);
-        tmem_ld_wait();
+        acc_load_row32(accbuf + (warp * 32 + lane) * P_ACC_LD + jp * BN + c0, r);
         if (ci == BN / 32 - 1 && jp == npair - 1) {
-          tc_fence_before_sync();
           __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty[acc]);
+          if (lane == 0) mbar_arrive(tempty);
         }
         const int nbase = n0 + c0;
         if (nbase >= p.Ndim) continue;  // warp-uniform
@@ -216,53 +212,63 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
 #pragma unroll
       for (int i = 0; i < BN / 32; ++i) {
         if (stat_n0 + i * 32 + lane < p.Ndim) {
-          atomicAdd(p.col_sum + stat_n0 + i * 32 + lane, csum[i]);
-          atomicAdd(p.col_sqsum + stat_n0 + i * 32 + lane, csq[i]);
+          fix_add(p.fx + stat_n0 + i * 32 + lane, csum[i]);
+          fix_add(p.fx + p.Ndim + stat_n0 + i * 32 + lane, csq[i]);
         }
       }
     }
-  } else if (warp == 4) {
-    // ======================= MMA issuer ===================================================
-    // whole warp, warp-uniform operands, one elected lane issues (umma_*_elect, common.cuh)
-    {
-      constexpr uint32_t idesc = make_idesc(1u, 128, BN, 0u, 0u);
-      int pit = 0, bit = 0, local = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++local) {
-        const int acc = local & 1;
-        const int mt0 = (tile / p.tiles_n) * 2;
-        const int npair = (mt0 + 1 < p.num_mt) ? 2 : 1;
-        mbar_wait(&tempty[acc], (uint32_t)(((local >> 1) & 1) ^ 1));
-        tc_fence_after_sync();
-        for (int cc = 0; cc < p.nchunks; ++cc, ++pit) {
-          const int ps = pit % P_PSTAGES;
-          mbar_wait(&pfull[ps], (uint32_t)((pit / P_PSTAGES) & 1));
-          const uint32_t patch = smem_u32(smemP + ps * 2 * P_PATCH_SLOT);
-          for (int tap = 0; tap < 9; ++tap, ++bit) {
-            const int bs = bit % P_BSTAGES;
-            mbar_wait(&bfull[bs], (uint32_t)((bit / P_BSTAGES) & 1));
-            tc_fence_after_sync();
-            const int kh = tap / 3, kw = tap - kh * 3;
-            const int shift = p.flip ? ((2 - kh) * p.Wp + (2 - kw)) : (kh * p.Wp + kw);
-            const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smemB + bs * B_STAGE), 16, 1024);
-            // the same weight tile multiplies the patches of both M-tiles of the pair
-            for (int jp = 0; jp < npair; ++jp) {
-              // shifted window over the swizzled patch image: start address only 128-byte aligned, base_offset 0
-              const uint64_t adesc =
-                  make_smem_desc_sw128(patch + (uint32_t)jp * P_PATCH_SLOT + (uint32_t)shift * 128u, 16, 1024);
-              const uint32_t tmem_d = tmem_base + (uint32_t)((acc * 2 + jp) * BN);
+  } else if (warp < 12) {
+    // ======================= MMA warpgroups ===============================================
+    // warpgroup wg: tile rows 64*wg .. +63 = the patch image 64 rows (8 KB) further on
+    const int wg = (warp - 4) >> 2;
+    const bool leader = (threadIdx.x & 127) == 0;
+    float d[2][BN / 2];
+    int pit = 0, bit = 0, local = 0;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++local) {
+      const int mt0 = (tile / p.tiles_n) * 2;
+      const int npair = (mt0 + 1 < p.num_mt) ? 2 : 1;
+      for (int cc = 0; cc < p.nchunks; ++cc, ++pit) {
+        const int ps = pit % P_PSTAGES;
+        mbar_wait(&pfull[ps], (uint32_t)((pit / P_PSTAGES) & 1));
+        const uint32_t patch = smem_u32(smemP + ps * 2 * P_PATCH_SLOT) + (uint32_t)wg * 8192u;
+        int prev_bs = -1;
+        for (int tap = 0; tap < 9; ++tap, ++bit) {
+          const int bs = bit % P_BSTAGES;
+          mbar_wait(&bfull[bs], (uint32_t)((bit / P_BSTAGES) & 1));
+          const int kh = tap / 3, kw = tap - kh * 3;
+          const int shift = p.flip ? ((2 - kh) * p.Wp + (2 - kw)) : (kh * p.Wp + kw);
+          const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smemB + bs * B_STAGE), 16, 1024);
+          wg_fence();
+          // the same weight tile multiplies the patches of both M-tiles of the pair.  Both are always issued (a branch
+          // around wgmma makes ptxas serialise every MMA); for a single-tile pair the second result is discarded.
 #pragma unroll
-              for (int k = 0; k < 4; ++k)
-                umma_bf16_elect(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc,
-                          (uint32_t)((cc | tap | k) != 0));
-            }
-            umma_commit_elect(&bempty[bs]);
+          for (int jp = 0; jp < 2; ++jp) {
+            // shifted window over the swizzled patch image: start address only 128-byte aligned, base_offset 0
+            const uint64_t adesc =
+                make_smem_desc_sw128(patch + (uint32_t)jp * P_PATCH_SLOT + (uint32_t)shift * 128u, 16, 1024);
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+              wgmma_bf16<BN, 0, 0>(d[jp], adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k),
+                                   (uint32_t)((cc | tap | k) != 0));
           }
-          umma_commit_elect(&pempty[ps]);
+          wg_commit();
+          wg_wait<1>();   // the previous tap's MMAs are done with their weight stage
+          if (leader && prev_bs >= 0) mbar_arrive(&bempty[prev_bs]);
+          prev_bs = bs;
         }
-        umma_commit_elect(&tfull[acc]);
+        wg_wait<0>();
+        if (leader) {
+          mbar_arrive(&bempty[prev_bs]);
+          mbar_arrive(&pempty[ps]);
+        }
       }
+      wg_fence_acc(d[0]);
+      wg_fence_acc(d[1]);
+      mbar_wait(tempty, (uint32_t)((local & 1) ^ 1));
+      acc_store_smem<BN>(accbuf, P_ACC_LD, wg * 64, 0, d[0]);
+      if (npair == 2) acc_store_smem<BN>(accbuf, P_ACC_LD, wg * 64, BN, d[1]);
+      mbar_arrive(tfull);
     }
-    __syncwarp();
   } else {
     // ======================= TMA producer =================================================
     // Flat loop over this CTA's (tile, channel-chunk) pairs.  The patch of the NEXT pair is requested while the
@@ -303,13 +309,6 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
     }
     __syncwarp();
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 4 * BN);
-  }
 }
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -332,7 +331,8 @@ static PFN_encodeTiled patch_encode_fn() {
 template <int BN>
 static int launch_patch(const CUtensorMap& tx, const CUtensorMap& tb, const PatchParams& p, int sms,
                         cudaStream_t stream) {
-  constexpr int SMEM = P_PSTAGES * 2 * P_PATCH_SLOT + P_BSTAGES * BN * 128 + 4 * 2048 + 256 + 1024;
+  constexpr int SMEM = P_PSTAGES * 2 * P_PATCH_SLOT + P_BSTAGES * BN * 128 + 4 * 2048 + 128 * P_ACC_LD * 4 + 256 + 1024;
+  static_assert(SMEM <= 232448, "conv3x3_patch_kernel: shared memory");
   auto kern = conv3x3_patch_kernel<BN>;
   static bool attr_set[kMaxDevices] = {};
   const int dev_slot = device_slot();
@@ -345,7 +345,7 @@ static int launch_patch(const CUtensorMap& tx, const CUtensorMap& tb, const Patc
     attr_set[dev_slot] = true;
   }
   int grid = sms < p.num_tiles ? sms : p.num_tiles;
-  kern<<<grid, 192, SMEM, stream>>>(tx, tb, p);
+  kern<<<grid, P_THREADS, SMEM, stream>>>(tx, tb, p);
   return check_launch("conv3x3_patch_kernel");
 }
 
@@ -355,8 +355,7 @@ bool patch_conv_applicable(int H, int W, int C, int Ndim, int KH, int KW, int st
   if (KH != 3 || KW != 3 || stride != 1 || pad != 1 || out_fp32 || bias != nullptr) return false;
   if (C % 64 != 0 || Ndim % 8 != 0) return false;
   const int Wp = W + 2;
-  // measured on B200 (512 images): faster than the gather kernel at 56x56 (1.4x) and 28x28, slower at 14x14 and
-  // below, where few of the 128 tile rows are valid and the gather kernel's two CTAs per SM hide more latency
+  // at 14x14 and below few of the 128 tile rows are valid: the gather kernel is used there
   if (Wp > 128 || W < 12) return false;
   const int TH = 128 / Wp;
   if (128 * (128 + 2 * Wp + 2) > P_PATCH_SLOT) return false;
@@ -379,7 +378,8 @@ int patch_conv_launch(const void* src, const void* wt, void* dst, const void* re
   p.TH = 128 / p.Wp;
   if (p.TH > H) p.TH = H;
   p.HB = (H + p.TH - 1) / p.TH;
-  const int BN = Ndim > 64 ? 128 : 64;
+  // 64 columns: the accumulators of both M-tiles of a pair (2 x 64 x BN per warpgroup) must fit in registers
+  const int BN = 64;
   p.tiles_n = (Ndim + BN - 1) / BN;
   p.num_mt = Nimg * p.HB;
   p.num_tiles = ((p.num_mt + 1) / 2) * p.tiles_n;
@@ -409,7 +409,14 @@ int patch_conv_launch(const void* src, const void* wt, void* dst, const void* re
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_last_error("patch conv: weight tensor map encode failed (%d)", (int)r); return -3; }
   }
-  return BN == 128 ? launch_patch<128>(tx, tb, p, sms, stream) : launch_patch<64>(tx, tb, p, sms, stream);
+  if (col_sum != nullptr) {
+    p.fx = fix_scratch(stream, 2 * (int64_t)Ndim);
+    if (p.fx == nullptr) return -2;
+  }
+  int rc = launch_patch<64>(tx, tb, p, sms, stream);
+  if (rc != 0 || col_sum == nullptr) return rc;
+  if ((rc = fix_flush(p.fx, col_sum, Ndim, stream)) != 0) return rc;
+  return fix_done(stream, fix_flush(p.fx + Ndim, col_sqsum, Ndim, stream));
 }
 
 }  // namespace byol
@@ -421,8 +428,9 @@ int patch_conv_launch(const void* src, const void* wt, void* dst, const void* re
 //   A = dY tile  [128 pixel rows][128 co]  MN-major, TMA box {64 co, W+2, TH, 1}: the two garbage columns and rows
 //       beyond the image are out-of-bounds -> ZERO, so garbage rows contribute nothing
 //   B = X patch  [(TH+2)*(W+2) pixel rows][64*NB ci] MN-major; tap (kh,kw) = the same image shifted by kh*(W+2)+kw rows
-//   D[128 co][kw*64*NB + ci] for the three taps of ONE kh row per CTA, accumulated in TMEM over the CTA's range of
-//   M-tiles, then added to the fp32 gradient with L2 reductions.
+//   D[128 co][kw*64*NB + ci] for the three taps of ONE kh row per CTA, accumulated in the registers of two MMA
+//   warpgroups (co rows 0-63 / 64-127; warps 0-7) over the CTA's range of M-tiles, then added to the fp32 gradient
+//   with L2 reductions.  Warp 8 is the TMA producer.
 // Rows of the smem slots that TMA never writes (beyond the boxes) are zeroed once, so stale shared memory can not
 // inject Inf/NaN through the zero rows of A.
 // =================================================================================================
@@ -430,6 +438,7 @@ namespace byol {
 
 struct WPatchParams {
   float* dw;            // [Cout][Cin][3][3] fp32
+  Fix128* fx;        // fixed-point accumulators over the whole dw (fix_scratch)
   int Nimg, H, W, C, Cout;
   int Wp, TH, HB, num_mt;
   int co_tiles, ci_groups;
@@ -440,24 +449,22 @@ struct WPatchParams {
 
 static constexpr int WP_STAGES = 2;
 
+static constexpr int WP_THREADS = 9 * 32;
+
 template <int NB>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(WP_THREADS, 1)
 conv3x3_wgrad_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_constant__ CUtensorMap tmapDY,
                            const WPatchParams p) {
   constexpr int X_STAGE = NB * P_PATCH_SLOT;
   constexpr int DY_STAGE = 2 * 16384;
   constexpr int DY_OFF = WP_STAGES * X_STAGE;
   constexpr int BAR_OFF = DY_OFF + WP_STAGES * DY_STAGE;
-  constexpr int NCOLS = 3 * 64 * NB;
-  constexpr int TMEM_COLS = NCOLS <= 256 ? 256 : 512;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* smemX = smem;
   uint8_t* smemDY = smem + DY_OFF;
   uint64_t* full_bar = (uint64_t*)(smem + BAR_OFF);
   uint64_t* empty_bar = full_bar + WP_STAGES;
-  uint64_t* accum_bar = empty_bar + WP_STAGES;
-  uint32_t* tmem_slot = (uint32_t*)(accum_bar + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -476,23 +483,15 @@ conv3x3_wgrad_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __gr
   // zero every operand slot once (see header comment)
   for (int i = threadIdx.x; i < BAR_OFF / 16; i += blockDim.x) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
   fence_proxy_async_smem();
-  if (warp == 5 && lane == 0) {
-    for (int s = 0; s < WP_STAGES; ++s) { mbar_init(&full_bar[s], 1u); mbar_init(&empty_bar[s], 1u); }
-    mbar_init(accum_bar, 1u);
+  if (warp == 8 && lane == 0) {
+    for (int s = 0; s < WP_STAGES; ++s) { mbar_init(&full_bar[s], 1u); mbar_init(&empty_bar[s], 2u); }
     fence_mbar_init();
     tma_prefetch_desc(&tmapX);
     tma_prefetch_desc(&tmapDY);
   }
-  if (warp == 4) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 5) {
+  if (warp == 8) {
     if (lane == 0) {
       for (int it = 0; it < ntiles; ++it) {
         const int mt = mt_begin + it;
@@ -510,57 +509,48 @@ conv3x3_wgrad_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __gr
       }
     }
     __syncwarp();
-  } else if (warp == 4) {
-    // whole warp, warp-uniform operands, one elected lane issues (umma_*_elect, common.cuh)
-    {
-      constexpr uint32_t idesc = make_idesc(1u, 128, 64 * NB, 1u, 1u);   // both operands MN-major
-      for (int it = 0; it < ntiles; ++it) {
-        const int s = it % WP_STAGES;
-        mbar_wait(&full_bar[s], (uint32_t)((it / WP_STAGES) & 1));
-        tc_fence_after_sync();
-        const uint32_t a_base = smem_u32(smemDY + s * DY_STAGE);
-        const uint32_t x_base = smem_u32(smemX + s * X_STAGE);
-#pragma unroll
-        for (int kw = 0; kw < 3; ++kw) {
-          const uint32_t shift = (uint32_t)(kh * p.Wp + kw) * 128u;
-          // A: 2 co chunks 16384 B apart; B: NB ci chunks P_PATCH_SLOT apart; 8-row groups 1024 B apart
-          const uint64_t adesc = make_smem_desc_sw128(a_base, 16384, 1024);
-          const uint64_t bdesc = make_smem_desc_sw128(x_base + shift, P_PATCH_SLOT, 1024);
-#pragma unroll
-          for (int k = 0; k < 8; ++k)   // 16 pixel rows = 2048 bytes per step
-            umma_bf16_elect(tmem_base + (uint32_t)(kw * 64 * NB), adesc + (uint64_t)(128 * k), bdesc + (uint64_t)(128 * k),
-                      idesc, (uint32_t)((it | k) != 0));
-        }
-        umma_commit_elect(&empty_bar[s]);
-      }
-      umma_commit_elect(accum_bar);
-    }
-    __syncwarp();
   } else {
-    // ---------------- epilogue: TMEM -> L2 reductions into dW[co][ci][kh][kw] ----------------
-    mbar_wait(accum_bar, 0);
-    tc_fence_after_sync();
-    const int co = co0 + warp * 32 + lane;
-    const bool covalid = co < p.Cout;
-#pragma unroll 1
-    for (int c0 = 0; c0 < NCOLS; c0 += 32) {
-      uint32_t r[32];
-      tmem_ld_32x32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, r);
-      tmem_ld_wait();
-      if (!covalid) continue;
-      const int kw = c0 / (64 * NB);
-      const int cib = ci0 + (c0 - kw * 64 * NB);
-      float* gp = p.dw + ((int64_t)co * p.C) * 9 + kh * 3 + kw;
+    const int wg = warp >> 2;
+    const bool leader = (threadIdx.x & 127) == 0;
+    float d[3][32 * NB];
+    int prev_s = -1;
+    for (int it = 0; it < ntiles; ++it) {
+      const int s = it % WP_STAGES;
+      mbar_wait(&full_bar[s], (uint32_t)((it / WP_STAGES) & 1));
+      const uint32_t a_base = smem_u32(smemDY + s * DY_STAGE) + (uint32_t)wg * 16384u;   // this warpgroup's 64 co
+      const uint32_t x_base = smem_u32(smemX + s * X_STAGE);
+      wg_fence();
 #pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (cib + j < p.C) atomicAdd(gp + (int64_t)(cib + j) * 9, __uint_as_float(r[j]));
+      for (int kw = 0; kw < 3; ++kw) {
+        const uint32_t shift = (uint32_t)(kh * p.Wp + kw) * 128u;
+        // A: co chunks 16384 B apart; B: NB ci chunks P_PATCH_SLOT apart; 8-row groups 1024 B apart
+        const uint64_t adesc = make_smem_desc_sw128(a_base, 16384, 1024);
+        const uint64_t bdesc = make_smem_desc_sw128(x_base + shift, P_PATCH_SLOT, 1024);
+#pragma unroll
+        for (int k = 0; k < 8; ++k)   // 16 pixel rows = 2048 bytes per step
+          wgmma_bf16<64 * NB, 1, 1>(d[kw], adesc + (uint64_t)(128 * k), bdesc + (uint64_t)(128 * k),
+                                    (uint32_t)((it | k) != 0));
+      }
+      wg_commit();
+      wg_wait<1>();
+      if (leader && prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
+      prev_s = s;
     }
-    tc_fence_before_sync();
-  }
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, TMEM_COLS);
+    wg_wait<0>();
+#pragma unroll
+    for (int kw = 0; kw < 3; ++kw) wg_fence_acc(d[kw]);
+    // ---------------- epilogue: registers -> L2 reductions into dW[co][ci][kh][kw] ----------------
+    const int t = threadIdx.x & 127;
+    const int r0 = co0 + wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
+#pragma unroll
+    for (int kw = 0; kw < 3; ++kw) {
+#pragma unroll
+      for (int i = 0; i < 32 * NB; ++i) {
+        const int co = r0 + ((i & 2) ? 8 : 0);
+        const int ci = ci0 + 8 * (i >> 2) + 2 * (t & 3) + (i & 1);
+        if (co < p.Cout && ci < p.C) fix_add(p.fx + ((int64_t)co * p.C + ci) * 9 + kh * 3 + kw, d[kw][i]);
+      }
+    }
   }
 }
 
@@ -579,7 +569,7 @@ static int launch_wpatch(const CUtensorMap& tx, const CUtensorMap& ty, const WPa
     }
     attr_set[dev_slot] = true;
   }
-  kern<<<grid, 192, SMEM, stream>>>(tx, ty, p);
+  kern<<<grid, WP_THREADS, SMEM, stream>>>(tx, ty, p);
   return check_launch("conv3x3_wgrad_patch_kernel");
 }
 
@@ -606,7 +596,8 @@ int patch_wgrad_launch(const void* x, const void* dy, float* dw, int Nimg, int H
   if (p.TH > H) p.TH = H;
   p.HB = (H + p.TH - 1) / p.TH;
   p.num_mt = Nimg * p.HB;
-  const int NB = (C % 128 == 0) ? 2 : 1;
+  // one 64-channel chunk per CTA: 3 taps x 64 x 64 accumulators per warpgroup already take 96 registers per thread
+  constexpr int NB = 1;
   p.co_tiles = (Cout + 127) / 128;
   p.ci_groups = C / (64 * NB);
   const int base = p.co_tiles * p.ci_groups * 3;
@@ -630,7 +621,11 @@ int patch_wgrad_launch(const void* x, const void* dy, float* dw, int Nimg, int H
     if (r != CUDA_SUCCESS) { set_last_error("patch wgrad: tensor map encode failed (%d)", (int)r); return -3; }
   }
   const int grid = base * p.splits;
-  return NB == 2 ? launch_wpatch<2>(tx, ty, p, grid, stream) : launch_wpatch<1>(tx, ty, p, grid, stream);
+  const int64_t ndw = (int64_t)Cout * C * 9;
+  p.fx = fix_scratch(stream, ndw);
+  if (p.fx == nullptr) return -2;
+  const int rc = launch_wpatch<NB>(tx, ty, p, grid, stream);
+  return fix_done(stream, rc != 0 ? rc : fix_flush(p.fx, dw, ndw, stream));
 }
 
 }  // namespace byol

@@ -4,15 +4,16 @@
 // overlapping windows), which made the stem L2-bound at ~100 TFLOP/s.  Here the input is stored once as
 // NHWC4 bf16 with the zero padding baked in ([N][H+6][264][4], 8 bytes per pixel).  Because the stride is 2 and a
 // pixel is 8 bytes, the window of output pixel m along an input row starts 16 bytes after the window of pixel
-// m - 1 — exactly the row pitch of a no-swizzle UMMA core matrix.  So with LBO = 16 and SBO = 128 the shared-memory
-// matrix descriptor ALONE forms the im2col rows (rows and K chunks overlap in smem; verified exact on B200 by
-// tools/experiments/noswz_test.cu): an input row is bulk-copied into smem once and then read by the tensor core
-// for all 128 output pixels x 8 window taps, and a row pair is loaded once per CTA for the 3-4 output rows that
-// use it.  Per output row: 7 kernel rows x 2 MMAs (M = 128 pixels, N = 64 channels, K = 16 = 4 pixels x 4 ch).
+// m - 1 — exactly the row pitch of a no-swizzle core matrix.  So with LBO = 16 and SBO = 128 the wgmma shared-memory
+// matrix descriptor ALONE forms the im2col rows (rows and K chunks overlap in smem): an input row is bulk-copied
+// into smem once and then read by the tensor core for all 128 output pixels x 8 window taps, and a row pair is
+// loaded once per CTA for the 3-4 output rows that use it.  Per output row and warpgroup: 7 kernel rows x 2 MMAs
+// (M = 64 pixels, N = 64 channels, K = 16 = 4 pixels x 4 ch).
 //
-//   warps 0-7 : epilogue (TMEM -> regs -> bf16 -> swizzled staging -> TMA store, fused BatchNorm statistics)
-//   warp 8    : MMA issuer (four TMEM accumulator stages)
-//   warp 9    : producer (1-D bulk copies of input row pairs into an 8-slot ring; weights once)
+//   warps 0-7  : epilogue (smem accumulator tile -> regs -> bf16 -> swizzled staging -> TMA store, fused BatchNorm
+//                statistics)
+//   warps 8-15 : two MMA warpgroups (output pixels 0-63 / 64-127 of the row)
+//   warp 16    : producer (1-D bulk copies of input row pairs into an 8-slot ring; weights once)
 // Replaces the cuDNN stem convolution reached from /root/reference/main.py:237 (torchvision resnet conv1) and its
 // weight gradient under main.py:617.
 #include <stdlib.h>
@@ -26,27 +27,30 @@ static constexpr int ST_WP = 264;                    // padded pixels per input 
 static constexpr int ST_ROW_BYTES = ST_WP * 8;       // 2112
 static constexpr int ST_PAIR_BYTES = 2 * ST_ROW_BYTES;
 static constexpr int ST_NP = 8;                      // row-pair ring slots
-static constexpr int ST_NACC = 4;                    // TMEM accumulator stages (64 fp32 columns each)
 static constexpr int ST_W_BYTES = 7 * 4 * 64 * 16;   // [kh][k-chunk][cout][8] bf16 = 28672
 static constexpr int ST_W_OFF = 0;
 static constexpr int ST_RING_OFF = ST_W_BYTES;
 static constexpr int ST_STAGE_OFF = ((ST_RING_OFF + ST_NP * ST_PAIR_BYTES + 1023) / 1024) * 1024;
-static constexpr int ST_BAR_OFF = ST_STAGE_OFF + 8 * 2 * 2048;
+static constexpr int ST_ACC_LD = acc_ld(64);
+static constexpr int ST_ACC_OFF = ST_STAGE_OFF + 8 * 2 * 2048;    // [128][ST_ACC_LD] fp32 accumulator tile
+static constexpr int ST_BAR_OFF = ST_ACC_OFF + 128 * ST_ACC_LD * 4;
 static constexpr int ST_NEEDED = ST_BAR_OFF + 256;
 static constexpr int ST_TOTAL = ST_NEEDED + 768;
-static_assert(ST_TOTAL <= 115712, "two CTAs per SM");
+static constexpr int ST_THREADS = 17 * 32;
+static_assert(ST_TOTAL <= 232448, "one CTA per SM");
 
 struct StemParams {
   const bf16* xs;   // [N][H+6][264][4]
   const bf16* w;    // [7][4][64][8]
   float* col_sum;   // optional [64]
   float* col_sqsum;
+  Fix128* fx;    // with col_sum: [2][64] fixed-point accumulators (fix_scratch)
   int N, Ho, Wo;
   int pairs_per_img;   // (H + 6) / 2
   int num_tiles;       // N * Ho (one tile = one output row, Wo <= 128 pixels)
 };
 
-__global__ void __launch_bounds__(320, 2)
+__global__ void __launch_bounds__(ST_THREADS, 1)
 stem_fprop_kernel(const __grid_constant__ CUtensorMap tmapY, const StemParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -57,9 +61,9 @@ stem_fprop_kernel(const __grid_constant__ CUtensorMap tmapY, const StemParams p)
   uint64_t* wfull = (uint64_t*)(smem + ST_BAR_OFF);
   uint64_t* full_bar = wfull + 1;
   uint64_t* empty_bar = full_bar + ST_NP;
-  uint64_t* tfull_bar = empty_bar + ST_NP;
-  uint64_t* tempty_bar = tfull_bar + ST_NACC;
-  uint32_t* tmem_slot = (uint32_t*)(tempty_bar + ST_NACC);
+  uint64_t* tfull_bar = empty_bar + ST_NP;   // accumulator tile ready for the epilogue
+  uint64_t* tempty_bar = tfull_bar + 1;      // accumulator tile drained
+  float* accbuf = reinterpret_cast<float*>(smem + ST_ACC_OFF);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -67,21 +71,15 @@ stem_fprop_kernel(const __grid_constant__ CUtensorMap tmapY, const StemParams p)
   const int t_begin = (int)((int64_t)blockIdx.x * p.num_tiles / gridDim.x);
   const int t_end = (int)((int64_t)(blockIdx.x + 1) * p.num_tiles / gridDim.x);
 
-  if (warp == 9 && lane == 0) {
+  if (warp == 16 && lane == 0) {
     mbar_init(wfull, 1u);
-    for (int s = 0; s < ST_NP; ++s) { mbar_init(&full_bar[s], 1u); mbar_init(&empty_bar[s], 1u); }
-    for (int a = 0; a < ST_NACC; ++a) { mbar_init(&tfull_bar[a], 1u); mbar_init(&tempty_bar[a], 8u); }
+    for (int s = 0; s < ST_NP; ++s) { mbar_init(&full_bar[s], 1u); mbar_init(&empty_bar[s], 2u); }
+    mbar_init(tfull_bar, 256u);
+    mbar_init(tempty_bar, 8u);
     fence_mbar_init();
     tma_prefetch_desc(&tmapY);
   }
-  if (warp == 8) {
-    tmem_alloc(tmem_slot, ST_NACC * 64);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < 8) {
     // ======================= epilogue =====================================================
@@ -94,16 +92,17 @@ stem_fprop_kernel(const __grid_constant__ CUtensorMap tmapY, const StemParams p)
     uint64_t cs1 = 0ull, cs2 = 0ull;
     int sbuf = 0, local = 0;
     for (int t = t_begin; t < t_end; ++t, ++local) {
-      const int acc = local % ST_NACC;
-      mbar_wait(&tfull_bar[acc], (uint32_t)((local / ST_NACC) & 1));
-      tc_fence_after_sync();
+      mbar_wait(tfull_bar, (uint32_t)(local & 1));
       uint32_t r[32];
-      tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * 64 + c0), r);
-      tmem_ld_wait();
-      tc_fence_before_sync();
+      acc_load_row32(accbuf + (quarter * 32 + lane) * ST_ACC_LD + c0, r);
       __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
+      if (lane == 0) mbar_arrive(tempty_bar);
       if (rows_valid == 0) continue;   // warp-uniform
+      if (lane >= rows_valid) {
+        // pixels beyond Wo see windows over the right padding: non-zero garbage that must not reach the statistics
+#pragma unroll
+        for (int j = 0; j < 32; ++j) r[j] = 0u;
+      }
       const uint32_t stage_base = stage_base0 + (uint32_t)sbuf * 2048u;
       if (lane == 0) tma_store_wait_read1();
       __syncwarp();
@@ -136,67 +135,69 @@ stem_fprop_kernel(const __grid_constant__ CUtensorMap tmapY, const StemParams p)
       b.y += __shfl_xor_sync(0xffffffffu, b.y, 16);
       if (lane < 16) {
         const int col = c0 + 2 * lane;
-        atomicAdd(p.col_sum + col, a.x);
-        atomicAdd(p.col_sum + col + 1, a.y);
-        atomicAdd(p.col_sqsum + col, b.x);
-        atomicAdd(p.col_sqsum + col + 1, b.y);
+        fix_add(p.fx + col, a.x);
+        fix_add(p.fx + col + 1, a.y);
+        fix_add(p.fx + 64 + col, b.x);
+        fix_add(p.fx + 64 + col + 1, b.y);
       }
     }
     if (lane == 0) tma_store_wait_all();
-  } else if (warp == 8) {
-    // ======================= MMA issuer ===================================================
-    // the whole warp runs the loop (uniform control flow and operands); one elected lane issues (see common.cuh)
-    {
-      constexpr uint32_t idesc = make_idesc(1u, 128, 64, 0u, 0u);
-      mbar_wait(wfull, 0u);
-      tc_fence_after_sync();
-      const uint32_t w_addr = smem_u32(sW);
-      const uint32_t ring_addr = smem_u32(ring);
-      // B: [k-chunk][cout][8]: chunk step 1024, 8-row group step 128; kh block 4096 B, K step (2 chunks) 2048 B
-      const uint64_t bdesc0 = make_smem_desc_none(w_addr, 1024u, 128u);
-      int qb = 0, qn = 0, local = 0;
-      for (int t = t_begin; t < t_end; ++t, ++local) {
-        const int oh = t % p.Ho;
-        const bool first = (t == t_begin) || (oh == 0);
-        if (first) {
-          qb = qn;
-          qn += 4;
-          for (int j = 0; j < 4; ++j) mbar_wait(&full_bar[(qb + j) % ST_NP], (uint32_t)(((qb + j) / ST_NP) & 1));
-        } else {
-          qb += 1;
-          qn += 1;
-          mbar_wait(&full_bar[(qb + 3) % ST_NP], (uint32_t)(((qb + 3) / ST_NP) & 1));
-        }
-        const int acc = local % ST_NACC;
-        mbar_wait(&tempty_bar[acc], (uint32_t)(((local / ST_NACC) & 1) ^ 1));
-        tc_fence_after_sync();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc * 64);
+  } else if (warp < 16) {
+    // ======================= MMA warpgroups ===============================================
+    // warpgroup wg: output pixels 64*wg .. +63 of the row = A rows 64 * 16 B further into the row pair
+    const int wg = (warp - 8) >> 2;
+    const bool leader = (threadIdx.x & 127) == 0;
+    mbar_wait(wfull, 0u);
+    const uint32_t w_addr = smem_u32(sW);
+    const uint32_t ring_addr = smem_u32(ring);
+    // B: [k-chunk][cout][8]: chunk step 1024, 8-row group step 128; kh block 4096 B, K step (2 chunks) 2048 B
+    const uint64_t bdesc0 = make_smem_desc_none(w_addr, 1024u, 128u);
+    float d[32];
+    int qb = 0, qn = 0, local = 0;
+    for (int t = t_begin; t < t_end; ++t, ++local) {
+      const int oh = t % p.Ho;
+      const bool first = (t == t_begin) || (oh == 0);
+      if (first) {
+        qb = qn;
+        qn += 4;
+        for (int j = 0; j < 4; ++j) mbar_wait(&full_bar[(qb + j) % ST_NP], (uint32_t)(((qb + j) / ST_NP) & 1));
+      } else {
+        qb += 1;
+        qn += 1;
+        mbar_wait(&full_bar[(qb + 3) % ST_NP], (uint32_t)(((qb + 3) / ST_NP) & 1));
+      }
+      wg_fence();
 #pragma unroll
-        for (int kp = 0; kp < 4; ++kp) {   // row pair kp holds kernel rows 2*kp and 2*kp + 1
-          // A: row m = output pixel m, 16-byte chunk c = input pixels 2m + 4s + 2c, +1 -> LBO 16, SBO 128 (overlapping)
-          const uint64_t adesc0 =
-              make_smem_desc_none(ring_addr + (uint32_t)(((qb + kp) % ST_NP) * ST_PAIR_BYTES), 16u, 128u);
+      for (int kp = 0; kp < 4; ++kp) {   // row pair kp holds kernel rows 2*kp and 2*kp + 1
+        // A: row m = output pixel m, 16-byte chunk c = input pixels 2m + 4s + 2c, +1 -> LBO 16, SBO 128 (overlapping)
+        const uint64_t adesc0 = make_smem_desc_none(
+            ring_addr + (uint32_t)(((qb + kp) % ST_NP) * ST_PAIR_BYTES) + (uint32_t)wg * 1024u, 16u, 128u);
 #pragma unroll
-          for (int r = 0; r < 2; ++r) {
-            const int kh = 2 * kp + r;
-            if (kh < 7) {
+        for (int r = 0; r < 2; ++r) {
+          const int kh = 2 * kp + r;
+          if (kh < 7) {
 #pragma unroll
-              for (int s = 0; s < 2; ++s)
-                umma_bf16_elect(tmem_d, adesc0 + (uint64_t)((r * ST_ROW_BYTES + 32 * s) >> 4),
-                                bdesc0 + (uint64_t)((kh * 4096 + s * 2048) >> 4), idesc, (uint32_t)((kh | s) != 0));
-            }
+            for (int s = 0; s < 2; ++s)
+              wgmma_bf16<64, 0, 0>(d, adesc0 + (uint64_t)((r * ST_ROW_BYTES + 32 * s) >> 4),
+                                   bdesc0 + (uint64_t)((kh * 4096 + s * 2048) >> 4), (uint32_t)((kh | s) != 0));
           }
         }
-        const bool last = (t + 1 == t_end) || ((t + 1) % p.Ho == 0);
-        if (last) {
-          for (int j = 0; j < 4; ++j) umma_commit_elect(&empty_bar[(qb + j) % ST_NP]);
-        } else {
-          umma_commit_elect(&empty_bar[qb % ST_NP]);
-        }
-        umma_commit_elect(&tfull_bar[acc]);
       }
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(d);
+      const bool last = (t + 1 == t_end) || ((t + 1) % p.Ho == 0);
+      if (leader) {
+        if (last) {
+          for (int j = 0; j < 4; ++j) mbar_arrive(&empty_bar[(qb + j) % ST_NP]);
+        } else {
+          mbar_arrive(&empty_bar[qb % ST_NP]);
+        }
+      }
+      mbar_wait(tempty_bar, (uint32_t)((local & 1) ^ 1));
+      acc_store_smem<64>(accbuf, ST_ACC_LD, wg * 64, 0, d);
+      mbar_arrive(tfull_bar);
     }
-    __syncwarp();
   } else {
     // ======================= producer =====================================================
     if (lane == 0) {
@@ -219,13 +220,6 @@ stem_fprop_kernel(const __grid_constant__ CUtensorMap tmapY, const StemParams p)
     }
     __syncwarp();
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, ST_NACC * 64);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -236,10 +230,11 @@ stem_fprop_kernel(const __grid_constant__ CUtensorMap tmapY, const StemParams p)
 //     (a-3, a-2) with a = v >> 1; rows outside the image are TMA out-of-bounds zero tiles
 //   B (N-major, no swizzle)       = the input row itself: N = 8 window pixels x 4 channels, pixel k's window starts
 //     16 bytes after pixel k-1's (overlapping no-swizzle core matrices, as in the forward kernel)
-//   D = four TMEM accumulators [128 = 2 kh x 64 co][32 = (kw, c)] (row parity x chain), kept for the CTA's whole
-//     contiguous range of units and added to the fp32 gradient with atomics at the end.
+//   D = four accumulators [128 = 2 kh x 64 co][32 = (kw, c)] (row parity x chain), kept in registers for the CTA's
+//     whole contiguous range of units and added to the fp32 gradient with atomics at the end.
 // The dY ring has 11 slots + a mirror of slot 0 behind slot 10, so that "row oh-1, row oh" are always adjacent in smem.
-//   warps 0-3: final epilogue, warps 4 and 6: MMA issuers (one per chain), warp 5: producer.
+//   warps 0-7: two MMA warpgroups (warpgroup wg owns rows 64*wg .. +63 = the dY row tile wg of each pair), warp 8:
+//   producer.
 // ---------------------------------------------------------------------------------------------
 static constexpr int SW_NS = 11;   // 4 rows in use + 7 rows of prefetch (dY streams from HBM: the ring depth hides its latency)
 static constexpr int SW_TILE = 128 * 128;
@@ -253,6 +248,7 @@ static_assert(SW_BAR_OFF % 8 == 0 && SW_TOTAL <= 232448 - 1024, "stem wgrad smem
 struct StemWgradParams {
   const bf16* xs;   // [N][Hp][264][4]
   float* dw;        // [64][Cin][7][7] fp32, accumulated
+  Fix128* fx;    // fixed-point accumulators over the whole dw (fix_scratch)
   int N, Ho, Wo, Hp, Cin;
   int num_units;    // N * Hp
   int ksteps;       // ceil(Wo / 16)
@@ -267,7 +263,9 @@ __device__ __forceinline__ void tma_load_4d_stem(uint32_t dst_smem, const CUtens
       : "memory");
 }
 
-__global__ void __launch_bounds__(224, 1)
+static constexpr int SW_THREADS = 9 * 32;
+
+__global__ void __launch_bounds__(SW_THREADS, 1)
 stem_wgrad_kernel(const __grid_constant__ CUtensorMap tmapDY, const StemWgradParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -278,31 +276,21 @@ stem_wgrad_kernel(const __grid_constant__ CUtensorMap tmapDY, const StemWgradPar
   uint64_t* dempty = dfull + SW_NS;
   uint64_t* xfull = dempty + SW_NS;
   uint64_t* xempty = xfull + SW_NX;
-  uint64_t* done = xempty + SW_NX;
-  uint32_t* tmem_slot = (uint32_t*)(done + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int u_begin = (int)((int64_t)blockIdx.x * p.num_units / gridDim.x);
   const int u_end = (int)((int64_t)(blockIdx.x + 1) * p.num_units / gridDim.x);
 
-  if (warp == 5 && lane == 0) {
-    for (int s = 0; s < SW_NS; ++s) { mbar_init(&dfull[s], 1u); mbar_init(&dempty[s], 2u); }   // 2 = both MMA warps
+  if (warp == 8 && lane == 0) {
+    for (int s = 0; s < SW_NS; ++s) { mbar_init(&dfull[s], 1u); mbar_init(&dempty[s], 2u); }   // 2 = both warpgroups
     for (int s = 0; s < SW_NX; ++s) { mbar_init(&xfull[s], 1u); mbar_init(&xempty[s], 2u); }
-    mbar_init(done, 2u);
     fence_mbar_init();
     tma_prefetch_desc(&tmapDY);
   }
-  if (warp == 4) {
-    tmem_alloc(tmem_slot, 128);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 5) {
+  if (warp == 8) {
     // ======================= producer =====================================================
     if (lane == 0) {
       int q = 0, xq = 0;
@@ -327,90 +315,83 @@ stem_wgrad_kernel(const __grid_constant__ CUtensorMap tmapDY, const StemWgradPar
       }
     }
     __syncwarp();
-  } else if (warp == 4 || warp == 6) {
-    // ======================= MMA issuers (one warp per chain) =============================
-    // N = 32 MMAs take only 16 tensor-core cycles, so instruction issue is the limit: the two chains (independent
-    // accumulators) are issued by two warps, descriptors are built once per unit and advanced by immediates.
-    // the whole warp runs the loop (uniform control flow and operands); one elected lane issues (see common.cuh)
-    {
-      constexpr uint32_t idesc = make_idesc(1u, 128, 32, 1u, 1u);   // both operands MN-major
-      const int chain = warp == 4 ? 0 : 1;
-      const uint32_t dy_addr = smem_u32(sDY), x_addr = smem_u32(sX);
-      int qb = 0, qn = 0, xq = 0;
-      uint32_t used = 0;
-      for (int u = u_begin; u < u_end; ++u, ++xq) {
-        const int v = u % p.Hp;
-        const bool first = (u == u_begin) || (v == 0);
-        if (first) {
-          qb = qn;
-          qn += 4;
-          for (int j = 0; j < 4; ++j) mbar_wait(&dfull[(qb + j) % SW_NS], (uint32_t)(((qb + j) / SW_NS) & 1));
-        } else if ((v & 1) == 0) {
-          qb += 1;
-          qn += 1;
-          mbar_wait(&dfull[(qb + 3) % SW_NS], (uint32_t)(((qb + 3) / SW_NS) & 1));
-        }
-        const int xs = xq % SW_NX;
-        mbar_wait(&xfull[xs], (uint32_t)((xq / SW_NX) & 1));
-        tc_fence_after_sync();
-        // chain 0: dY rows (a-1, a) <-> kh = (par+2, par); chain 1: rows (a-3, a-2) <-> kh = (par+6, par+4)
-        const int par = v & 1;
-        const uint32_t tmem_d = tmem_base + (uint32_t)((par * 2 + chain) * 32);
-        const uint32_t tile0 = dy_addr + (uint32_t)(((qb + (chain == 0 ? 2 : 0)) % SW_NS) * SW_TILE);
-        const uint64_t adesc = make_smem_desc_sw128(tile0, (uint32_t)SW_TILE, 1024u);
-        const uint64_t bdesc = make_smem_desc_none(x_addr + (uint32_t)(xs * ST_ROW_BYTES), p.b_lbo, p.b_sbo);
-        const uint32_t acc0 = (used >> par) & 1u;
-        if (p.ksteps == 7) {
+  } else {
+    // ======================= MMA warpgroups ===============================================
+    const int wg = warp >> 2;
+    const bool leader = (threadIdx.x & 127) == 0;
+    const uint32_t dy_addr = smem_u32(sDY), x_addr = smem_u32(sX);
+    float d[4][16];   // [par * 2 + chain]
+    int qb = 0, qn = 0, xq = 0;
+    uint32_t used = 0;
+    for (int u = u_begin; u < u_end; ++u, ++xq) {
+      const int v = u % p.Hp;
+      const bool first = (u == u_begin) || (v == 0);
+      if (first) {
+        qb = qn;
+        qn += 4;
+        for (int j = 0; j < 4; ++j) mbar_wait(&dfull[(qb + j) % SW_NS], (uint32_t)(((qb + j) / SW_NS) & 1));
+      } else if ((v & 1) == 0) {
+        qb += 1;
+        qn += 1;
+        mbar_wait(&dfull[(qb + 3) % SW_NS], (uint32_t)(((qb + 3) / SW_NS) & 1));
+      }
+      const int xs = xq % SW_NX;
+      mbar_wait(&xfull[xs], (uint32_t)((xq / SW_NX) & 1));
+      // chain 0: dY rows (a-1, a) <-> kh = (par+2, par); chain 1: rows (a-3, a-2) <-> kh = (par+6, par+4)
+      const int par = v & 1;
+      const uint64_t bdesc = make_smem_desc_none(x_addr + (uint32_t)(xs * ST_ROW_BYTES), p.b_lbo, p.b_sbo);
+      const uint32_t acc0 = (used >> par) & 1u;
+      wg_fence();
 #pragma unroll
-          for (int ks = 0; ks < 7; ++ks)   // K step = 16 pixels: +2048 B in the dY tile, +256 B in the input row
-            umma_bf16_elect(tmem_d, adesc + (uint64_t)(128 * ks), bdesc + (uint64_t)(16 * ks), idesc, ks == 0 ? acc0 : 1u);
+      for (int chain = 0; chain < 2; ++chain) {
+        const uint32_t tile0 = dy_addr + (uint32_t)(((qb + (chain == 0 ? 2 : 0)) % SW_NS) * SW_TILE);
+        const uint64_t adesc = make_smem_desc_sw128(tile0 + (uint32_t)wg * SW_TILE, (uint32_t)SW_TILE, 1024u);
+        // K step = 16 pixels: +2048 B in the dY tile, +256 B in the input row
+        if (par == 0) {
+          for (int ks = 0; ks < p.ksteps; ++ks)
+            wgmma_bf16<32, 1, 1>(d[chain], adesc + (uint64_t)(128 * ks), bdesc + (uint64_t)(16 * ks), ks == 0 ? acc0 : 1u);
         } else {
           for (int ks = 0; ks < p.ksteps; ++ks)
-            umma_bf16_elect(tmem_d, adesc + (uint64_t)(128 * ks), bdesc + (uint64_t)(16 * ks), idesc, ks == 0 ? acc0 : 1u);
+            wgmma_bf16<32, 1, 1>(d[2 + chain], adesc + (uint64_t)(128 * ks), bdesc + (uint64_t)(16 * ks),
+                                 ks == 0 ? acc0 : 1u);
         }
-        used |= 1u << par;
-        umma_commit_elect(&xempty[xs]);
+      }
+      wg_commit();
+      wg_wait<0>();
+#pragma unroll
+      for (int a = 0; a < 4; ++a) wg_fence_acc(d[a]);
+      used |= 1u << par;
+      if (leader) {
+        mbar_arrive(&xempty[xs]);
         const bool last = (u + 1 == u_end) || (v == p.Hp - 1);
         if (last) {
-          for (int j = 0; j < 4; ++j) umma_commit_elect(&dempty[(qb + j) % SW_NS]);
+          for (int j = 0; j < 4; ++j) mbar_arrive(&dempty[(qb + j) % SW_NS]);
         } else if (v & 1) {
-          umma_commit_elect(&dempty[qb % SW_NS]);
+          mbar_arrive(&dempty[qb % SW_NS]);
         }
       }
-      umma_commit_elect(done);
     }
-    __syncwarp();
-  } else {
-    // ======================= epilogue (once) ==============================================
+    // ======================= epilogue (once): registers -> fp32 gradient ===================
     if (u_end > u_begin) {
-      mbar_wait(done, 0u);
-      tc_fence_after_sync();
-      const int L = warp * 32 + lane;
-      const int half = L >> 6, co = L & 63;
+      const int t = threadIdx.x & 127;
+      const int co = (t >> 5) * 16 + ((t & 31) >> 2);   // + 8 for the second row of a fragment pair
       const bool both = (u_end - u_begin) >= 2;
       const int only_par = (u_begin % p.Hp) & 1;
-      for (int acc = 0; acc < 4; ++acc) {
-        const int par = acc >> 1, chain = acc & 1;
+#pragma unroll
+      for (int a = 0; a < 4; ++a) {
+        const int par = a >> 1, chain = a & 1;
         if (!both && par != only_par) continue;   // this row parity never ran: the accumulator is uninitialised
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(acc * 32), r);
-        tmem_ld_wait();
-        const int kh = par + (chain == 0 ? (half == 0 ? 2 : 0) : (half == 0 ? 6 : 4));
+        const int kh = par + (chain == 0 ? (wg == 0 ? 2 : 0) : (wg == 0 ? 6 : 4));
         if (kh > 6) continue;
 #pragma unroll
-        for (int col = 0; col < 32; ++col) {
+        for (int i = 0; i < 16; ++i) {
+          const int col = 8 * (i >> 2) + 2 * (t & 3) + (i & 1);
+          const int row = co + ((i & 2) ? 8 : 0);
           const int kw = col >> 2, c = col & 3;
-          if (kw < 7 && c < p.Cin) atomicAdd(p.dw + ((co * p.Cin + c) * 7 + kh) * 7 + kw, __uint_as_float(r[col]));
+          if (kw < 7 && c < p.Cin) fix_add(p.fx + ((row * p.Cin + c) * 7 + kh) * 7 + kw, d[a][i]);
         }
       }
     }
-  }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 128);
   }
 }
 
@@ -484,7 +465,7 @@ extern "C" int byol_nchw_to_stem4(const float* x, void* xs, int N, int Cin, int 
   BYOL_CHECK_ARG(x && xs && N > 0 && byol_stem4_supported(Cin, 64, H, W, 7, 2, 3), "byol_nchw_to_stem4: bad args");
   const int64_t total = (int64_t)N * (H + 6) * ST_WP;
   int64_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   nchw_to_stem4_kernel<<<(int)blocks, 256, 0, stream>>>(x, (bf16*)xs, N, Cin, H, W);
   return check_launch("nchw_to_stem4_kernel");
 }
@@ -528,10 +509,17 @@ extern "C" int byol_stem_conv_fprop(const void* xs, const void* ws, void* y, flo
     if (e != cudaSuccess) { set_last_error("cudaFuncSetAttribute(stem_fprop) failed: %s", cudaGetErrorString(e)); return -2; }
     attr_set[dev_slot] = true;
   }
-  int grid = 2 * stem_sm_count();
+  int grid = stem_sm_count();
   if (grid > p.num_tiles) grid = p.num_tiles;
-  stem_fprop_kernel<<<grid, 320, ST_TOTAL, stream>>>(tmY, p);
-  return check_launch("stem_fprop_kernel");
+  if (col_sum != nullptr) {
+    p.fx = fix_scratch(stream, 128);
+    if (p.fx == nullptr) return -2;
+  }
+  stem_fprop_kernel<<<grid, ST_THREADS, ST_TOTAL, stream>>>(tmY, p);
+  int rc = check_launch("stem_fprop_kernel");
+  if (rc != 0 || col_sum == nullptr) return rc;
+  if ((rc = fix_flush(p.fx, col_sum, 64, stream)) != 0) return rc;
+  return fix_done(stream, fix_flush(p.fx + 64, col_sqsum, 64, stream));
 }
 
 // dw[64][Cin][7][7] (fp32) += dY^T * im2col(xs); dy: [N, H/2, W/2, 64] bf16
@@ -548,7 +536,7 @@ extern "C" int byol_stem_conv_wgrad(const void* xs, const void* dy, float* dw, i
   p.num_units = N * Hp;
   p.ksteps = (Wo + 15) / 16;
   // no-swizzle MN-major B: LBO = step between 8-pixel (K) groups, SBO = step between 16-byte N chunks
-  // (for no-swizzle MN-major operands the roles are swapped w.r.t. K-major: measured, the swapped assignment fails)
+  // (for no-swizzle MN-major operands the roles are swapped w.r.t. K-major)
   p.b_lbo = 128u;
   p.b_sbo = 16u;
   PFN_encodeTiledStem fn = stem_encode_fn();
@@ -571,6 +559,10 @@ extern "C" int byol_stem_conv_wgrad(const void* xs, const void* dy, float* dw, i
   }
   int grid = stem_sm_count();
   if (grid > p.num_units) grid = p.num_units;
-  stem_wgrad_kernel<<<grid, 224, SW_TOTAL, stream>>>(tmDY, p);
-  return check_launch("stem_wgrad_kernel");
+  const int64_t ndw = (int64_t)64 * Cin * 49;
+  p.fx = fix_scratch(stream, ndw);
+  if (p.fx == nullptr) return -2;
+  stem_wgrad_kernel<<<grid, SW_THREADS, SW_TOTAL, stream>>>(tmDY, p);
+  const int rc = check_launch("stem_wgrad_kernel");
+  return fix_done(stream, rc != 0 ? rc : fix_flush(p.fx, dw, ndw, stream));
 }

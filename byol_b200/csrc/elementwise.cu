@@ -3,13 +3,13 @@
 // These replace the ATen elementwise / pooling kernels under torchvision's ResNet stem and tail reached from
 // /root/reference/main.py:237 (`self.base_network(augmentation)`): MaxPool2d(3, 2, 1), AdaptiveAvgPool2d(1),
 // plus the NCHW fp32 -> NHWC bf16 input conversion and the fp32 master -> bf16 K-major weight layouts the
-// tcgen05 kernels consume.  All are HBM-bound streaming kernels: 16-byte vector accesses, grid-stride loops.
+// tensor-core (wgmma) kernels consume.  All are HBM-bound streaming kernels: 16-byte vector accesses, grid-stride loops.
 #include <stdlib.h>
 #include "common.cuh"
 
 namespace byol {
 
-static inline int grid_for(int64_t n, int block, int max_blocks = 148 * 16) {
+static inline int grid_for(int64_t n, int block, int max_blocks = 132 * 16) {
   int64_t b = (n + block - 1) / block;
   if (b > max_blocks) b = max_blocks;
   if (b < 1) b = 1;

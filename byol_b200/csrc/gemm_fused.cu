@@ -1,4 +1,4 @@
-// byol_b200 — plain GEMM (1x1 / stride-1 convolution, both operands by TMA) with a RICH epilogue, on tcgen05.
+// byol_b200 — plain GEMM (1x1 / stride-1 convolution, both operands by TMA) with a RICH epilogue, on wgmma.
 //
 //   out[M, N] = epilogue( src[M, K] x wt[N, K]^T ),   M = pixels, N = output channels (> 64), bf16 in / fp32 accumulate
 //
@@ -16,8 +16,9 @@
 // swizzled staging buffer — prefetched one chunk ahead, so its latency hides behind the MMA — and the same buffer is
 // then reused to stage the output tile for the TMA store; per-column vectors live in shared memory.
 //
-// Warp roles (320 threads, 2 CTAs / SM): warps 0-7 epilogue (TMEM lane quarter w & 3, column half w >> 2),
-// warp 8 MMA issuer, warp 9 TMA producer (2-stage operand ring, 2 TMEM accumulator stages, persistent tile loop).
+// Warp roles (544 threads, 1 CTA / SM): warps 0-7 epilogue (tile row quarter w & 3, column half w >> 2), warps 8-15
+// two MMA warpgroups (tile rows 0-63 / 64-127, accumulators in registers, handed to the epilogue through an fp32
+// tile in shared memory), warp 16 TMA producer (2-stage operand ring, persistent tile loop).
 #include <string.h>
 
 #include "common.cuh"
@@ -31,10 +32,13 @@ static constexpr int GF_A_OFF = 0;
 static constexpr int GF_B_OFF = GF_STAGES * GF_A_STAGE;
 static constexpr int GF_STAGE_OFF = GF_B_OFF + GF_STAGES * GF_B_STAGE;          // per warp 2 x 2048 B
 static constexpr int GF_PARAM_OFF = GF_STAGE_OFF + GF_EW * 4096;                // per warp 3 x 64 floats
-static constexpr int GF_BAR_OFF = GF_PARAM_OFF + GF_EW * 768;
+static constexpr int GF_ACC_LD = acc_ld(GF_BN);
+static constexpr int GF_ACC_OFF = GF_PARAM_OFF + GF_EW * 768;                   // [GF_BM][GF_ACC_LD] fp32
+static constexpr int GF_BAR_OFF = GF_ACC_OFF + GF_BM * GF_ACC_LD * 4;
 static constexpr int GF_NEEDED = GF_BAR_OFF + 512;
 static constexpr int GF_TOTAL = GF_NEEDED + 768;
-static_assert(GF_TOTAL <= 115712, "two CTAs per SM");
+static constexpr int GF_THREADS = 17 * 32;
+static_assert(GF_TOTAL <= 232448, "one CTA per SM");
 
 struct GemmFusedParams {
   const uint8_t* resid_mask;     // optional ReLU bits over the [M, ldc] index space of resid: add / use resid where set
@@ -44,6 +48,7 @@ struct GemmFusedParams {
   uint8_t* mask_out;             // optional: bits (stored value > 0), [M * ldc / 8]
   float* col_sum;                // statistics / backward sums, [N]
   float* col_sqsum;
+  Fix128* fx;                 // with col_sum: [2][N] fixed-point accumulators (fix_scratch)
   int has_resid, relu, no_store, bwd_reduce;
   int M, N, ldc, num_kb, tiles_n;
 };
@@ -54,7 +59,7 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
   return v;
 }
 
-__global__ void __launch_bounds__(320, 2)
+__global__ void __launch_bounds__(GF_THREADS, 1)
 gemm_fused_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB,
                   const __grid_constant__ CUtensorMap tmapC, const __grid_constant__ CUtensorMap tmapR,
                   const GemmFusedParams p, const int num_tiles) {
@@ -65,18 +70,19 @@ gemm_fused_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   uint8_t* smemB = smem + GF_B_OFF;
   uint64_t* full_bar = (uint64_t*)(smem + GF_BAR_OFF);
   uint64_t* empty_bar = full_bar + GF_STAGES;
-  uint64_t* tfull_bar = empty_bar + GF_STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint64_t* rbar = tempty_bar + 2;              // [GF_EW][2] residual tile landed
-  uint32_t* tmem_slot = (uint32_t*)(rbar + 2 * GF_EW);
+  uint64_t* tfull_bar = empty_bar + GF_STAGES;  // accumulator tile ready for the epilogue
+  uint64_t* tempty_bar = tfull_bar + 1;         // accumulator tile drained
+  uint64_t* rbar = tempty_bar + 1;              // [GF_EW][2] residual tile landed
+  float* accbuf = reinterpret_cast<float*>(smem + GF_ACC_OFF);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  constexpr int MMA_WARP = 8, TMA_WARP = 9;
+  constexpr int MMA_WARP = 8, TMA_WARP = 16;
 
   if (warp == TMA_WARP && lane == 0) {
-    for (int s = 0; s < GF_STAGES; ++s) { mbar_init(&full_bar[s], 1u); mbar_init(&empty_bar[s], 1u); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&tfull_bar[a], 1u); mbar_init(&tempty_bar[a], (uint32_t)GF_EW); }
+    for (int s = 0; s < GF_STAGES; ++s) { mbar_init(&full_bar[s], 1u); mbar_init(&empty_bar[s], 2u); }
+    mbar_init(tfull_bar, 256u);
+    mbar_init(tempty_bar, (uint32_t)GF_EW);
     for (int i = 0; i < 2 * GF_EW; ++i) mbar_init(&rbar[i], 1u);
     fence_mbar_init();
     tma_prefetch_desc(&tmapA);
@@ -84,14 +90,7 @@ gemm_fused_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     if (!p.no_store && !p.bwd_reduce) tma_prefetch_desc(&tmapC);
     if (p.has_resid) tma_prefetch_desc(&tmapR);
   }
-  if (warp == MMA_WARP) {
-    tmem_alloc(tmem_slot, 2 * GF_BN);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < GF_EW) {
     // ======================= epilogue =====================================================
@@ -115,8 +114,8 @@ gemm_fused_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         if (red_mode) {
           const int col = stat_n0 + col_w0 + i * 32 + lane;
           if (col < p.N) {
-            atomicAdd(p.col_sum + col, racc1[i]);
-            atomicAdd(p.col_sqsum + col, racc2[i]);
+            fix_add(p.fx + col, racc1[i]);
+            fix_add(p.fx + p.N + col, racc2[i]);
           }
           racc1[i] = 0.f; racc2[i] = 0.f;
         } else {
@@ -127,10 +126,10 @@ gemm_fused_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
           b.y += __shfl_xor_sync(0xffffffffu, b.y, 16);
           const int col = stat_n0 + col_w0 + i * 32 + 2 * (lane & 15);
           if (lane < 16 && col < p.N) {   // N is a multiple of 8: col + 1 is valid too
-            atomicAdd(p.col_sum + col, a.x);
-            atomicAdd(p.col_sum + col + 1, a.y);
-            atomicAdd(p.col_sqsum + col, b.x);
-            atomicAdd(p.col_sqsum + col + 1, b.y);
+            fix_add(p.fx + col, a.x);
+            fix_add(p.fx + col + 1, a.y);
+            fix_add(p.fx + p.N + col, b.x);
+            fix_add(p.fx + p.N + col + 1, b.y);
           }
           cs1[i] = 0ull; cs2[i] = 0ull;
         }
@@ -179,14 +178,12 @@ gemm_fused_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         }
         __syncwarp();
       }
-      const int acc = local & 1;
       const int mrow0 = m0 + quarter * 32;
       const int m = mrow0 + lane;
       const bool mvalid = m < p.M;
       int rows_valid = p.M - mrow0;
       rows_valid = rows_valid < 0 ? 0 : (rows_valid > 32 ? 32 : rows_valid);
-      mbar_wait(&tfull_bar[acc], (uint32_t)((local >> 1) & 1));
-      tc_fence_after_sync();
+      mbar_wait(tfull_bar, (uint32_t)(local & 1));
 #pragma unroll
       for (int cl = 0; cl < GF_CPW; ++cl) {
         const int c0 = col_w0 + cl * 32;
@@ -217,12 +214,10 @@ gemm_fused_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
           }
         }
         uint32_t r[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * GF_BN + c0), r);
-        tmem_ld_wait();
+        acc_load_row32(accbuf + (quarter * 32 + lane) * GF_ACC_LD + c0, r);
         if (cl == GF_CPW - 1) {
-          tc_fence_before_sync();
           __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty_bar[acc]);
+          if (lane == 0) mbar_arrive(tempty_bar);
         }
         if (!valid) continue;
         float v[32];
@@ -333,29 +328,36 @@ gemm_fused_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     }
     if (do_stats && stat_n0 >= 0) flush_stats();
     if (lane == 0) tma_store_wait_all();
-  } else if (warp == MMA_WARP) {
-    constexpr uint32_t idesc = make_idesc(1u, GF_BM, GF_BN, 0u, 0u);
+  } else if (warp >= MMA_WARP && warp < TMA_WARP) {
+    // warpgroup wg: tile rows 64*wg .. +63 (A rows 8 KB further into the stage)
+    const int wg = (warp - MMA_WARP) >> 2;
+    const bool leader = (threadIdx.x & 127) == 0;
+    float d[GF_BN / 2];
     int it = 0, local = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-      const int acc = local & 1;
-      mbar_wait(&tempty_bar[acc], (uint32_t)(((local >> 1) & 1) ^ 1));
-      tc_fence_after_sync();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(acc * GF_BN);
+      int prev_s = -1;
       for (int kb = 0; kb < p.num_kb; ++kb, ++it) {
         const int s = it % GF_STAGES;
         const uint32_t ph = (it / GF_STAGES) & 1;
         mbar_wait(&full_bar[s], ph);
-        tc_fence_after_sync();
-        const uint64_t adesc = make_smem_desc_sw128(smem_u32(smemA + s * GF_A_STAGE), 16, 1024);
+        const uint64_t adesc = make_smem_desc_sw128(smem_u32(smemA + s * GF_A_STAGE + wg * 8192), 16, 1024);
         const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smemB + s * GF_B_STAGE), 16, 1024);
+        wg_fence();
 #pragma unroll
         for (int k = 0; k < GF_BK / 16; ++k)
-          umma_bf16_elect(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (uint32_t)((kb | k) != 0));
-        umma_commit_elect(&empty_bar[s]);
+          wgmma_bf16<GF_BN, 0, 0>(d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)((kb | k) != 0));
+        wg_commit();
+        wg_wait<1>();
+        if (leader && prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
+        prev_s = s;
       }
-      umma_commit_elect(&tfull_bar[acc]);
+      wg_wait<0>();
+      wg_fence_acc(d);
+      if (leader && prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
+      mbar_wait(tempty_bar, (uint32_t)((local & 1) ^ 1));
+      acc_store_smem<GF_BN>(accbuf, GF_ACC_LD, wg * 64, 0, d);
+      mbar_arrive(tfull_bar);
     }
-    __syncwarp();
   } else if (warp == TMA_WARP) {
     if (lane == 0) {
       constexpr uint32_t tx = (uint32_t)(GF_A_STAGE + GF_B_STAGE);
@@ -373,12 +375,6 @@ gemm_fused_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       }
     }
     __syncwarp();
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == MMA_WARP) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 2 * GF_BN);
   }
 }
 
@@ -469,10 +465,17 @@ int gemm_fused_launch(const void* src, const void* wt, void* dst, const void* re
     if (e != cudaSuccess) { set_last_error("cudaFuncSetAttribute(gemm_fused) failed: %s", cudaGetErrorString(e)); return -2; }
     attr_set[dev_slot] = true;
   }
-  int grid = 2 * device_sm_count();
+  int grid = device_sm_count();
   if (grid > num_tiles) grid = num_tiles;
-  gemm_fused_kernel<<<grid, 320, GF_TOTAL, stream>>>(ta, tb, tc, tr, p, num_tiles);
-  return check_launch("gemm_fused_kernel");
+  if (col_sum != nullptr) {
+    p.fx = fix_scratch(stream, 2 * (int64_t)Ndim);
+    if (p.fx == nullptr) return -2;
+  }
+  gemm_fused_kernel<<<grid, GF_THREADS, GF_TOTAL, stream>>>(ta, tb, tc, tr, p, num_tiles);
+  int rc = check_launch("gemm_fused_kernel");
+  if (rc != 0 || col_sum == nullptr) return rc;
+  if ((rc = fix_flush(p.fx, col_sum, Ndim, stream)) != 0) return rc;
+  return fix_done(stream, fix_flush(p.fx + Ndim, col_sqsum, Ndim, stream));
 }
 
 }  // namespace byol

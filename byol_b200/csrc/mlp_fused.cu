@@ -5,17 +5,20 @@
 //
 //   x [B, K1] bf16,  W1 [H, K1],  b1 [H],  gamma / beta [H],  W2 [O, H],  b2 [O]      (H % 128 == 0, O <= 256, B <= 128 * tiles_m)
 //
-// Cooperative grid of tiles_m x (H / 128) CTAs, one per SM (B = 512, H = 4096 -> 128 CTAs), 192 threads:
-//   phase 1  h-tile[128 x 128] = x-tile . W1-tile^T            tcgen05, fp32 accumulator stays in TMEM
-//   phase 2  per-column sum / sum of squares of h = acc + b1     TMEM -> registers, transpose-reduce, global atomics
+// Cooperative grid of tiles_m x (H / 128) CTAs, one per SM (B = 512, H = 4096 -> 128 CTAs), 416 threads (warps 0-3
+// epilogue, warps 4-11 two MMA warpgroups owning tile rows 0-63 / 64-127, warp 12 TMA producer):
+//   phase 1  h-tile[128 x 128] = x-tile . W1-tile^T            wgmma, the fp32 accumulator is parked in shared memory
+//   phase 2  per-column sum / sum of squares of h = acc + b1     smem -> registers, transpose-reduce, global atomics
 //   ----- grid barrier (all M-tiles have contributed); under SyncBatchNorm CTA 0 then runs the peer-memory exchange of
 //         csrc/xchg.cu on the statistics vector and a second grid barrier follows -----
 //   phase 3  scale / shift per column (CTAs of M-tile 0 also update the running statistics and store the coefficients),
-//            a = relu(h * scale + shift) from the SAME TMEM accumulator -> bf16 -> shared memory in the K-major 128-byte
+//            a = relu(h * scale + shift) from the SAME parked accumulator -> bf16 -> shared memory in the K-major 128-byte
 //            swizzle, i.e. directly the A operand of the second GEMM (h and a are TMA-stored for the backward pass
 //            only when the lane is differentiated)
 //   phase 4  out-partial[128 x O] = a-tile[128 x 128] . W2[:, 128-column slice]^T   (K split over the H / 128 CTAs of a row
-//            block), accumulated into the fp32 output with vector reductions (+ b2 from the first slice)
+//            block), 64 output columns at a time, accumulated from the MMA registers in fixed point (+ b2 from the first
+//            slice) and added to the fp32 output after the kernel
+// Cross-CTA sums (statistics, output) are fixed point, so every run gives the same bits (common.cuh).
 // The hidden activation never makes a round trip through HBM between the two GEMMs.
 #include <cooperative_groups.h>
 #include <string.h>
@@ -29,9 +32,13 @@ static constexpr int MF_STAGES = 3;
 static constexpr int MF_RING = MF_STAGES * MF_STAGE;   // 96 KB; after GEMM1: [a-tile 32 KB | W2 slice 64 KB]
 static constexpr int MF_HSTAGE_OFF = MF_RING;          // 32 KB staging of h (bf16) for its TMA store
 static constexpr int MF_COEF_OFF = MF_HSTAGE_OFF + 32768;   // scale[128], shift[128], bias1[128]
-static constexpr int MF_BAR_OFF = MF_COEF_OFF + 3 * 512;
+static constexpr int MF_ACC_LD = acc_ld(128);
+static constexpr int MF_ACC_OFF = MF_COEF_OFF + 3 * 512;    // GEMM1 accumulator [128][MF_ACC_LD] fp32
+static constexpr int MF_BAR_OFF = MF_ACC_OFF + 128 * MF_ACC_LD * 4;
 static constexpr int MF_NEEDED = MF_BAR_OFF + 256;
 static constexpr int MF_TOTAL = MF_NEEDED + 1024;
+static constexpr int MF_THREADS = 13 * 32;
+static_assert(MF_TOTAL <= 232448, "mlp_fused: shared memory");
 
 struct MlpPeer {           // SyncBatchNorm exchange (csrc/xchg.cu layout); world <= 1: unused
   uint64_t p[8];
@@ -51,6 +58,7 @@ struct MlpParams {
   float* coeffs;           // [4][H] scale, shift, mean, invstd (always written by the CTAs of M-tile 0)
   float* out;              // [B, O] fp32, zeroed by the caller
   uint32_t* grid_bar;      // [2] count, generation (zero-initialised once)
+  Fix128* fx;           // fixed-point accumulators (fix_scratch): [2H] statistics, then [B, O] output
   int B, K1, H, O;
   int tiles_h;
   int train, save;
@@ -117,7 +125,7 @@ __device__ void peer_sum(float* vals, int n, const MlpPeer& pe) {
   if (threadIdx.x == 0) *pe.counter = seq;
 }
 
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(MF_THREADS, 1)
 mlp_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_constant__ CUtensorMap tmapW1,
                      const __grid_constant__ CUtensorMap tmapW2, const __grid_constant__ CUtensorMap tmapH,
                      const __grid_constant__ CUtensorMap tmapA, const MlpParams p) {
@@ -129,11 +137,10 @@ mlp_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
   float* s_b1 = s_shift + 128;
   uint64_t* full_bar = (uint64_t*)(smem + MF_BAR_OFF);
   uint64_t* empty_bar = full_bar + MF_STAGES;
-  uint64_t* acc1_bar = empty_bar + MF_STAGES;    // GEMM1 accumulator complete (also: the ring is free)
+  uint64_t* acc1_bar = empty_bar + MF_STAGES;    // GEMM1 accumulator parked in smem (also: the ring is free)
   uint64_t* w2_bar = acc1_bar + 1;               // W2 slice landed
   uint64_t* a_bar = w2_bar + 1;                  // a-tile written by the 128 epilogue threads
-  uint64_t* acc2_bar = a_bar + 1;
-  uint32_t* tmem_slot = (uint32_t*)(acc2_bar + 1);
+  float* accbuf = reinterpret_cast<float*>(smem + MF_ACC_OFF);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -142,29 +149,23 @@ mlp_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
   const int m0 = tile_m * 128, n0 = tile_h * 128;
   const int num_kb = p.K1 / 64;
 
-  if (warp == 5 && lane == 0) {
-    for (int s = 0; s < MF_STAGES; ++s) { mbar_init(&full_bar[s], 1u); mbar_init(&empty_bar[s], 1u); }
-    mbar_init(acc1_bar, 1u);
+  if (warp == 12 && lane == 0) {
+    for (int s = 0; s < MF_STAGES; ++s) { mbar_init(&full_bar[s], 1u); mbar_init(&empty_bar[s], 2u); }
+    mbar_init(acc1_bar, 256u);
     mbar_init(w2_bar, 1u);
     mbar_init(a_bar, 128u);
-    mbar_init(acc2_bar, 1u);
     fence_mbar_init();
     tma_prefetch_desc(&tmapX);
     tma_prefetch_desc(&tmapW1);
     tma_prefetch_desc(&tmapW2);
   }
-  if (warp == 4) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
   if (threadIdx.x < 128) s_b1[threadIdx.x] = p.b1 != nullptr ? p.b1[n0 + threadIdx.x] : 0.f;
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
   const uint32_t ring = smem_u32(smem);
+  const int wg = (warp - 4) >> 2;                       // MMA warpgroup (warps 4-11): tile rows 64*wg .. +63
+  const bool wg_leader = (threadIdx.x & 127) == 0;
 
-  if (warp == 5) {
+  if (warp == 12) {
     // ---------------- TMA producer ----------------
     if (lane == 0) {
       for (int kb = 0; kb < num_kb; ++kb) {
@@ -182,37 +183,40 @@ mlp_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
       tma_load_2d(ring + 65536, &tmapW2, w2_bar, n0 + 64, 0);
     }
     __syncwarp();
-  } else if (warp == 4) {
-    // ---------------- MMA issuer ----------------
-    {
-      constexpr uint32_t idesc1 = make_idesc(1u, 128, 128, 0u, 0u);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % MF_STAGES;
-        const uint32_t ph = (kb / MF_STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after_sync();
-        const uint64_t adesc = make_smem_desc_sw128(ring + s * MF_STAGE, 16, 1024);
-        const uint64_t bdesc = make_smem_desc_sw128(ring + s * MF_STAGE + 16384, 16, 1024);
+  } else if (warp >= 4) {
+    // ---------------- MMA warpgroups: GEMM1 ----------------
+    float d[64];
+    int prev_s = -1;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      const int s = kb % MF_STAGES;
+      const uint32_t ph = (kb / MF_STAGES) & 1;
+      mbar_wait(&full_bar[s], ph);
+      const uint64_t adesc = make_smem_desc_sw128(ring + s * MF_STAGE + wg * 8192, 16, 1024);
+      const uint64_t bdesc = make_smem_desc_sw128(ring + s * MF_STAGE + 16384, 16, 1024);
+      wg_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16_elect(tmem_base, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc1, (uint32_t)((kb | k) != 0));
-        umma_commit_elect(&empty_bar[s]);
-      }
-      umma_commit_elect(acc1_bar);
+      for (int k = 0; k < 4; ++k)
+        wgmma_bf16<128, 0, 0>(d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)((kb | k) != 0));
+      wg_commit();
+      wg_wait<1>();
+      if (wg_leader && prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
+      prev_s = s;
     }
+    wg_wait<0>();
+    wg_fence_acc(d);
+    acc_store_smem<128>(accbuf, MF_ACC_LD, wg * 64, 0, d);
+    mbar_arrive(acc1_bar);
   }
   // ---------------- phase 2: statistics of h (epilogue warps 0-3; lane = row) ----------------
   const int row = warp * 32 + lane;          // valid for warps 0-3
   const bool rvalid = warp < 4 && (m0 + row) < p.B;
   if (warp < 4) {
     mbar_wait(acc1_bar, 0);
-    tc_fence_after_sync();
     uint8_t* hst = smem + MF_HSTAGE_OFF;
 #pragma unroll 1
     for (int c0 = 0; c0 < 128; c0 += 32) {
       uint32_t r[32];
-      tmem_ld_32x32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, r);
-      tmem_ld_wait();
+      acc_load_row32(accbuf + row * MF_ACC_LD + c0, r);
       float v[32], q[32];
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
@@ -244,8 +248,8 @@ mlp_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
             }
           }
         }
-        atomicAdd(p.stats + n0 + c0 + lane, v[0]);
-        atomicAdd(p.stats + p.H + n0 + c0 + lane, q[0]);
+        fix_add(p.fx + n0 + c0 + lane, v[0]);
+        fix_add(p.fx + p.H + n0 + c0 + lane, q[0]);
       }
     }
     if (p.save) {
@@ -261,6 +265,17 @@ mlp_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
     }
   }
   if (p.train) {
+    grid_barrier(p.grid_bar, (int)gridDim.x);
+    // the fixed-point sums (identical in every run, whatever the order of the CTAs) -> fp32 statistics
+    if (tile_m == 0 && threadIdx.x < 128) {
+      const int c = n0 + (int)threadIdx.x;
+      const Fix128* f1 = p.fx + c;
+      const Fix128* f2 = p.fx + p.H + c;
+      p.stats[c] = (float)fix_value(Fix128{__ldcg(&f1->lo), __ldcg(&f1->hi), __ldcg(&f1->spill)});
+      p.stats[p.H + c] = (float)fix_value(Fix128{__ldcg(&f2->lo), __ldcg(&f2->hi), __ldcg(&f2->spill)});
+      p.fx[c] = Fix128{0ull, 0ll, 0.0};         // only these threads read them: leave the scratch zeroed (fix_scratch)
+      p.fx[p.H + c] = Fix128{0ull, 0ll, 0.0};
+    }
     grid_barrier(p.grid_bar, (int)gridDim.x);
     if (p.peer.world > 1) {
       if (blockIdx.x == 0) peer_sum(p.stats, 2 * p.H, p.peer);
@@ -302,8 +317,7 @@ mlp_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
 #pragma unroll 1
     for (int c0 = 0; c0 < 128; c0 += 32) {
       uint32_t r[32];
-      tmem_ld_32x32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, r);
-      tmem_ld_wait();
+      acc_load_row32(accbuf + row * MF_ACC_LD + c0, r);
 #pragma unroll
       for (int j = 0; j < 32; j += 8) {
         float a[8];
@@ -319,66 +333,57 @@ mlp_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
         *reinterpret_cast<uint4*>(smem + (c >> 6) * 16384 + sw128_offset((uint32_t)row, (uint32_t)((c & 63) >> 3))) = w;
       }
     }
-    tc_fence_before_sync();
     fence_proxy_async_smem();
     mbar_arrive(a_bar);
   }
-  if (warp == 4) {
-    // ---------------- phase 4: GEMM2 partial, K = this CTA's 128 hidden columns ----------------
+  if (warp >= 4 && warp < 12) {
+    // ---------------- phase 4: GEMM2 partial, K = this CTA's 128 hidden columns, 64 output columns at a time -----
     mbar_wait(a_bar, 0);
     mbar_wait(w2_bar, 0);
-    tc_fence_after_sync();
-    const uint32_t idesc2 = make_idesc(1u, 128, (uint32_t)p.O, 0u, 0u);
+    const int t = threadIdx.x & 127;
+    const int r0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);   // tile row of d[4j], d[4j+1]; +8 for d[4j+2 ..]
+    float d2[32];
+#pragma unroll 1
+    for (int o0 = 0; o0 < p.O; o0 += 64) {
+      wg_fence();
 #pragma unroll
-    for (int kb = 0; kb < 2; ++kb) {
-      const uint64_t adesc = make_smem_desc_sw128(ring + kb * 16384, 16, 1024);
-      const uint64_t bdesc = make_smem_desc_sw128(ring + 32768 + kb * 32768, 16, 1024);
+      for (int kb = 0; kb < 2; ++kb) {
+        const uint64_t adesc = make_smem_desc_sw128(ring + kb * 16384 + wg * 8192, 16, 1024);
+        const uint64_t bdesc = make_smem_desc_sw128(ring + 32768 + kb * 32768 + o0 * 128, 16, 1024);
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        umma_bf16_elect(tmem_base + 128u, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc2, (uint32_t)((kb | k) != 0));
+        for (int k = 0; k < 4; ++k)
+          wgmma_bf16<64, 0, 0>(d2, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)((kb | k) != 0));
+      }
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(d2);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int c = o0 + 8 * j + 2 * (t & 3);
+        if (c >= p.O) continue;   // O is a multiple of 16: c + 1 < O too
+        float2 bb = make_float2(0.f, 0.f);
+        if (tile_h == 0 && p.b2 != nullptr) bb = make_float2(p.b2[c], p.b2[c + 1]);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int rr = m0 + r0 + 8 * h;
+          if (rr < p.B) {
+            Fix128* acc = p.fx + 2 * p.H + (int64_t)rr * p.O + c;
+            fix_add(acc, d2[4 * j + 2 * h] + bb.x);
+            fix_add(acc + 1, d2[4 * j + 2 * h + 1] + bb.y);
+          }
+        }
+      }
     }
-    umma_commit_elect(acc2_bar);
-    __syncwarp();
   }
-  if (warp < 4) {
-    if (p.save && threadIdx.x == 0) {
+  if (warp < 4 && p.save) {
+    if (threadIdx.x == 0) {
       // a (bf16) for the backward pass: the GEMM2 operand buffers are already in the TMA-storable layout
       mbar_wait(a_bar, 0);                 // all 128 rows written and fenced
       tma_store_2d(&tmapA, ring, n0, m0);
       tma_store_2d(&tmapA, ring + 16384, n0 + 64, m0);
       tma_store_commit();
+      tma_store_wait_all();
     }
-    mbar_wait(acc2_bar, 0);
-    tc_fence_after_sync();
-    float* orow = p.out + (int64_t)(m0 + row) * p.O;
-#pragma unroll 1
-    for (int c0 = 0; c0 < p.O; c0 += 32) {
-      uint32_t r[32];
-      tmem_ld_32x32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(128 + c0), r);
-      tmem_ld_wait();
-      if (rvalid) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          if (c0 + j < p.O) {
-            float4 v = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
-                                   __uint_as_float(r[j + 3]));
-            if (tile_h == 0 && p.b2 != nullptr) {
-              v.x += p.b2[c0 + j]; v.y += p.b2[c0 + j + 1]; v.z += p.b2[c0 + j + 2]; v.w += p.b2[c0 + j + 3];
-            }
-            asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(orow + c0 + j), "f"(v.x), "f"(v.y),
-                         "f"(v.z), "f"(v.w)
-                         : "memory");
-          }
-        }
-      }
-    }
-    tc_fence_before_sync();
-    if (p.save && threadIdx.x == 0) tma_store_wait_all();
-  }
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -479,7 +484,7 @@ extern "C" int byol_mlp_fused_fwd(const void* x, const void* w1, const float* b1
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(192);
+  cfg.blockDim = dim3(MF_THREADS);
   cfg.dynamicSmemBytes = MF_TOTAL;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
@@ -487,10 +492,13 @@ extern "C" int byol_mlp_fused_fwd(const void* x, const void* w1, const float* b1
   attr[0].val.cooperative = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
+  p.fx = fix_scratch(stream, 2 * (int64_t)H + (int64_t)B * O);
+  if (p.fx == nullptr) return -2;
   cudaError_t e = cudaLaunchKernelEx(&cfg, mlp_fused_fwd_kernel, tx, tw1, tw2, th, ta, p);
   if (e != cudaSuccess) {
     set_last_error("byol_mlp_fused_fwd: cooperative launch failed: %s", cudaGetErrorString(e));
     return -100;
   }
-  return check_launch("mlp_fused_fwd_kernel");
+  if (check_launch("mlp_fused_fwd_kernel") != 0) return -100;
+  return fix_done(stream, fix_flush(p.fx + 2 * (int64_t)H, out, (int64_t)B * O, stream));
 }

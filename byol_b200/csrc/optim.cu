@@ -16,7 +16,7 @@ namespace byol {
 // ---------------------------------------------------------------------------------------------
 __global__ void loss_fwd_partial_kernel(const float* __restrict__ q1, const float* __restrict__ q2,
                                         const float* __restrict__ z1, const float* __restrict__ z2,
-                                        double* __restrict__ sums, int64_t n4) {
+                                        Fix128* __restrict__ sums, int64_t n4) {
   float acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
     const float4 a = __ldg(reinterpret_cast<const float4*>(q1) + i);
@@ -44,18 +44,23 @@ __global__ void loss_fwd_partial_kernel(const float* __restrict__ q1, const floa
     for (int k = 0; k < 6; ++k) {
       float v = lane < nw ? sh[k][lane] : 0.f;
       v = warp_sum(v);
-      if (lane == 0) atomicAdd(sums + k, (double)v);
+      if (lane == 0) fix_add(sums + k, v);   // fixed point: order-independent
     }
   }
 }
 
 // loss = -2/b * ( <q1,z2>/(|q1||z2|) + <q2,z1>/(|q2||z1|) );  also stores fp32 copies of the six sums
-__global__ void loss_finalize_kernel(const double* __restrict__ sums, float* __restrict__ loss,
+__global__ void loss_finalize_kernel(Fix128* __restrict__ sums, float* __restrict__ loss,
                                      float* __restrict__ saved, int rows) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
-    const float nq1 = sqrtf((float)sums[0]), nq2 = sqrtf((float)sums[1]);
-    const float nz1 = sqrtf((float)sums[2]), nz2 = sqrtf((float)sums[3]);
-    const float s12 = (float)sums[4], s21 = (float)sums[5];
+    float v[6];
+    for (int k = 0; k < 6; ++k) {
+      v[k] = (float)fix_value(sums[k]);
+      sums[k] = Fix128{0ull, 0ll, 0.0};   // the scratch is left zeroed (fix_scratch)
+    }
+    const float nq1 = sqrtf(v[0]), nq2 = sqrtf(v[1]);
+    const float nz1 = sqrtf(v[2]), nz2 = sqrtf(v[3]);
+    const float s12 = v[4], s21 = v[5];
     const float l = (-2.f * s12 / (nq1 * nz2) + -2.f * s21 / (nq2 * nz1)) / (float)rows;
     loss[0] = l;
     saved[0] = nq1; saved[1] = nq2; saved[2] = nz1; saved[3] = nz2; saved[4] = s12; saved[5] = s21;
@@ -342,7 +347,7 @@ ce_bwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labe
   for (int c = lane; c < C; c += 32) d[c] = k * (expf(x[c] - lse) - (c == lab ? 1.f : 0.f));
 }
 
-static inline int grid_for(int64_t n, int block, int max_blocks = 148 * 16) {
+static inline int grid_for(int64_t n, int block, int max_blocks = 132 * 16) {
   int64_t b = (n + block - 1) / block;
   if (b > max_blocks) b = max_blocks;
   if (b < 1) b = 1;
@@ -354,17 +359,18 @@ static inline int grid_for(int64_t n, int block, int max_blocks = 148 * 16) {
 using namespace byol;
 
 // q1,q2,z1,z2: [rows, dim] fp32 contiguous (rows*dim % 4 == 0).  workspace: 6 doubles (zeroed here).
-// loss: 1 float.  saved: 6 floats consumed by byol_loss_bwd.
+// loss: 1 float.  saved: 6 floats consumed by byol_loss_bwd.  The six sums are accumulated in fixed point in the
+// stream's scratch (fix_scratch); `workspace` is part of the ABI but no longer used.
 extern "C" int byol_loss_fwd(const float* q1, const float* q2, const float* z1, const float* z2, int rows, int dim,
                              double* workspace, float* loss, float* saved, cudaStream_t stream) {
   BYOL_CHECK_ARG(q1 && q2 && z1 && z2 && workspace && loss && saved, "byol_loss_fwd: null pointer");
   const int64_t n = (int64_t)rows * dim;
   BYOL_CHECK_ARG(rows > 0 && dim > 0 && n % 4 == 0, "byol_loss_fwd: rows*dim must be a positive multiple of 4");
-  cudaError_t e = cudaMemsetAsync(workspace, 0, 6 * sizeof(double), stream);
-  if (e != cudaSuccess) { set_last_error("byol_loss_fwd: memset failed: %s", cudaGetErrorString(e)); return -2; }
-  loss_fwd_partial_kernel<<<grid_for(n / 4, 256, 148), 256, 0, stream>>>(q1, q2, z1, z2, workspace, n / 4);
-  loss_finalize_kernel<<<1, 32, 0, stream>>>(workspace, loss, saved, rows);
-  return check_launch("loss_fwd kernels");
+  Fix128* sums = fix_scratch(stream, 6);
+  if (sums == nullptr) return -2;
+  loss_fwd_partial_kernel<<<grid_for(n / 4, 256, 132), 256, 0, stream>>>(q1, q2, z1, z2, sums, n / 4);
+  loss_finalize_kernel<<<1, 32, 0, stream>>>(sums, loss, saved, rows);
+  return fix_done(stream, check_launch("loss_fwd kernels"));
 }
 
 extern "C" int byol_loss_bwd(const float* q1, const float* q2, const float* z1, const float* z2, const float* saved,
@@ -372,7 +378,7 @@ extern "C" int byol_loss_bwd(const float* q1, const float* q2, const float* z1, 
   BYOL_CHECK_ARG(q1 && q2 && z1 && z2 && saved && dq1 && dq2, "byol_loss_bwd: null pointer");
   const int64_t n = (int64_t)rows * dim;
   BYOL_CHECK_ARG(rows > 0 && dim > 0 && n % 4 == 0, "byol_loss_bwd: rows*dim must be a positive multiple of 4");
-  loss_bwd_kernel<<<grid_for(n / 4, 256, 148 * 4), 256, 0, stream>>>(q1, q2, z1, z2, saved, grad_out, dq1, dq2,
+  loss_bwd_kernel<<<grid_for(n / 4, 256, 132 * 4), 256, 0, stream>>>(q1, q2, z1, z2, saved, grad_out, dq1, dq2,
                                                                     n / 4, rows);
   return check_launch("loss_bwd_kernel");
 }
@@ -382,7 +388,7 @@ extern "C" int byol_ema_update(const float* x, float* mean, float one_minus_deca
                                cudaStream_t stream) {
   BYOL_CHECK_ARG(x && mean && n > 0, "byol_ema_update: bad args");
   BYOL_CHECK_ARG(((uintptr_t)x % 16 == 0) && ((uintptr_t)mean % 16 == 0), "byol_ema_update: pointers must be 16-byte aligned");
-  ema_kernel<<<grid_for(n / 4 + 1, 256, 148 * 8), 256, 0, stream>>>(x, mean, one_minus_decay, decay, n);
+  ema_kernel<<<grid_for(n / 4 + 1, 256, 132 * 8), 256, 0, stream>>>(x, mean, one_minus_decay, decay, n);
   return check_launch("ema_kernel");
 }
 

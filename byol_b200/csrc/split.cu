@@ -1,7 +1,7 @@
 // byol_b200 — the fp32-accurate forward path ("split-bf16"): elementwise kernels.
 //
 // BASELINE.json configs[1] asks for the reference's fp32 results (/root/reference/main.py:229-276 runs every conv /
-// linear / BatchNorm in fp32) within 1e-3.  tcgen05 has no fp32 MMA, and single-pass TF32 misses that bar by two orders
+// linear / BatchNorm in fp32) within 1e-3.  The tensor cores have no fp32 MMA, and single-pass TF32 misses that bar by two orders
 // of magnitude on a randomly initialised ResNet-50 (DESIGN.md §4: 5-19 % relative error, bf16 30-80 %), so the
 // accurate path keeps the bf16 tensor-core kernels and feeds them EXACT SPLITS of the fp32 operands instead:
 //
@@ -44,7 +44,7 @@ __device__ __forceinline__ void split3(float x, bf16 (&pl)[3]) {
   pl[2] = __float2bfloat16_rn(r2);
 }
 
-static inline int grid_for(int64_t n, int block, int max_blocks = 148 * 16) {
+static inline int grid_for(int64_t n, int block, int max_blocks = 132 * 16) {
   int64_t b = (n + block - 1) / block;
   if (b > max_blocks) b = max_blocks;
   if (b < 1) b = 1;
@@ -116,7 +116,9 @@ __global__ void prep_weight_planes_kernel(const float* __restrict__ w, bf16* __r
 // BatchNorm statistics of an fp32 [M, C] matrix, accumulated in fp64: stats[0:C] += sum, stats[C:2C] += sum of squares
 // block = 256 threads = (256 / CT) row lanes x CT columns (CT = min(C, 256)); grid.x strides rows, grid.y tiles columns
 // ---------------------------------------------------------------------------------------------
-__global__ void stats_f32_kernel(const float* __restrict__ y, double* __restrict__ stats, int64_t M, int C, int CT,
+// part: [gridDim.x][2][C] fp64 partial sums, one slot per row block (summed in block order by stats_f32_sum_kernel, so
+// the statistics are the same bits in every run at full fp64 precision)
+__global__ void stats_f32_kernel(const float* __restrict__ y, double* __restrict__ part, int64_t M, int C, int CT,
                                  int64_t rows_per_block) {
   const int col = blockIdx.y * CT + (int)(threadIdx.x % CT);
   const int rlane = (int)(threadIdx.x / CT);
@@ -141,8 +143,8 @@ __global__ void stats_f32_kernel(const float* __restrict__ y, double* __restrict
       s += sh[0][l * CT + (threadIdx.x % CT)];
       q += sh[1][l * CT + (threadIdx.x % CT)];
     }
-    atomicAdd(stats + col, s);
-    atomicAdd(stats + C + col, q);
+    part[(int64_t)blockIdx.x * 2 * C + col] = s;
+    part[(int64_t)blockIdx.x * 2 * C + C + col] = q;
   }
 }
 
@@ -329,17 +331,33 @@ extern "C" int byol_prep_weight_planes(const float* w, void* out, int Cout, int 
   return check_launch("prep_weight_planes_kernel");
 }
 
+__global__ void stats_f32_sum_kernel(double* __restrict__ part, double* __restrict__ stats, int nblocks, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double s = 0.0;
+  for (int k = 0; k < nblocks; ++k) {
+    s += part[(int64_t)k * n + i];
+    part[(int64_t)k * n + i] = 0.0;   // the scratch is left zeroed (fix_scratch)
+  }
+  stats[i] += s;
+}
+
 // stats: 2C doubles, zeroed by the caller
 extern "C" int byol_stats_f32(const float* y, double* stats, int64_t M, int C, cudaStream_t stream) {
   BYOL_CHECK_ARG(y && stats && M > 0 && C > 0, "byol_stats_f32: bad args");
   int CT = 1;
   while (CT < C && CT < 256) CT <<= 1;           // power of two <= 256 covering min(C, 256) columns per block
   const int lanes = 256 / CT;
-  int64_t rows_per_block = (M + 148 * 4 - 1) / (148 * 4);
+  int64_t rows_per_block = (M + 132 * 4 - 1) / (132 * 4);
   if (rows_per_block < 4 * lanes) rows_per_block = 4 * lanes;
   dim3 grid((unsigned)((M + rows_per_block - 1) / rows_per_block), (unsigned)((C + CT - 1) / CT));
-  stats_f32_kernel<<<grid, 256, 0, stream>>>(y, stats, M, C, CT, rows_per_block);
-  return check_launch("stats_f32_kernel");
+  // the scratch of the fixed-point reductions holds the 2 * grid.x * C fp64 partials (three doubles per entry)
+  Fix128* scratch = fix_scratch(stream, ((int64_t)grid.x * C * 2 + 2) / 3);
+  if (scratch == nullptr) return -2;
+  double* part = reinterpret_cast<double*>(scratch);
+  stats_f32_kernel<<<grid, 256, 0, stream>>>(y, part, M, C, CT, rows_per_block);
+  stats_f32_sum_kernel<<<(2 * C + 255) / 256, 256, 0, stream>>>(part, stats, (int)grid.x, 2 * C);
+  return fix_done(stream, check_launch("stats_f32_kernel"));
 }
 
 extern "C" int byol_bn_finalize_lanes_f64(const double* stats, double count, int L, const float* gamma0,

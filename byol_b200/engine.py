@@ -1,6 +1,6 @@
 """Step engine: walks the (torchvision-shaped) module tree of :class:`byol_b200.model.BYOL`, keeps every
 parameter / gradient in flat fp32 buffers, and runs the BYOL forward and backward as explicit sequences of the
-sm_100a kernels in ``ops`` — no autograd graph, no ATen compute on the hot path.
+sm_90a kernels in ``ops`` — no autograd graph, no ATen compute on the hot path.
 
 Reference semantics reproduced (file:line are /root/reference):
 
@@ -149,11 +149,10 @@ class Engine(object):
         # terms (~16 / 24 mantissa bits), fp32 conv outputs, fp64 BatchNorm statistics (csrc/split.cu)
         self.T = 0
         self.s_online = self.s_target = None
-        # block-output BatchNorm fused into the expanding 1x1 GEMMs (see _fuse3).  OFF by default: measured on B200
-        # (tools/time_fused.py, ResNet-50 stage 1, 512 images) the two GEMM passes cost 250 + 483 us where the unfused
-        # conv + BN-apply kernels take 174 + 450 us, and the recomputing backward 484 + 447 us against 296 + 417 us —
-        # the statistics pass is pure overhead and the rich epilogue runs at ~65 % of its HBM floor, the plain
-        # elementwise kernels at ~85 %.  It saves 7-14 GB of activations per 512 images; BYOL_B200_FUSE3=1 enables it.
+        # block-output BatchNorm fused into the expanding 1x1 GEMMs (see _fuse3).  OFF by default: the statistics pass
+        # re-runs the GEMM, so the fused form moves more work than the unfused conv + BN-apply kernels
+        # (tools/time_fused.py times both).  It saves 7-14 GB of activations per 512 images; BYOL_B200_FUSE3=1
+        # enables it.
         self.fuse3 = os.environ.get("BYOL_B200_FUSE3", "0") == "1"
         self.fuse3_max_planes = int(os.environ.get("BYOL_B200_FUSE3_MAX_PLANES", "128"))
         # projector / predictor forward as one cooperative kernel per lane (csrc/mlp_fused.cu); =0: four launches
@@ -170,7 +169,7 @@ class Engine(object):
         params = list(model.parameters())
         dev = params[0].device
         if dev.type != "cuda":
-            raise RuntimeError("byol_b200.BYOL runs on CUDA only (sm_100a kernels; no CPU path): move the model "
+            raise RuntimeError("byol_b200.BYOL runs on CUDA only (sm_90a kernels; no CPU path): move the model "
                                "to the GPU with .cuda() before calling it")
         total = sum(p.numel() for p in params)
         theta = torch.empty(total, dtype=F32, device=dev)
@@ -482,7 +481,7 @@ class Engine(object):
 
     def _mlp_fwd_fused(self, mlp, xs, lanes, train, key):
         """Linear -> BatchNorm1d -> ReLU -> Linear as ONE cooperative kernel per lane (csrc/mlp_fused.cu): the hidden
-        activation stays in TMEM / shared memory between the two GEMMs; the BatchNorm statistics cross the grid
+        activation stays in shared memory between the two GEMMs; the BatchNorm statistics cross the grid
         (and, under SyncBatchNorm, the ranks) inside the kernel."""
         l1, l2 = mlp
         H, bn = l1.cout, l1.bn

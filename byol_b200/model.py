@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's model API (``/root/reference/main.py:133-276``): ``CosEMA`` and ``BYOL``
 with the same constructor arguments, attributes, ``state_dict`` keys and 13-key forward dict — but the compute
-runs in the sm_100a kernels of ``byol_b200`` through :class:`byol_b200.engine.Engine`.
+runs in the sm_90a kernels of ``byol_b200`` through :class:`byol_b200.engine.Engine`.
 
 The nn.Module tree (torchvision ResNet children[:-1], head, predictor, linear_classifier) is kept only as the
 *container* of parameters and buffers, so ``named_parameters()``, ``state_dict()``, ``nn.SyncBatchNorm

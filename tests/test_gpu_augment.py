@@ -101,7 +101,7 @@ def test_augment_parameter_distribution(cuda):
 
 
 def test_augment_throughput_and_step(cuda):
-    """Feeds the training step: 2 x [N, 3, 224, 224] views straight into BYOL; > 20 k images/s on a B200."""
+    """Feeds the training step: 2 x [N, 3, 224, 224] views straight into BYOL."""
     from byol_b200.augment import TwoViewAugment
     n = 256
     imgs = torch.rand(n, 3, 256, 256, device=cuda)

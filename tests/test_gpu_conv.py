@@ -1,4 +1,4 @@
-"""GPU parity: tcgen05 implicit-GEMM conv / linear (fprop, dgrad, wgrad) vs the CPU oracle (oracle/ops_ref.py).
+"""GPU parity: wgmma implicit-GEMM conv / linear (fprop, dgrad, wgrad) vs the CPU oracle (oracle/ops_ref.py).
 
 Inputs are bf16-representable, the oracle runs in fp32 on the same values, so the only differences are fp32
 accumulation order (tolerance 2e-3 relative to the output scale, stated per test) and, where the kernel
@@ -145,7 +145,7 @@ def test_stem_folded_layout(cuda, shape):
 
 @pytest.mark.parametrize("shape", [(2, 32, 32), (3, 30, 26), (2, 224, 224), (5, 64, 64), (1, 256, 256)])
 def test_stem4_fprop(cuda, shape):
-    """Dedicated stem kernel: padded NHWC4 input, im2col formed by overlapping no-swizzle UMMA descriptors."""
+    """Dedicated stem kernel: padded NHWC4 input, im2col formed by overlapping no-swizzle wgmma descriptors."""
     from byol_b200 import ops
     n, h, w = shape
     assert ops.stem4_supported(3, 64, h, w, 7, 2, 3)

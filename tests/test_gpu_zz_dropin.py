@@ -1,7 +1,6 @@
 """GPU: the byol_b200 classes dropped into the UNMODIFIED reference's own step loop.
 
-`baseline/_ref/` holds a verbatim copy of the reference's Python sources (made by tools/ship_reference.py in the
-build container; git-ignored, shipped with the gpurun snapshot — the GPU box has no /root/reference).  The test
+`oracle/_ref/` holds the reference's own modules, byte-compiled by build() (oracle/build_ref.py; git-ignored).  The test
 imports that `main` with the import shims of oracle/ref_shims for its three missing submodules, rebinds the four
 names INTEGRATION.md tells a maintainer to re-import (BYOL, loss_function, LARS, DistributedDataParallelPassthrough)
 and then calls the reference's `main.execute_graph` (/root/reference/main.py:559-662) — its loop, its
@@ -21,12 +20,12 @@ from tests.test_oracle_golden import _batches, load_case
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 def _import_reference_main(arch, rep, b, r):
-    if not os.path.exists(os.path.join(REF, "main.py")):
-        pytest.skip("baseline/_ref/main.py not shipped (run tools/ship_reference.py where /root/reference exists)")
+    if not os.path.exists(os.path.join(REF, "main.pyc")):
+        pytest.skip("oracle/_ref has no compiled reference (build() found no reference checkout)")
     for m in [k for k in sys.modules if k in ("main", "objective") or k.startswith(("optimizers", "helpers", "datasets", "tree"))]:
         del sys.modules[m]
     argv, path = sys.argv, list(sys.path)

@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""The UNMODIFIED reference's stock PyTorch path timed on the same B200s (the ">= 1.5x the reference PyTorch/DDP
+"""The UNMODIFIED reference's stock PyTorch path timed on the same GPUs (the ">= 1.5x the reference PyTorch/DDP
 images/sec" target of BASELINE.json's north_star; BASELINE.md section 5.2).
 
     python tools/ref_gpu_baseline.py --mode fp32 --batch-per-gpu 256                       # configs[1], 1 GPU
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29511 \
         tools/ref_gpu_baseline.py --mode bf16 --batch-per-gpu 512 --sync-bn               # configs[2], 8 GPUs
 
-What runs: `baseline/_ref/main.py` (verbatim copy of /root/reference/main.py, shipped by tools/ship_reference.py)
+What runs: the reference's `main.py`, byte-compiled into oracle/_ref by build() (oracle/build_ref.py)
 — its `BYOL`, its `loss_function`, its `LARS` around torch.optim.SGD(momentum 0.9), SyncBatchNorm conversion and
 DistributedDataParallel(find_unused_parameters=True) exactly as main.build_loader_model_grapher wires them
 (main.py:428-443) — driven by its own `main.execute_graph` over a synthetic on-device loader.  None of byol_b200's
@@ -21,7 +21,7 @@ import os
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 def parse():
