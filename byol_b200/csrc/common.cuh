@@ -28,18 +28,22 @@ int device_sm_count();   // SM count of the current device (cached per device; 1
 // (rounded to an integer) is split into hi = floor(x / 2^32) and lo = x - hi * 2^32 in [0, 2^32], added to two
 // independent 64-bit words (fire-and-forget reductions, no carry between them).  Integer addition is associative, so
 // the totals do not depend on the order in which blocks arrive and every run gives the same bits; the value is
-// hi * 2^-18 + lo * 2^-50 (resolution 8.9e-16).  Addends that are not finite or whose magnitude reaches kFixMax go to
-// an fp64 side sum instead, so NaN / Inf propagate to the result and huge values keep their magnitude (that side sum
-// is order-dependent in its last bits, which only happens on a diverging step).  With every fixed-point addend below
-// 2^36 the integer part cannot overflow for fewer than 512 such addends per element.  The accumulators live in a
-// per-stream scratch buffer (fix_scratch) and are added to their fp32 destination once by fix_flush.
+// hi * 2^-18 + lo * 2^-50 (resolution 8.9e-16).  Only the part of an addend below kFixSplit = 2^20 in magnitude goes to
+// the fixed-point words; the rest, a multiple of 2^20 (v truncated towards zero), goes to an fp64 side sum.  Sums of
+// multiples of 2^20 are exact in fp64 up to 2^73, so that side sum is order-independent too, and a total keeps every
+// bit however large its addends are.  NaN / Inf go to the side sum whole and propagate to the result (beyond 2^73, and
+// with NaN / Inf, the side sum is order-dependent in its last bits: a diverging step).  With every fixed-point part
+// below 2^20 the hi word (range 2^45) cannot wrap for fewer than 2^25 (33 M) addends per element, and the lo word not
+// for fewer than 2^32; the kernels add at most one partial per 32 rows (2 x 10^5 for a 6.4 M-row BatchNorm).  The
+// accumulators live in a per-stream scratch buffer (fix_scratch) and are added to their fp32 destination once by
+// fix_flush.
 // ----------------------------------------------------------------------------
 struct Fix128 {
   unsigned long long lo;
   long long hi;
-  double spill;   // non-finite / out-of-range addends
+  double spill;   // multiples of 2^20 and non-finite addends
 };
-static constexpr double kFixMax = 68719476736.0;   // 2^36
+static constexpr double kFixSplit = 1048576.0;   // 2^20
 // n zeroed accumulators on `stream` (stream-ordered), nullptr on error.  Whoever reads them leaves them at zero; a
 // wrapper that got the scratch calls fix_done when its reduction is complete, otherwise the next fix_scratch on that
 // stream zeroes the buffer again (an error path can not leave stale sums behind).
@@ -53,9 +57,11 @@ __device__ __forceinline__ void fix_add_words(Fix128* acc, unsigned long long lo
   atomicAdd(reinterpret_cast<unsigned long long*>(&acc->hi), (unsigned long long)hi);
 }
 __device__ __forceinline__ void fix_add(Fix128* acc, double v) {
-  if (!(fabs(v) < kFixMax)) {   // NaN, Inf or too large for the fixed-point words
-    atomicAdd(&acc->spill, v);
-    return;
+  if (!(fabs(v) < kFixSplit)) {   // NaN, Inf, or a part too large for the fixed-point words
+    const double big = isfinite(v) ? trunc(v * 0x1p-20) * 0x1p20 : v;
+    atomicAdd(&acc->spill, big);
+    if (!isfinite(v)) return;
+    v -= big;                      // exact: the bits of v below 2^20, |v| < 2^20
   }
   const double x = v * 0x1p50;                 // exact (power-of-two scaling)
   const double hi = floor(x * 0x1p-32);

@@ -17,6 +17,7 @@ Reference semantics reproduced (file:line are /root/reference):
 Data layout: activations NHWC bf16; conv outputs are stored raw ("y") and normalised copies ("a") are
 materialised by a fused BN-apply(+residual)+ReLU kernel; BN statistics come from the conv epilogue.
 """
+import gc
 import os
 
 import torch
@@ -1091,24 +1092,35 @@ class Engine(object):
         st.mean_ptr = mean.data_ptr()
         rep_cat = model._rep_cat
         torch.cuda.synchronize()
-        pool = torch.cuda.graph_pool_handle()
-        st.fwd = torch.cuda.CUDAGraph()
-        n0 = launch_count[0]
-        with torch.cuda.graph(st.fwd, pool=pool, capture_error_mode="thread_local"):
-            self.prep_step(mean, True)
-            outs, _ = self.forward_lanes(None, lanes, True, rep_bf16_out=[rep_cat[:b], rep_cat[b:], None, None],
-                                         x8=[st.inputs[0], st.inputs[1], st.inputs[0], st.inputs[1]])
-            st.logits = self.classifier_forward(rep_cat, [outs[0][0], outs[1][0]])
-        st.fwd_launches = launch_count[0] - n0
-        st.outs = [t for o in outs for t in o]
-        # backward for the usual gradient pattern: only the two online predictions receive a gradient
-        # (objective.py:23-24 detaches the targets; main.py:601 adds the classifier loss, which is stop-grad)
-        st.d_pred = [torch.zeros_like(st.outs[2]), torch.zeros_like(st.outs[5])]
-        st.bwd = torch.cuda.CUDAGraph()
-        n0 = launch_count[0]
-        with torch.cuda.graph(st.bwd, pool=pool, capture_error_mode="thread_local"):
-            self.backward_online(st.saved, [None, None], [None, None], st.d_pred, notify=False)
-        st.bwd_launches = launch_count[0] - n0
+        # A dead model that is part of a reference cycle still owns its captured graphs until Python's cycle collector
+        # runs.  If that happened during this capture, destroying those graphs (cudaGraphExecDestroy) would be an
+        # unsafe call from the capturing thread and would invalidate the capture.  So collect first and keep the
+        # collector off until both graphs are captured.
+        gc.collect()
+        gc_was_enabled = gc.isenabled()
+        gc.disable()
+        try:
+            pool = torch.cuda.graph_pool_handle()
+            st.fwd = torch.cuda.CUDAGraph()
+            n0 = launch_count[0]
+            with torch.cuda.graph(st.fwd, pool=pool, capture_error_mode="thread_local"):
+                self.prep_step(mean, True)
+                outs, _ = self.forward_lanes(None, lanes, True, rep_bf16_out=[rep_cat[:b], rep_cat[b:], None, None],
+                                             x8=[st.inputs[0], st.inputs[1], st.inputs[0], st.inputs[1]])
+                st.logits = self.classifier_forward(rep_cat, [outs[0][0], outs[1][0]])
+            st.fwd_launches = launch_count[0] - n0
+            st.outs = [t for o in outs for t in o]
+            # backward for the usual gradient pattern: only the two online predictions receive a gradient
+            # (objective.py:23-24 detaches the targets; main.py:601 adds the classifier loss, which is stop-grad)
+            st.d_pred = [torch.zeros_like(st.outs[2]), torch.zeros_like(st.outs[5])]
+            st.bwd = torch.cuda.CUDAGraph()
+            n0 = launch_count[0]
+            with torch.cuda.graph(st.bwd, pool=pool, capture_error_mode="thread_local"):
+                self.backward_online(st.saved, [None, None], [None, None], st.d_pred, notify=False)
+            st.bwd_launches = launch_count[0] - n0
+        finally:
+            if gc_was_enabled:
+                gc.enable()
         st.pool = pool
         return st
 

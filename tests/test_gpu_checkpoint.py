@@ -40,15 +40,17 @@ def test_checkpoint_round_trip(cuda):
     r1 = wiring.train_step(m1, o1, *batches[2])
     r2 = wiring.train_step(m2, o2, *batches[2])
     torch.cuda.synchronize()
-    # BN statistics and wgrad accumulate with fp32 atomics (order varies run to run) and small-batch BatchNorm
-    # amplifies that, so two executions of the same step agree to ~1e-4, not bit-for-bit
-    assert abs(float(r1["loss_mean"]) - float(r2["loss_mean"])) < 2e-3 * abs(float(r1["loss_mean"]))
+    # every cross-block sum is order-independent (fixed point, csrc/common.cuh): the restored model continues with
+    # the same bits as the original
+    assert torch.equal(r1["loss_mean"], r2["loss_mean"])
     t0 = torch.cat([sd_m[k].reshape(-1).float() for k, _ in m1.named_parameters()])
-    t1 = torch.nn.utils.parameters_to_vector(m1.parameters())
-    t2 = torch.nn.utils.parameters_to_vector(m2.parameters())
-    u1, u2 = (t1 - t0).double(), (t2 - t0).double()
-    assert float(u1.norm()) > 0 and float((u1 @ u2) / (u1.norm() * u2.norm())) > 0.99   # incl. restored momentum
-    assert torch.allclose(m1.target_network.mean, m2.target_network.mean, rtol=1e-4, atol=1e-6)
+    t1 = torch.nn.utils.parameters_to_vector(m1.parameters()).detach()
+    t2 = torch.nn.utils.parameters_to_vector(m2.parameters()).detach()
+    assert float((t1 - t0).norm()) > 0 and torch.equal(t1, t2)          # incl. the restored momentum
+    mom = [torch.cat([s["momentum_buffer"].reshape(-1) for s in o.state_dict()["state"].values()]) for o in (o1, o2)]
+    assert torch.equal(mom[0], mom[1])
+    assert torch.equal(m1.target_network.mean, m2.target_network.mean)
+    assert all(torch.equal(a, b) for a, b in zip(m1.buffers(), m2.buffers()))
     for p in m2.parameters():                              # still views of the flat buffer after load_state_dict
         assert p.data_ptr() >= m2._engine.theta.data_ptr()
     assert m2._engine.is_flat()
