@@ -83,6 +83,19 @@ _SIGNATURES = {
                           c_void_p, c_int64, c_int, c_int, c_int, c_void_p],
     "byol_maxpool_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "byol_avgpool_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
+    # fp32-accurate backward path
+    "byol_prep_weight_dgrad_planes": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
+    "byol_conv_dgrad_planes": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                               c_int, c_int, c_int, c_int, c_int, c_void_p],
+    "byol_conv_wgrad_planes": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                               c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    "byol_bn_bwd_reduce_f32": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
+                               c_int, c_int, c_void_p],
+    "byol_bn_bwd_apply_f32": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                              c_void_p, c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int,
+                              c_int, c_void_p],
+    "byol_maxpool_bwd_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    "byol_avgpool_bwd_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
     "byol_mlp_fused_supported": [c_int, c_int, c_int, c_int],
     "byol_mlp_fused_fwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                            c_void_p, c_float, c_float, c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,

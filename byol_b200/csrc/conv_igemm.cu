@@ -32,6 +32,7 @@ struct ConvGemmParams {
   const bf16* resid;   // optional, [M, ldc] bf16, added in the epilogue
   const uint8_t* resid_mask;   // optional ReLU mask bits over the same [M, ldc] index space: add resid only where set
   int resid_up;                // 1: resid is [Nimg, Ho/2, Wo/2, ldc] and belongs to the even (h, w) pixels only
+  const float* resid_f32;      // optional fp32 residual over the same index space (fp32 outputs only)
   const float* bias;   // optional, [Ndim]
   float* col_sum;      // optional, [Ndim] fp32: += sum over rows of the stored value
   float* col_sqsum;    // optional, [Ndim] fp32: += sum over rows of value^2
@@ -270,6 +271,12 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
               }
             }
           }
+        }
+        if (p.resid_f32 != nullptr && rvalid) {
+          const float* rp = p.resid_f32 + rrow * p.ldc + nbase;
+#pragma unroll
+          for (int j = 0; j < 32; ++j)
+            if (nbase + j < p.Ndim) v[j] += rp[j];
         }
         if (p.relu) {
 #pragma unroll
@@ -641,6 +648,13 @@ struct WgradParams {
   int fold_kw;       // 1: C == 8 and the KW taps are folded into the 64-wide column group: column = kw*8 + c
   int small_src;     // 1: 32-bit element offsets are safe
   Fix128* fx;     // fixed-point accumulators over the whole dw (fix_scratch), flushed into dw after the kernel
+  // split-operand plane layouts (byol_conv_wgrad_planes): the product terms are an outer K loop.  K-block kb belongs
+  // to term kb / kb_per_term, which reads dY columns from term * dy_term on and src channels from src_term[term] on.
+  // Plain bf16 operands: terms = 1, ldsrc = C.
+  int terms, kb_per_term;
+  int ldsrc;         // src pixel pitch in elements
+  int dy_term;
+  int src_term[6];
 };
 
 static constexpr int WG_KROWS = 64;  // pixels per k-block
@@ -706,9 +720,10 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       if (p.fold_kw) { kh = group; kw = cw >> 3; ci = 0; cvalid = cvalid && kw < p.KW; }
       else           { kh = group / p.KW; kw = group - kh * p.KW; ci = cw; }
       const int dh = kh - p.pad, dw = kw - p.pad;
-      const int64_t sC = (int64_t)p.stride * p.C;
+      const int64_t sC = (int64_t)p.stride * p.ldsrc;
       for (int it = 0; it < nkb; ++it) {
         const int kb = kb_begin + it;
+        const int term = p.terms == 1 ? 0 : kb / p.kb_per_term;
         const int s = it % STAGES;
         const uint32_t ph = (it / STAGES) & 1;
         if (it >= GATHER_LAG) {   // publish the older stage before blocking on a free slot (see conv_igemm_kernel)
@@ -718,7 +733,8 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         }
         mbar_wait(&empty_bar[s], ph ^ 1);
         const uint32_t stage_base = smem_u32(smemB + s * B_STAGE) + ch64 * (WG_KROWS * 128);
-        int m = kb * WG_KROWS + rbase;
+        const int cterm = ci + p.src_term[term];
+        int m = (kb - term * p.kb_per_term) * WG_KROWS + rbase;
         int ow = m % p.Wo;
         int t = m / p.Wo;
         int oh = t % p.Ho;
@@ -726,7 +742,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         int sw = ow * p.stride + dw;
         int sh = oh * p.stride + dh;
         bool hvalid = cvalid && sh >= 0 && sh < p.Hs;
-        int64_t off = (((int64_t)n * p.Hs + sh) * p.Ws + sw) * p.C + ci;
+        int64_t off = (((int64_t)n * p.Hs + sh) * p.Ws + sw) * p.ldsrc + cterm;
 #pragma unroll
         for (int i = 0; i < PER_THREAD; ++i) {
           const bool v = hvalid && m < p.M && sw >= 0 && sw < p.Ws;
@@ -740,7 +756,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
             sw = dw;
             sh = oh * p.stride + dh;
             hvalid = cvalid && sh >= 0 && sh < p.Hs;
-            off = (((int64_t)n * p.Hs + sh) * p.Ws + sw) * p.C + ci;
+            off = (((int64_t)n * p.Hs + sh) * p.Ws + sw) * p.ldsrc + cterm;
           }
         }
         cp_async_commit();
@@ -811,18 +827,22 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       constexpr uint32_t tx = (uint32_t)WG_A_STAGE + (B_TMA ? (uint32_t)B_STAGE : 0u);
       for (int it = 0; it < nkb; ++it) {
         const int kb = kb_begin + it;
+        const int term = p.terms == 1 ? 0 : kb / p.kb_per_term;
+        const int row = (kb - term * p.kb_per_term) * WG_KROWS;
+        const int col_a = co0 + term * p.dy_term;
         const int s = it % STAGES;
         const uint32_t ph = (it / STAGES) & 1;
         mbar_wait(&empty_bar[s], ph ^ 1);
         mbar_arrive_expect_tx(&full_bar[s], tx);
         const uint32_t a_base = smem_u32(smemA + s * WG_A_STAGE);
-        tma_load_2d(a_base, &tmapA, &full_bar[s], co0, kb * WG_KROWS);
-        tma_load_2d(a_base + WG_KROWS * 128, &tmapA, &full_bar[s], co0 + 64, kb * WG_KROWS);
+        // with several terms, co rows past Cout read the next term's columns: those accumulator rows are discarded
+        tma_load_2d(a_base, &tmapA, &full_bar[s], col_a, row);
+        tma_load_2d(a_base + WG_KROWS * 128, &tmapA, &full_bar[s], col_a + 64, row);
         if (B_TMA) {
           const uint32_t b_base = smem_u32(smemB + s * B_STAGE);
 #pragma unroll
           for (int c = 0; c < NCH; ++c)
-            tma_load_2d(b_base + c * (WG_KROWS * 128), &tmapB, &full_bar[s], n0 + 64 * c, kb * WG_KROWS);
+            tma_load_2d(b_base + c * (WG_KROWS * 128), &tmapB, &full_bar[s], n0 + 64 * c + p.src_term[term], row);
         }
       }
     }
@@ -924,11 +944,15 @@ using namespace byol;
 // mode 0 (fprop):  src coord = o*stride - pad + k
 // mode 1 (dgrad):  src coord = (o + pad - k) / stride  (valid only when divisible); here `src` is dY,
 //                  (Hs, Ws) its spatial size and (Ho, Wo) the spatial size of dX.
-extern "C" int byol_conv_igemm(const void* src, const void* wt, void* dst, const void* resid,
-                               const void* resid_mask, int resid_up, const float* bias, float* col_sum, float* col_sqsum, int Nimg, int Hs, int Ws, int C, int Ho, int Wo,
-                               int Ndim, int KH, int KW, int stride, int pad, int mode, int ldw, int ldc,
-                               int out_fp32, int relu, int force_gather, cudaStream_t stream) {
+// resid_f32 (fp32 outputs only): an fp32 residual added in the epilogue (the fp32 backward's residual-branch gradient)
+static int conv_igemm_impl(const void* src, const void* wt, void* dst, const void* resid, const float* resid_f32,
+                           const void* resid_mask, int resid_up, const float* bias, float* col_sum, float* col_sqsum,
+                           int Nimg, int Hs, int Ws, int C, int Ho, int Wo, int Ndim, int KH, int KW, int stride,
+                           int pad, int mode, int ldw, int ldc, int out_fp32, int relu, int force_gather,
+                           cudaStream_t stream) {
   BYOL_CHECK_ARG(src && wt && dst, "byol_conv_igemm: null pointer");
+  BYOL_CHECK_ARG(resid_f32 == nullptr || (out_fp32 && resid == nullptr && !resid_up),
+                 "byol_conv_igemm: an fp32 residual needs an fp32 output and no other residual");
   BYOL_CHECK_ARG(C % 8 == 0 && C >= 8, "byol_conv_igemm: C=%d must be a multiple of 8", C);
   // bf16 outputs are TMA-stored (16-byte row pitch); fp32 outputs (logits, MLP outputs) may have any width
   BYOL_CHECK_ARG(Ndim > 0 && (Ndim % 8 == 0 || (out_fp32 && resid == nullptr && col_sum == nullptr)),
@@ -948,11 +972,13 @@ extern "C" int byol_conv_igemm(const void* src, const void* wt, void* dst, const
                  "byol_conv_igemm: resid_up needs resid, even output dims and a non-parity mode");
   // 1x1 / stride 1 with a residual tile in the epilogue (conv1 dgrad + the residual-branch gradient): the kernel that
   // stages the residual by TMA instead of per-lane global loads (3.5x faster at 56x56, tools/time_dgrad_resid.py)
-  if (!force_gather && resid != nullptr && !resid_up && KH == 1 && KW == 1 && stride == 1 && pad == 0 && !out_fp32 &&
+  // (these two kernels take no fp32 residual: an fp32 residual always goes to conv_igemm_kernel)
+  if (!force_gather && resid_f32 == nullptr && resid != nullptr && !resid_up && KH == 1 && KW == 1 && stride == 1 &&
+      pad == 0 && !out_fp32 &&
       col_sum == nullptr && gemm_fused_applicable((int)M64, C, Ndim, ldw, ldc))
     return gemm_fused_launch(src, wt, dst, resid, resid_mask, nullptr, bias, nullptr, nullptr, nullptr, nullptr,
                              (int)M64, C, Ndim, ldw, ldc, relu, 0, 0, stream);
-  if (!force_gather && resid_mask == nullptr && !resid_up && Hs == Ho && Ws == Wo && ldw >= 9 * C &&
+  if (!force_gather && resid_f32 == nullptr && resid_mask == nullptr && !resid_up && Hs == Ho && Ws == Wo && ldw >= 9 * C &&
       patch_conv_applicable(Hs, Ws, C, Ndim, KH, KW, stride, pad, out_fp32, bias, (int64_t)Nimg * Hs * Ws * C))
     return patch_conv_launch(src, wt, dst, resid, col_sum, col_sqsum, Nimg, Hs, Ws, C, Ndim, ldw, ldc, mode, relu,
                              sm_count(), stream);
@@ -963,6 +989,7 @@ extern "C" int byol_conv_igemm(const void* src, const void* wt, void* dst, const
   p.resid = (const bf16*)resid;
   p.resid_mask = (const uint8_t*)resid_mask;
   p.resid_up = resid_up ? 1 : 0;
+  p.resid_f32 = resid_f32;
   p.bias = bias;
   p.col_sum = col_sum;
   p.col_sqsum = col_sqsum;
@@ -1035,6 +1062,26 @@ extern "C" int byol_conv_igemm(const void* src, const void* wt, void* dst, const
   return fix_done(stream, fix_flush(p.fx + Ndim, col_sqsum, Ndim, stream));
 }
 
+extern "C" int byol_conv_igemm(const void* src, const void* wt, void* dst, const void* resid,
+                               const void* resid_mask, int resid_up, const float* bias, float* col_sum, float* col_sqsum, int Nimg, int Hs, int Ws, int C, int Ho, int Wo,
+                               int Ndim, int KH, int KW, int stride, int pad, int mode, int ldw, int ldc,
+                               int out_fp32, int relu, int force_gather, cudaStream_t stream) {
+  return conv_igemm_impl(src, wt, dst, resid, nullptr, resid_mask, resid_up, bias, col_sum, col_sqsum, Nimg, Hs, Ws, C,
+                         Ho, Wo, Ndim, KH, KW, stride, pad, mode, ldw, ldc, out_fp32, relu, force_gather, stream);
+}
+
+// fp32-accurate dgrad: dx[Nimg, H, W, Cin] (fp32) = conv_transpose(dY, W) (+ resid_f32, fp32 [Nimg, H, W, Cin]).
+// dy: bf16 planes [Nimg, Hs, Ws, T*Cout] (activation pattern), wd: bf16 [Cin, taps*T*Cout] (byol_prep_weight_dgrad_planes).
+// One implicit GEMM over T*Cout channels.  Stride-2 layers take the gather path (the parity mode stores bf16 only).
+extern "C" int byol_conv_dgrad_planes(const void* dy, const void* wd, float* dx, const float* resid_f32, int Nimg,
+                                      int Hs, int Ws, int Cout, int H, int W, int Cin, int KH, int KW, int stride,
+                                      int pad, int T, cudaStream_t stream) {
+  BYOL_CHECK_ARG((T == 3 || T == 6) && Cout % 8 == 0 && Cin % 8 == 0, "byol_conv_dgrad_planes: bad args (T=%d Cout=%d Cin=%d)",
+                 T, Cout, Cin);
+  return conv_igemm_impl(dy, wd, dx, nullptr, resid_f32, nullptr, 0, nullptr, nullptr, nullptr, Nimg, Hs, Ws, T * Cout,
+                         H, W, Cin, KH, KW, stride, pad, 1, KH * KW * T * Cout, Cin, 1, 0, 0, stream);
+}
+
 template <int BN, bool B_TMA>
 static int launch_wgrad(const CUtensorMap& ta, const CUtensorMap& tb, const WgradParams& p, int grid,
                         cudaStream_t stream) {
@@ -1058,21 +1105,31 @@ static int launch_wgrad(const CUtensorMap& ta, const CUtensorMap& tb, const Wgra
 // dW[Cout][Cin_real][KH][KW] (fp32) += dY^T x gather(src);  dy: [M, Cout] bf16, src: NHWC [Nimg,Hs,Ws,C]
 // ldy: row pitch of dy in elements (0 = Cout); a pitch > Cout lets Cout be any width (TMA zero-fills the columns
 // beyond Cout), e.g. the gradient of a 10-class classifier stored with a pitch of 16.
-extern "C" int byol_conv_wgrad(const void* src, const void* dy, float* dw, int Nimg, int Hs, int Ws, int C,
-                               int Cin_real, int Ho, int Wo, int Cout, int ldy, int KH, int KW, int stride, int pad,
-                               int force_gather, cudaStream_t stream) {
+// T: 0 = plain bf16 operands; 3 / 6 = split-operand planes (byol_conv_wgrad_planes)
+static int conv_wgrad_impl(const void* src, const void* dy, float* dw, int Nimg, int Hs, int Ws, int C, int Cin_real,
+                           int Ho, int Wo, int Cout, int ldy, int KH, int KW, int stride, int pad, int force_gather,
+                           int T, cudaStream_t stream) {
   BYOL_CHECK_ARG(src && dy && dw, "byol_conv_wgrad: null pointer");
   if (ldy == 0) ldy = Cout;
   BYOL_CHECK_ARG(C % 8 == 0 && ldy % 8 == 0 && ldy >= Cout && Cout > 0,
                  "byol_conv_wgrad: C=%d and the dy pitch %d must be multiples of 8 (Cout=%d)", C, ldy, Cout);
   BYOL_CHECK_ARG(Cin_real <= C, "byol_conv_wgrad: Cin_real > C");
+  BYOL_CHECK_ARG(T == 0 || T == 3 || T == 6, "byol_conv_wgrad: bad T=%d", T);
   const int64_t M64 = (int64_t)Nimg * Ho * Wo;
   BYOL_CHECK_ARG(M64 > 0 && M64 < (1ll << 31), "byol_conv_wgrad: M out of range");
   // 3x3 / stride 1 / pad 1: shifted-window kernel over TMA patches (no gather)
-  if (!force_gather && ldy == Cout && Hs == Ho && Ws == Wo && patch_wgrad_applicable(Hs, Ws, C, Cin_real, Cout, KH, KW, stride, pad))
+  if (T == 0 && !force_gather && ldy == Cout && Hs == Ho && Ws == Wo && patch_wgrad_applicable(Hs, Ws, C, Cin_real, Cout, KH, KW, stride, pad))
     return patch_wgrad_launch(src, dy, dw, Nimg, Hs, Ws, C, Cout, sm_count(), stream);
+  const int terms = T == 0 ? 1 : T;
   WgradParams p;
   memset(&p, 0, sizeof(p));
+  p.terms = terms;
+  p.ldsrc = C * terms;
+  p.dy_term = ldy;
+  // Term j pairs plane A_PAT[j] of dY (column j of its activation-pattern planes) with plane B_PAT[j] of src, which
+  // its activation-pattern planes hold at column perm[j] (A_PAT[perm[j]] == B_PAT[j], csrc/split.cu).
+  const int perm3[3] = {0, 2, 1}, perm6[6] = {0, 2, 1, 3, 5, 4};
+  for (int j = 0; j < terms; ++j) p.src_term[j] = (T == 3 ? perm3[j] : T == 6 ? perm6[j] : 0) * C;
   p.src = (const bf16*)src;
   p.dw = dw;
   p.Nimg = Nimg; p.Hs = Hs; p.Ws = Ws; p.C = C; p.Ho = Ho; p.Wo = Wo; p.KH = KH; p.KW = KW;
@@ -1089,8 +1146,9 @@ extern "C" int byol_conv_wgrad(const void* src, const void* dy, float* dw, int N
   const int BN = ncols > 64 ? 128 : 64;
   p.tiles_co = (Cout + 127) / 128;
   p.tiles_n = (ncols + BN - 1) / BN;
-  p.num_kb_total = (p.M + WG_KROWS - 1) / WG_KROWS;
-  p.small_src = ((int64_t)Nimg * Hs * Ws * C < (1ll << 31) - (1ll << 24)) ? 1 : 0;
+  p.kb_per_term = (p.M + WG_KROWS - 1) / WG_KROWS;
+  p.num_kb_total = terms * p.kb_per_term;
+  p.small_src = ((int64_t)Nimg * Hs * Ws * p.ldsrc < (1ll << 31) - (1ll << 24)) ? 1 : 0;
   const int taps = KH * KW;
   const int base_ctas = p.tiles_co * p.tiles_n;
   // The epilogue adds 128 x BN values per CTA to the gradient with L2 reductions, so the split count trades
@@ -1109,9 +1167,11 @@ extern "C" int byol_conv_wgrad(const void* src, const void* dy, float* dw, int N
 
   BYOL_CHECK_ARG(!b_tma || C % 8 == 0, "byol_conv_wgrad: bad C");
   CUtensorMap ta, tb;
-  if (make_tmap_2d(&ta, dy, (uint64_t)p.M, (uint64_t)Cout, (uint64_t)ldy, (uint32_t)WG_KROWS) != 0) return -3;
+  // plain operands: the map ends at column Cout (TMA zero-fills a co tile past it); planes: all terms side by side
+  const uint64_t dy_cols = T == 0 ? (uint64_t)Cout : (uint64_t)terms * ldy;
+  if (make_tmap_2d(&ta, dy, (uint64_t)p.M, dy_cols, (uint64_t)terms * ldy, (uint32_t)WG_KROWS) != 0) return -3;
   if (b_tma) {
-    if (make_tmap_2d(&tb, src, (uint64_t)p.M, (uint64_t)C, (uint64_t)C, (uint32_t)WG_KROWS) != 0) return -3;
+    if (make_tmap_2d(&tb, src, (uint64_t)p.M, (uint64_t)p.ldsrc, (uint64_t)p.ldsrc, (uint32_t)WG_KROWS) != 0) return -3;
   } else {
     tb = ta;
   }
@@ -1121,4 +1181,23 @@ extern "C" int byol_conv_wgrad(const void* src, const void* dy, float* dw, int N
   const int rc = BN == 128 ? (b_tma ? launch_wgrad<128, true>(ta, tb, p, grid, stream) : launch_wgrad<128, false>(ta, tb, p, grid, stream))
                            : (b_tma ? launch_wgrad<64, true>(ta, tb, p, grid, stream) : launch_wgrad<64, false>(ta, tb, p, grid, stream));
   return fix_done(stream, rc != 0 ? rc : fix_flush(p.fx, dw, ndw, stream));
+}
+
+extern "C" int byol_conv_wgrad(const void* src, const void* dy, float* dw, int Nimg, int Hs, int Ws, int C,
+                               int Cin_real, int Ho, int Wo, int Cout, int ldy, int KH, int KW, int stride, int pad,
+                               int force_gather, cudaStream_t stream) {
+  return conv_wgrad_impl(src, dy, dw, Nimg, Hs, Ws, C, Cin_real, Ho, Wo, Cout, ldy, KH, KW, stride, pad, force_gather,
+                         0, stream);
+}
+
+// fp32-accurate wgrad: dW (fp32) += sum over the T product terms of dY-plane^T x im2col(src-plane).
+// src: bf16 planes [Nimg, Hs, Ws, T*C], dy: bf16 planes [Nimg, Ho, Wo, T*ldy] (both in the activation pattern of
+// byol_split_planes; ldy >= Cout, a multiple of 8).  All terms accumulate into one fixed-point scratch and reach dw with
+// ONE fp32 addition per element.  Always the gather / TMA kernel (no 3x3 patch kernel); a 7x7 stem over 8 padded
+// channels keeps its folded (kw, c) columns.
+extern "C" int byol_conv_wgrad_planes(const void* src, const void* dy, float* dw, int Nimg, int Hs, int Ws, int C,
+                                      int Cin_real, int Ho, int Wo, int Cout, int ldy, int KH, int KW, int stride,
+                                      int pad, int T, cudaStream_t stream) {
+  BYOL_CHECK_ARG(T == 3 || T == 6, "byol_conv_wgrad_planes: T=%d must be 3 or 6", T);
+  return conv_wgrad_impl(src, dy, dw, Nimg, Hs, Ws, C, Cin_real, Ho, Wo, Cout, ldy, KH, KW, stride, pad, 0, T, stream);
 }

@@ -402,3 +402,274 @@ extern "C" int byol_avgpool_f32(const float* x, float* y, int N, int HW, int C, 
   avgpool_f32_kernel<<<grid_for((int64_t)N * C, 256), 256, 0, stream>>>(x, y, N, HW, C);
   return check_launch("avgpool_f32_kernel");
 }
+
+// =============================================================================================
+// fp32-accurate backward path (BYOL(backward_precision="fp32")): the same split scheme on the backward GEMMs.
+//   dgrad  dX = dY * W^T : dY in activation-pattern planes, W in the dgrad plane layout below (weight pattern)
+//   wgrad  dW = dY^T * X : the planes of dY and X as they are (byol_conv_wgrad_planes pairs the columns)
+// BatchNorm backward reads the fp32 conv output and the fp32 incoming gradient; its per-channel sums are per-block
+// fp64 partials added in block order (same bits in every run, no float atomics).
+// =============================================================================================
+namespace byol {
+
+// fp32 weight [Cout, Cin, taps] -> bf16 [Cin, taps * T * Cout]: column (tap*T + j)*Cout + co = plane B_PAT[j] of
+// w[co, ci, tap] (the dgrad layout of byol_prep_weight with T planes per output channel)
+__global__ void prep_weight_dgrad_planes_kernel(const float* __restrict__ w, bf16* __restrict__ out, int Cout, int Cin,
+                                                int taps, SplitPattern pat) {
+  const int64_t total = (int64_t)Cin * taps * Cout;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int co = (int)(i % Cout);
+    int64_t t = i / Cout;
+    const int tap = (int)(t % taps);
+    const int64_t ci = t / taps;
+    bf16 pl[3];
+    split3(w[((int64_t)co * Cin + ci) * taps + tap], pl);
+    bf16* o = out + (ci * taps + tap) * (int64_t)pat.T * Cout + co;
+#pragma unroll
+    for (int j = 0; j < 6; ++j)
+      if (j < pat.T) o[(int64_t)j * Cout] = pl[pat.b[j]];
+  }
+}
+
+// dz = g masked by the ReLU of the BatchNorm output: MASK 0 none, 1 (y*scale + shift) > 0, 3 bit of the mask bytes
+template <int MASK>
+__device__ __forceinline__ float bwd_mask(float g, float y, const uint8_t* mask, int64_t e, float sc, float sh) {
+  if (MASK == 1) return (y * sc + sh) > 0.f ? g : 0.f;
+  if (MASK == 3) return ((__ldg(mask + (e >> 3)) >> (e & 7)) & 1u) ? g : 0.f;
+  return g;
+}
+
+// part[block][0:C] = sum dz, part[block][C:2C] = sum dz * xhat over this block's rows (fp64); layout of stats_f32_kernel
+template <int MASK>
+__global__ void bn_bwd_reduce_f32_kernel(const float* __restrict__ g, const float* __restrict__ y,
+                                         const uint8_t* __restrict__ mask, const float* __restrict__ scale,
+                                         const float* __restrict__ shift, const float* __restrict__ mean,
+                                         const float* __restrict__ invstd, double* __restrict__ part, int64_t M, int C,
+                                         int CT, int64_t rows_per_block) {
+  const int col = blockIdx.y * CT + (int)(threadIdx.x % CT);
+  const int rlane = (int)(threadIdx.x / CT);
+  const int lanes = (int)(blockDim.x / CT);
+  const int64_t r0 = blockIdx.x * rows_per_block;
+  int64_t r1 = r0 + rows_per_block;
+  if (r1 > M) r1 = M;
+  double s = 0.0, q = 0.0;
+  if (col < C) {
+    const float sc = MASK == 1 ? scale[col] : 0.f, sh = MASK == 1 ? shift[col] : 0.f;
+    const double mu = (double)mean[col], is = (double)invstd[col];
+    for (int64_t r = r0 + rlane; r < r1; r += lanes) {
+      const int64_t e = r * C + col;
+      const float yv = y[e];
+      const double dz = (double)bwd_mask<MASK>(g[e], yv, mask, e, sc, sh);
+      s += dz;
+      q += dz * (((double)yv - mu) * is);
+    }
+  }
+  __shared__ double sh[2][256];
+  sh[0][threadIdx.x] = s;
+  sh[1][threadIdx.x] = q;
+  __syncthreads();
+  if (rlane == 0 && col < C) {
+    for (int l = 1; l < lanes; ++l) {
+      s += sh[0][l * CT + (threadIdx.x % CT)];
+      q += sh[1][l * CT + (threadIdx.x % CT)];
+    }
+    part[(int64_t)blockIdx.x * 2 * C + col] = s;
+    part[(int64_t)blockIdx.x * 2 * C + C + col] = q;
+  }
+}
+
+// 8 fp32 values of one row -> their T activation-pattern planes at base (plane stride C elements)
+__device__ __forceinline__ void store_planes8(bf16* base, int C, const float (&o)[8], const SplitPattern& pat) {
+  bf16 pl[8][3];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) split3(o[e], pl[e]);
+#pragma unroll
+  for (int j = 0; j < 6; ++j) {
+    if (j < pat.T) {
+      const int a = pat.a[j];
+      uint4 q;
+      __nv_bfloat162 h0 = __halves2bfloat162(pl[0][a], pl[1][a]), h1 = __halves2bfloat162(pl[2][a], pl[3][a]);
+      __nv_bfloat162 h2 = __halves2bfloat162(pl[4][a], pl[5][a]), h3 = __halves2bfloat162(pl[6][a], pl[7][a]);
+      q.x = *reinterpret_cast<uint32_t*>(&h0);
+      q.y = *reinterpret_cast<uint32_t*>(&h1);
+      q.z = *reinterpret_cast<uint32_t*>(&h2);
+      q.w = *reinterpret_cast<uint32_t*>(&h3);
+      *reinterpret_cast<uint4*>(base + (int64_t)j * C) = q;
+    }
+  }
+}
+
+// dy = gamma*invstd*(dz - s1/n - xhat*s2/n) on fp32 [M, C] -> planes (bf16 [M, T*C]) and / or fp32 dy; optional fp32
+// dz (the residual branch's gradient).  Block 0 adds the rank-local sums to dgamma / dbeta: plain read-modify-write,
+// the lanes of one layer are launched one after another on one stream.  One thread per 8 consecutive channels.
+template <int MASK>
+__global__ void bn_bwd_apply_f32_kernel(const float* __restrict__ g, const float* __restrict__ y,
+                                        const uint8_t* __restrict__ mask, const float* __restrict__ scale,
+                                        const float* __restrict__ shift, const float* __restrict__ mean,
+                                        const float* __restrict__ invstd, const float* __restrict__ gamma,
+                                        const double* __restrict__ s12, double inv_count, bf16* __restrict__ planes,
+                                        float* __restrict__ dy32, float* __restrict__ dz_out, int64_t nvec, int C,
+                                        SplitPattern pat, const double* __restrict__ s12_local,
+                                        float* __restrict__ dgamma, float* __restrict__ dbeta) {
+  if (blockIdx.x == 0 && dgamma != nullptr) {
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
+      dgamma[c] += (float)s12_local[C + c];
+      dbeta[c] += (float)s12_local[c];
+    }
+  }
+  const int groups = C >> 3;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < nvec; i += (int64_t)gridDim.x * blockDim.x) {
+    const int gi = (int)(i % groups);
+    const int64_t m = i / groups;
+    const float4 g0 = __ldg(reinterpret_cast<const float4*>(g) + 2 * i);
+    const float4 g1 = __ldg(reinterpret_cast<const float4*>(g) + 2 * i + 1);
+    const float4 y0 = __ldg(reinterpret_cast<const float4*>(y) + 2 * i);
+    const float4 y1 = __ldg(reinterpret_cast<const float4*>(y) + 2 * i + 1);
+    const float gv[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
+    const float yv[8] = {y0.x, y0.y, y0.z, y0.w, y1.x, y1.y, y1.z, y1.w};
+    float dz[8], o[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int c = gi * 8 + e;
+      const float sc = MASK == 1 ? __ldg(scale + c) : 0.f, sh = MASK == 1 ? __ldg(shift + c) : 0.f;
+      dz[e] = bwd_mask<MASK>(gv[e], yv[e], mask, 8 * i + e, sc, sh);
+      const float is = __ldg(invstd + c);
+      const float xhat = (yv[e] - __ldg(mean + c)) * is;
+      const float k1 = (float)(s12[c] * inv_count), k2 = (float)(s12[C + c] * inv_count);
+      o[e] = __ldg(gamma + c) * is * (dz[e] - k1 - xhat * k2);
+    }
+    if (planes != nullptr) store_planes8(planes + m * (int64_t)pat.T * C + gi * 8, C, o, pat);
+    if (dy32 != nullptr) {
+      reinterpret_cast<float4*>(dy32)[2 * i] = make_float4(o[0], o[1], o[2], o[3]);
+      reinterpret_cast<float4*>(dy32)[2 * i + 1] = make_float4(o[4], o[5], o[6], o[7]);
+    }
+    if (dz_out != nullptr) {
+      reinterpret_cast<float4*>(dz_out)[2 * i] = make_float4(dz[0], dz[1], dz[2], dz[3]);
+      reinterpret_cast<float4*>(dz_out)[2 * i + 1] = make_float4(dz[4], dz[5], dz[6], dz[7]);
+    }
+  }
+}
+
+// max-pool backward over fp32 NHWC with the window positions maxpool_f32 wrote: every input pixel gathers the
+// gradients of the windows that chose it (fixed order, no atomics)
+__global__ void maxpool_bwd_f32_kernel(const float* __restrict__ dy, const uint8_t* __restrict__ idx,
+                                       float* __restrict__ dx, int N, int H, int W, int C, int Ho, int Wo, int k, int s,
+                                       int p) {
+  const int64_t total = (int64_t)N * H * W * C;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    int64_t t = i / C;
+    const int iw = (int)(t % W); t /= W;
+    const int ih = (int)(t % H);
+    const int n = (int)(t / H);
+    float acc = 0.f;
+    for (int kh = (ih + p) % s; kh < k; kh += s) {
+      const int oh = (ih + p - kh) / s;
+      if (oh < 0 || oh >= Ho) continue;
+      for (int kw = (iw + p) % s; kw < k; kw += s) {
+        const int ow = (iw + p - kw) / s;
+        if (ow < 0 || ow >= Wo) continue;
+        const int64_t o = (((int64_t)n * Ho + oh) * Wo + ow) * C + c;
+        if ((int)idx[o] == kh * k + kw) acc += dy[o];
+      }
+    }
+    dx[i] = acc;
+  }
+}
+
+// dx[n, r, c] = (ga[n, c] + gb[n, c]) / HW   (either gradient may be absent)
+__global__ void avgpool_bwd_f32_kernel(const float* __restrict__ ga, const float* __restrict__ gb,
+                                       float* __restrict__ dx, int N, int HW, int C) {
+  const int64_t total = (int64_t)N * HW * C;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    const int64_t n = i / ((int64_t)HW * C);
+    const float a = ga != nullptr ? ga[n * C + c] : 0.f;
+    const float b = gb != nullptr ? gb[n * C + c] : 0.f;
+    dx[i] = (ga != nullptr && gb != nullptr ? a + b : (ga != nullptr ? a : b)) / (float)HW;
+  }
+}
+
+}  // namespace byol
+
+extern "C" int byol_prep_weight_dgrad_planes(const float* w, void* out, int Cout, int Cin, int taps, int T,
+                                             cudaStream_t stream) {
+  BYOL_CHECK_ARG(w && out && Cout > 0 && Cin > 0 && taps > 0, "byol_prep_weight_dgrad_planes: bad args");
+  BYOL_CHECK_T(T);
+  prep_weight_dgrad_planes_kernel<<<grid_for((int64_t)Cin * taps * Cout, 256), 256, 0, stream>>>(
+      w, (bf16*)out, Cout, Cin, taps, make_pattern(T));
+  return check_launch("prep_weight_dgrad_planes_kernel");
+}
+
+// s12 (fp64 [2C], accumulated): += [sum dz, sum dz * xhat] over the rows of g / y (fp32 [M, C])
+extern "C" int byol_bn_bwd_reduce_f32(const float* g, const float* y, const void* mask, const float* scale,
+                                      const float* shift, const float* mean, const float* invstd, double* s12,
+                                      int64_t M, int C, int mask_mode, cudaStream_t stream) {
+  BYOL_CHECK_ARG(g && y && mean && invstd && s12 && M > 0 && C > 0, "byol_bn_bwd_reduce_f32: bad args");
+  BYOL_CHECK_ARG((mask_mode == 0) || (mask_mode == 1 && scale && shift) || (mask_mode == 3 && mask),
+                 "byol_bn_bwd_reduce_f32: bad mask_mode %d", mask_mode);
+  int CT = 1;
+  while (CT < C && CT < 256) CT <<= 1;
+  const int lanes = 256 / CT;
+  int64_t rows_per_block = (M + 132 * 4 - 1) / (132 * 4);
+  if (rows_per_block < 4 * lanes) rows_per_block = 4 * lanes;
+  dim3 grid((unsigned)((M + rows_per_block - 1) / rows_per_block), (unsigned)((C + CT - 1) / CT));
+  Fix128* scratch = fix_scratch(stream, ((int64_t)grid.x * C * 2 + 2) / 3);
+  if (scratch == nullptr) return -2;
+  double* part = reinterpret_cast<double*>(scratch);
+  const uint8_t* mk = (const uint8_t*)mask;
+  if (mask_mode == 0)
+    bn_bwd_reduce_f32_kernel<0><<<grid, 256, 0, stream>>>(g, y, mk, scale, shift, mean, invstd, part, M, C, CT, rows_per_block);
+  else if (mask_mode == 1)
+    bn_bwd_reduce_f32_kernel<1><<<grid, 256, 0, stream>>>(g, y, mk, scale, shift, mean, invstd, part, M, C, CT, rows_per_block);
+  else
+    bn_bwd_reduce_f32_kernel<3><<<grid, 256, 0, stream>>>(g, y, mk, scale, shift, mean, invstd, part, M, C, CT, rows_per_block);
+  if (check_launch("bn_bwd_reduce_f32_kernel") != 0) return -100;
+  stats_f32_sum_kernel<<<(2 * C + 255) / 256, 256, 0, stream>>>(part, s12, (int)grid.x, 2 * C);
+  return fix_done(stream, check_launch("stats_f32_sum_kernel"));
+}
+
+// s12: global (cross-rank) sums over `count` rows; s12_local (optional, default s12): this rank's sums for dgamma/dbeta
+extern "C" int byol_bn_bwd_apply_f32(const float* g, const float* y, const void* mask, const float* scale,
+                                     const float* shift, const float* mean, const float* invstd, const float* gamma,
+                                     const double* s12, const double* s12_local, double count, void* planes,
+                                     float* dy32, float* dz_out, float* dgamma, float* dbeta, int64_t M, int C,
+                                     int mask_mode, int T, cudaStream_t stream) {
+  BYOL_CHECK_ARG(g && y && mean && invstd && gamma && s12 && count > 0 && M > 0 && C % 8 == 0 && (planes || dy32),
+                 "byol_bn_bwd_apply_f32: bad args");
+  BYOL_CHECK_ARG((mask_mode == 0) || (mask_mode == 1 && scale && shift) || (mask_mode == 3 && mask),
+                 "byol_bn_bwd_apply_f32: bad mask_mode %d", mask_mode);
+  BYOL_CHECK_ARG((dgamma == nullptr) == (dbeta == nullptr), "byol_bn_bwd_apply_f32: need dgamma and dbeta or neither");
+  BYOL_CHECK_T(T);
+  if (s12_local == nullptr) s12_local = s12;
+  const int64_t nvec = M * C / 8;
+  const uint8_t* mk = (const uint8_t*)mask;
+  const SplitPattern pat = make_pattern(T);
+  const int grid = grid_for(nvec, 256);
+  if (mask_mode == 0)
+    bn_bwd_apply_f32_kernel<0><<<grid, 256, 0, stream>>>(g, y, mk, scale, shift, mean, invstd, gamma, s12, 1.0 / count,
+                                                         (bf16*)planes, dy32, dz_out, nvec, C, pat, s12_local, dgamma, dbeta);
+  else if (mask_mode == 1)
+    bn_bwd_apply_f32_kernel<1><<<grid, 256, 0, stream>>>(g, y, mk, scale, shift, mean, invstd, gamma, s12, 1.0 / count,
+                                                         (bf16*)planes, dy32, dz_out, nvec, C, pat, s12_local, dgamma, dbeta);
+  else
+    bn_bwd_apply_f32_kernel<3><<<grid, 256, 0, stream>>>(g, y, mk, scale, shift, mean, invstd, gamma, s12, 1.0 / count,
+                                                         (bf16*)planes, dy32, dz_out, nvec, C, pat, s12_local, dgamma, dbeta);
+  return check_launch("bn_bwd_apply_f32_kernel");
+}
+
+extern "C" int byol_maxpool_bwd_f32(const float* dy, const void* idx, float* dx, int N, int H, int W, int C, int k,
+                                    int s, int p, cudaStream_t stream) {
+  BYOL_CHECK_ARG(dy && idx && dx && N > 0 && C > 0 && k * k <= 255 && s > 0, "byol_maxpool_bwd_f32: bad args");
+  const int Ho = (H + 2 * p - k) / s + 1, Wo = (W + 2 * p - k) / s + 1;
+  maxpool_bwd_f32_kernel<<<grid_for((int64_t)N * H * W * C, 256), 256, 0, stream>>>(dy, (const uint8_t*)idx, dx, N, H,
+                                                                                     W, C, Ho, Wo, k, s, p);
+  return check_launch("maxpool_bwd_f32_kernel");
+}
+
+extern "C" int byol_avgpool_bwd_f32(const float* ga, const float* gb, float* dx, int N, int HW, int C,
+                                    cudaStream_t stream) {
+  BYOL_CHECK_ARG((ga || gb) && dx && N > 0 && HW > 0 && C > 0, "byol_avgpool_bwd_f32: bad args");
+  avgpool_bwd_f32_kernel<<<grid_for((int64_t)N * HW * C, 256), 256, 0, stream>>>(ga, gb, dx, N, HW, C);
+  return check_launch("avgpool_bwd_f32_kernel");
+}

@@ -90,9 +90,10 @@ class _Weights(object):
 
 class _SplitWeights(object):
     """Weight-side plane layouts of one parameter set for the fp32-accurate forward path (csrc/split.cu):
-    per conv / linear a bf16 [Cout, taps * T * Cpad] matrix."""
+    per conv / linear a bf16 [Cout, taps * T * Cpad] matrix; with want_dgrad (fp32-accurate backward, online set) also
+    the dgrad layout [Cin, taps * T * Cout] of every layer whose input gradient is needed."""
 
-    def __init__(self, units, device, T):
+    def __init__(self, units, device, T, want_dgrad=False):
         self.T = T
         sizes = [u.cout * u.k * u.k * T * u.cpad for u in units]
         self.pool = torch.empty(sum(sizes), dtype=BF16, device=device)
@@ -100,11 +101,22 @@ class _SplitWeights(object):
         for u, n in zip(units, sizes):
             self.w.append(self.pool[off:off + n].view(u.cout, u.k * u.k * T * u.cpad))
             off += n
+        self.wd = [None] * len(units)
+        if want_dgrad:
+            dsizes = [u.cin * u.k * u.k * T * u.cout if u.want_dgrad else 0 for u in units]
+            self.pool_d = torch.empty(sum(dsizes), dtype=BF16, device=device)
+            off = 0
+            for u, n in zip(units, dsizes):
+                if n:
+                    self.wd[u.idx] = self.pool_d[off:off + n].view(u.cin, u.k * u.k * T * u.cout)
+                off += n
 
     def prepare(self, units, flat):
         for u in units:
             w = flat[u.w_off:u.w_off + u.w_numel].view(u.cout, u.cin, u.k * u.k)
             ops.prep_weight_planes(w, self.T, u.cpad, self.w[u.idx])
+            if self.wd[u.idx] is not None:
+                ops.prep_weight_dgrad_planes(w, self.T, self.wd[u.idx])
 
 
 class _Pool(object):
@@ -124,7 +136,7 @@ class _Pool(object):
 class _GraphedStep(object):
     """One captured training step: fixed buffers + the forward / backward CUDA graphs (see Engine.graphed_step)."""
     __slots__ = ("inputs", "saved", "outs", "logits", "d_pred", "fwd", "bwd", "pool", "fwd_launches", "bwd_launches",
-                 "mean_ptr", "pending")
+                 "mean_ptr", "pending", "cls_planes")
 
 
 class Engine(object):
@@ -149,6 +161,10 @@ class Engine(object):
         # forward precision: 0 = bf16 operands (fast path); 3 / 6 = fp32 operands split into 3 / 6 bf16 product
         # terms (~16 / 24 mantissa bits), fp32 conv outputs, fp64 BatchNorm statistics (csrc/split.cu)
         self.T = 0
+        # backward precision: False = bf16 operands; True (needs T) = the split scheme on every backward GEMM, fp32
+        # gradients between layers, fp64 BatchNorm-backward sums (_backward_group_split)
+        self.bwd32 = False
+        self.cls_planes = None
         self.s_online = self.s_target = None
         # block-output BatchNorm fused into the expanding 1x1 GEMMs (see _fuse3).  OFF by default: the statistics pass
         # re-runs the GEMM, so the fused form moves more work than the unfused conv + BN-apply kernels
@@ -299,7 +315,7 @@ class Engine(object):
         self.graphs = {}           # captured steps point into the old buffers
         self.s_online = self.s_target = None
         if self.T:
-            self.s_online = _SplitWeights(self.units, self.device, self.T)
+            self.s_online = _SplitWeights(self.units, self.device, self.T, want_dgrad=self.bwd32)
             self.s_target = _SplitWeights(self.units, self.device, self.T)
         self.ready = True
 
@@ -682,14 +698,16 @@ class Engine(object):
                                    bn.running_var, bn.eps, coeffs[i])
         return ys, coeffs
 
-    def _act_split(self, y, c, keep, resid=None, rc=None, block_out=False):
-        """BN-apply (+ residual) + ReLU of one lane's fp32 conv output -> (fp32 | None, planes NHWC, bf16 copy, mask)."""
+    def _act_split(self, y, c, keep, resid=None, rc=None, block_out=False, want_mask=None):
+        """BN-apply (+ residual) + ReLU of one lane's fp32 conv output -> (fp32 | None, planes NHWC, bf16 copy, mask).
+        keep: write the bf16 copy; want_mask (default keep): the ReLU mask bits of a block output."""
         C = y.shape[-1]
+        want_mask = keep if want_mask is None else want_mask
         o32, pl, cp, mask = ops.bn_apply_f32(y.view(-1, C), c[0], c[1], True, self.T,
                                              resid=None if resid is None else resid.view(-1, C),
                                              rscale=None if rc is None else rc[0],
                                              rshift=None if rc is None else rc[1], want_out32=block_out,
-                                             want_planes=True, want_copy=keep, want_mask=keep and block_out)
+                                             want_planes=True, want_copy=keep, want_mask=want_mask and block_out)
         shp = tuple(y.shape[:-1])
         return (None if o32 is None else o32.view(shp + (C,)), pl.view(shp + (self.T * C,)),
                 None if cp is None else cp.view(shp + (C,)), mask)
@@ -697,7 +715,9 @@ class Engine(object):
     def _block_fwd_split(self, b, X, lanes, train):
         """X: per lane (fp32 block input, its planes, its bf16 copy or None)."""
         L = len(lanes)
-        keep = [lanes[i][2] is not None for i in range(L)]
+        save = [lanes[i][2] is not None for i in range(L)]
+        # bf16 copies only for the bf16 backward; the fp32 backward keeps the fp32 tensors and recomputes the planes
+        keep = [s and not self.bwd32 for s in save]
         xs_p = [x[1] for x in X]
         y1, c1 = self._conv_bn_split(b.c1, xs_p, lanes, train)
         a1 = [self._act_split(y1[i], c1[i], keep[i]) for i in range(L)]
@@ -711,13 +731,19 @@ class Engine(object):
             ylast, clast = y2, c2
         if b.down is not None:
             yd, cd = self._conv_bn_split(b.down, xs_p, lanes, train)
-            outs = [self._act_split(ylast[i], clast[i], keep[i], resid=yd[i], rc=cd[i], block_out=True)
-                    for i in range(L)]
+            outs = [self._act_split(ylast[i], clast[i], keep[i], resid=yd[i], rc=cd[i], block_out=True,
+                                    want_mask=save[i]) for i in range(L)]
         else:
             yd, cd = None, None
-            outs = [self._act_split(ylast[i], clast[i], keep[i], resid=X[i][0], block_out=True) for i in range(L)]
+            outs = [self._act_split(ylast[i], clast[i], keep[i], resid=X[i][0], block_out=True, want_mask=save[i])
+                    for i in range(L)]
         for i, (_, _, saved) in enumerate(lanes):
-            if saved is not None:
+            if saved is not None and self.bwd32:
+                saved["blocks"].append({
+                    "mask": outs[i][3], "x": X[i][0], "y1": y1[i], "c1": c1[i], "y2": y2[i], "c2": c2[i],
+                    "y3": y3[i] if y3 is not None else None, "c3": c3[i] if c3 is not None else None,
+                    "yd": yd[i] if yd is not None else None, "cd": cd[i] if cd is not None else None})
+            elif saved is not None:
                 cb = ops.cast_bf16
                 saved["blocks"].append({
                     "mask": outs[i][3], "xsub": None, "x": X[i][2], "y1": cb(y1[i]), "c1": c1[i], "a1": a1[i][2],
@@ -728,7 +754,7 @@ class Engine(object):
         return [(o[0], o[1], o[2]) for o in outs]
 
     def _mlp_fwd_split(self, mlp, X, lanes, train, key):
-        """X: per lane (planes [b, T*in], bf16 copy [b, in]); returns fp32 outputs [b, out]."""
+        """X: per lane (planes [b, T*in], bf16 copy [b, in] | None, fp32 [b, in]); returns fp32 outputs [b, out]."""
         l1, l2 = mlp
         L = len(lanes)
         h, c = self._conv_bn_split(l1, [x[0] for x in X], lanes, train)
@@ -736,9 +762,11 @@ class Engine(object):
         for i, (flat, _, saved) in enumerate(lanes):
             wset = self.s_online if flat is self.theta else self.s_target
             _, ap, ab, _ = ops.bn_apply_f32(h[i], c[i][0], c[i][1], True, self.T, want_planes=True,
-                                            want_copy=saved is not None)
+                                            want_copy=saved is not None and not self.bwd32)
             outs.append(ops.linear_fprop(ap, wset.w[l2.idx], bias=flat[l2.b_off:l2.b_off + l2.cout], out_fp32=True))
-            if saved is not None:
+            if saved is not None and self.bwd32:
+                saved[key] = {"x": X[i][2], "h": h[i], "c": c[i]}
+            elif saved is not None:
                 saved[key] = {"x": X[i][1], "h": ops.cast_bf16(h[i]), "c": c[i], "a": ab}
         return outs
 
@@ -753,10 +781,13 @@ class Engine(object):
             a0, _, _, _ = ops.bn_apply_f32(y0[i].view(-1, C), c0[i][0], c0[i][1], True, T, want_out32=True,
                                            want_planes=False)
             p32, idx = ops.maxpool_f32(a0.view(y0[i].shape), self.pool_k, self.pool_s, self.pool_p, want_idx=keep[i])
-            pl, cp = ops.split_planes(p32.view(-1, C), T, want_copy=keep[i])
+            pl, cp = ops.split_planes(p32.view(-1, C), T, want_copy=keep[i] and not self.bwd32)
             shp = tuple(p32.shape[:-1])
             X.append((p32, pl.view(shp + (T * C,)), None if cp is None else cp.view(shp + (C,))))
-            if saved is not None:
+            if saved is not None and self.bwd32:
+                saved.update({"x8": x8[i][4], "y0": y0[i], "c0": c0[i], "a0_shape": tuple(y0[i].shape),
+                              "pool_idx": idx, "blocks": []})
+            elif saved is not None:
                 saved.update({"x8": x8[i][0] if x8[i][1] is None else (x8[i][1], x8[i][2], x8[i][3]),
                               "y0": ops.cast_bf16(y0[i]), "c0": c0[i], "a0_shape": tuple(y0[i].shape),
                               "pool_idx": idx, "blocks": []})
@@ -769,11 +800,11 @@ class Engine(object):
             pl, cp = ops.split_planes(rep, T, want_copy=True, copy_out=rep_bf16_out[i])
             reps_f.append(rep)
             reps_b.append(cp)
-            M.append((pl, cp))
+            M.append((pl, cp, rep))
             if keep[i]:
                 lanes[i][2]["final_shape"] = (n, h, w, c)
         proj = self._mlp_fwd_split(self.mlps[0], M, lanes, train, "head")
-        M2 = [ops.split_planes(p, T, want_copy=keep[i]) for i, p in enumerate(proj)]
+        M2 = [ops.split_planes(p, T, want_copy=keep[i] and not self.bwd32) + (p,) for i, p in enumerate(proj)]
         pred = self._mlp_fwd_split(self.mlps[1], M2, lanes, train, "pred")
         return [(reps_f[i], proj[i], pred[i]) for i in range(L)], reps_b
 
@@ -807,20 +838,22 @@ class Engine(object):
             dzs.append(dz)
         return dys, dzs
 
-    def _wgrad(self, u, xs, dys, unit_stride=None):
+    def _wgrad(self, u, xs, dys, unit_stride=None, planes=False):
         """dW += dY^T * im2col(X) on the side stream: the weight-gradient GEMMs only feed the flat gradient buffer, so
-        they overlap with the HBM-bound BatchNorm-backward kernels of the next layer on the main stream."""
+        they overlap with the HBM-bound BatchNorm-backward kernels of the next layer on the main stream.
+        planes: xs / dys are split-operand planes (fp32-accurate backward)."""
         dw = self._gview(u.w_off, u.w_numel).view(u.cout, u.cin, u.k, u.k)
+        launch = self._launch_wgrad_planes if planes else self._launch_wgrad
         main = torch.cuda.current_stream()
         side = self._side_stream
         if side is None:
-            self._launch_wgrad(u, xs, dys, dw, unit_stride)
+            launch(u, xs, dys, dw, unit_stride)
             return
         ev = torch.cuda.Event()
         ev.record(main)
         side.wait_event(ev)
         with torch.cuda.stream(side):
-            self._launch_wgrad(u, xs, dys, dw, unit_stride)
+            launch(u, xs, dys, dw, unit_stride)
         # keep the operands alive until the launching stream has joined the side stream (no record_stream: that would
         # add an allocator event per tensor); after the join, reuse by the owning stream is ordered behind the reads
         self._side_refs.append((xs, dys))
@@ -834,6 +867,14 @@ class Engine(object):
                 ops.conv_wgrad(x.view(x.shape[0], 1, 1, -1), dy.view(dy.shape[0], 1, 1, -1), dw, 1, 1, 1, 0)
             else:
                 ops.conv_wgrad(x, dy, dw, u.k, u.k, unit_stride or u.stride, u.pad)
+
+    def _launch_wgrad_planes(self, u, xps, dyps, dw, unit_stride=None):
+        for xp, dyp in zip(xps, dyps):
+            if u.kind == "linear":
+                ops.conv_wgrad_planes(xp.view(xp.shape[0], 1, 1, -1), dyp.view(dyp.shape[0], 1, 1, -1), dw, 1, 1, 1, 0,
+                                      self.T)
+            else:
+                ops.conv_wgrad_planes(xp, dyp, dw, u.k, u.k, u.stride, u.pad, self.T)
 
     def _join_side_stream(self):
         if self._side_stream is not None and self._side_used:
@@ -976,6 +1017,150 @@ class Engine(object):
         self._wgrad(l1, [s["x"] for s in S], dhs)
         return [ops.linear_dgrad(dhs[i], self.w_online.wd[l1.idx]) for i in range(L)]
 
+    # ------------------------------------------------------------------------------------------
+    # fp32-accurate backward (backward_precision="fp32"): the layer walk of _backward_group with the split scheme on
+    # every GEMM (dY planes x weight planes for dgrad, dY planes x input planes for wgrad, T product terms, fp32
+    # outputs), fp32 gradients between layers and fp64 BatchNorm-backward sums.  The online views run lock-step on
+    # the caller's stream (like the split forward), not on one stream each as in the bf16 backward: dgamma / dbeta
+    # then get the fp64 sum over both views with one rounding and no atomics, at the cost of the view-level overlap.
+    # The weight gradients run on the side stream, joined after every block so that the recomputed planes they read
+    # are freed block by block.
+    # ------------------------------------------------------------------------------------------
+    def _bn_bwd_f32(self, u, gs, ys, cs, mask_mode, masks=None, want_dz=False, want_f32=False):
+        """-> per lane (dy planes, fp32 dy | None, fp32 dz | None)."""
+        L, C = len(gs), u.cout
+        s12 = torch.zeros(L * 2 * C, dtype=torch.float64, device=self.device)
+        for i in range(L):
+            ops.bn_bwd_reduce_f32(gs[i].view(-1, C), ys[i].view(-1, C), cs[i], s12[i * 2 * C:(i + 1) * 2 * C],
+                                  mask_mode, mask=None if masks is None else masks[i])
+        count, local = ys[0].numel() // C, None
+        if self.sync and self.world() > 1:
+            local = torch.empty_like(s12)
+            comm.allreduce_sum_(s12, local_out=local)
+            count *= self.world()
+        gamma = self.theta[u.g_off:u.g_off + C]
+        # dgamma / dbeta: the lanes' rank-local fp64 sums are added first, so the flat gradient takes ONE fp32 rounding
+        # (by the last lane's apply kernel)
+        loc = (s12 if local is None else local).view(L, 2 * C)
+        loc = loc[0] if L == 1 else loc.sum(0)
+        res = []
+        for i in range(L):
+            sl = slice(i * 2 * C, (i + 1) * 2 * C)
+            last = i == L - 1
+            pl, d32, dz = ops.bn_bwd_apply_f32(gs[i].view(-1, C), ys[i].view(-1, C), cs[i], gamma, s12[sl], count,
+                                               mask_mode, self.T, mask=None if masks is None else masks[i],
+                                               want_f32=want_f32, want_dz=want_dz, s12_local=loc if last else None,
+                                               dgamma=self._gview(u.g_off, C) if last else None,
+                                               dbeta=self._gview(u.beta_off, C) if last else None)
+            shp = tuple(ys[i].shape[:-1])
+            res.append((pl.view(shp + (self.T * C,)), d32, None if dz is None else dz.view(ys[i].shape)))
+        return res
+
+    def _planes(self, x):
+        """fp32 [..., C] -> activation-pattern planes [..., T*C]."""
+        C = x.shape[-1]
+        return ops.split_planes(x.reshape(-1, C), self.T)[0].view(tuple(x.shape[:-1]) + (self.T * C,))
+
+    def _act_planes(self, y, c):
+        """relu(bn(y)) of a saved fp32 conv output, recomputed as planes (the input of the next layer)."""
+        C = y.shape[-1]
+        return ops.bn_apply_f32(y.view(-1, C), c[0], c[1], True, self.T)[1].view(tuple(y.shape[:-1]) + (self.T * C,))
+
+    def _wgrad_split(self, u, xps, dyps):
+        self._wgrad(u, xps, dyps, planes=True)
+
+    def _dgrad_split(self, u, dyps, in_shapes, resids=None):
+        wd = self.s_online.wd[u.idx]
+        return [ops.conv_dgrad_planes(dyp, wd, in_shapes[i][1], in_shapes[i][2], u.k, u.k, u.stride, u.pad, self.T,
+                                      resid=None if resids is None else resids[i]) for i, dyp in enumerate(dyps)]
+
+    def _block_bwd_split(self, b, S, gs):
+        """gs: per lane fp32 gradient of the block output; returns the fp32 gradient of the block input."""
+        xs = [s["x"] for s in S]
+        xshapes = [tuple(x.shape) for x in xs]
+        xps = [self._planes(x) for x in xs]
+        last = b.c3 if b.kind == "bottleneck" else b.c2
+        key = "3" if b.kind == "bottleneck" else "2"
+        masks = [s["mask"] for s in S]
+        rl = self._bn_bwd_f32(last, gs, [s["y" + key] for s in S], [s["c" + key] for s in S], 3, masks=masks,
+                              want_dz=b.down is None)
+        dyl = [r[0] for r in rl]
+        if b.down is not None:
+            dyd = [r[0] for r in self._bn_bwd_f32(b.down, gs, [s["yd"] for s in S], [s["cd"] for s in S], 3,
+                                                  masks=masks)]
+            self._wgrad_split(b.down, xps, dyd)
+            resid = self._dgrad_split(b.down, dyd, xshapes)
+        else:
+            resid = [r[2] for r in rl]
+        if b.kind == "bottleneck":
+            a2 = [self._act_planes(s["y2"], s["c2"]) for s in S]
+            self._wgrad_split(b.c3, a2, dyl)
+            g2 = self._dgrad_split(b.c3, dyl, [tuple(s["y2"].shape) for s in S])
+            dy2 = [r[0] for r in self._bn_bwd_f32(b.c2, g2, [s["y2"] for s in S], [s["c2"] for s in S], 1)]
+        else:
+            dy2 = dyl
+        a1 = [self._act_planes(s["y1"], s["c1"]) for s in S]
+        self._wgrad_split(b.c2, a1, dy2)
+        g1 = self._dgrad_split(b.c2, dy2, [tuple(s["y1"].shape) for s in S])
+        dy1 = [r[0] for r in self._bn_bwd_f32(b.c1, g1, [s["y1"] for s in S], [s["c1"] for s in S], 1)]
+        self._wgrad_split(b.c1, xps, dy1)
+        out = self._dgrad_split(b.c1, dy1, xshapes, resids=resid)
+        self._join_side_stream()
+        return out
+
+    def _mlp_bwd_split(self, mlp, S, douts):
+        """douts: per lane fp32 [b, out] gradient of the MLP output; returns fp32 grads of its input."""
+        l1, l2 = mlp
+        L, T = len(S), self.T
+        dps = []
+        for i in range(L):
+            ops.col_sum(douts[i], self._gview(l2.b_off, l2.cout))
+            dps.append(ops.split_planes(douts[i], T)[0])
+        self._wgrad_split(l2, [self._act_planes(s["h"], s["c"]) for s in S], dps)
+        das = [ops.linear_dgrad_planes(dps[i], self.s_online.wd[l2.idx], T) for i in range(L)]
+        rh = self._bn_bwd_f32(l1, das, [s["h"] for s in S], [s["c"] for s in S], 1, want_f32=True)
+        for i in range(L):
+            ops.col_sum(rh[i][1], self._gview(l1.b_off, l1.cout))
+        dhs = [r[0] for r in rh]
+        self._wgrad_split(l1, [self._planes(s["x"]) for s in S], dhs)
+        out = [ops.linear_dgrad_planes(dhs[i], self.s_online.wd[l1.idx], T) for i in range(L)]
+        self._join_side_stream()
+        return out
+
+    def _backward_group_split(self, saved, d_reps, d_projs, d_preds):
+        L = len(saved)
+        if all(d is None for d in d_preds) and all(d is None for d in d_projs) and all(d is None for d in d_reps):
+            return
+        zero = lambda ref: torch.zeros_like(ref)
+        head_in = None
+        if any(d is not None for d in d_preds):
+            ref = [d for d in d_preds if d is not None][0]
+            dq = [(d if d is not None else zero(ref)).contiguous() for d in d_preds]
+            head_in = self._mlp_bwd_split(self.mlps[1], [s["pred"] for s in saved], dq)
+        if any(d is not None for d in d_projs):
+            ref = [d for d in d_projs if d is not None][0]
+            extra = [(d if d is not None else zero(ref)).contiguous() for d in d_projs]
+            head_in = extra if head_in is None else [head_in[i] + e for i, e in enumerate(extra)]
+        rep_g = None
+        if head_in is not None:
+            rep_g = self._mlp_bwd_split(self.mlps[0], [s["head"] for s in saved], head_in)
+        if rep_g is None and all(d is None for d in d_reps):
+            return
+        gs = []
+        for i, s in enumerate(saved):
+            n, h, w, c = s["final_shape"]
+            du = d_reps[i].contiguous() if d_reps[i] is not None else None
+            gs.append(ops.avgpool_bwd_f32(None if rep_g is None else rep_g[i], du, n, h, w, c))
+        for bi in range(len(self.blocks) - 1, -1, -1):
+            gs = self._block_bwd_split(self.blocks[bi], [s["blocks"][bi] for s in saved], gs)
+        g0 = []
+        for i, s in enumerate(saved):
+            n, h, w, c = s["a0_shape"]
+            g0.append(ops.maxpool_bwd_f32(gs[i], s["pool_idx"], h, w, self.pool_k, self.pool_s, self.pool_p))
+        dy0 = [r[0] for r in self._bn_bwd_f32(self.stem, g0, [s["y0"] for s in saved], [s["c0"] for s in saved], 1)]
+        self._wgrad_split(self.stem, [s["x8"] for s in saved], dy0)
+        self._join_side_stream()
+
     def backward_online(self, saved, d_reps, d_projs, d_preds, notify=True):
         """Backward of the online views.  Each view runs on its own CUDA stream (forked from / joined into the
         caller's stream) so that one view's HBM-bound BatchNorm-backward kernels overlap the other's GEMMs; both
@@ -984,6 +1169,9 @@ class Engine(object):
             self.notify_backward()
         L = len(saved)
         main = torch.cuda.current_stream()
+        if self.bwd32:
+            self._backward_group_split(saved, d_reps, d_projs, d_preds)
+            return
         if not (self.multi_stream and L == 2) or (self.sync and comm.uses_nccl_for_statistics(self.device)):
             self._bwd_channel = 0
             self._backward_group(saved, d_reps, d_projs, d_preds)
@@ -1046,7 +1234,7 @@ class Engine(object):
     # ------------------------------------------------------------------------------------------
     def graph_key(self, a1):
         return (tuple(a1.shape), self.world(), bool(self.sync), self.theta.data_ptr(), self.multi_stream,
-                self.overlap_wgrad, self.T, self.fuse3, self.fuse3_max_planes, self.fused_mlp)
+                self.overlap_wgrad, self.T, self.bwd32, self.fuse3, self.fuse3_max_planes, self.fused_mlp)
 
     def prep_step(self, mean, training):
         """All weight layouts one forward (+ backward) needs, from the fp32 masters."""
@@ -1108,6 +1296,7 @@ class Engine(object):
                 outs, _ = self.forward_lanes(None, lanes, True, rep_bf16_out=[rep_cat[:b], rep_cat[b:], None, None],
                                              x8=[st.inputs[0], st.inputs[1], st.inputs[0], st.inputs[1]])
                 st.logits = self.classifier_forward(rep_cat, [outs[0][0], outs[1][0]])
+            st.cls_planes = self.cls_planes
             st.fwd_launches = launch_count[0] - n0
             st.outs = [t for o in outs for t in o]
             # backward for the usual gradient pattern: only the two online predictions receive a gradient
@@ -1129,18 +1318,27 @@ class Engine(object):
         u = self.cls
         flat = self.theta
         bias = flat[u.b_off:u.b_off + u.cout]
+        self.cls_planes = None
         if self.T and reps_f32 is not None:
             pl = torch.cat([ops.split_planes(r, self.T)[0] for r in reps_f32], 0)
+            if self.bwd32:
+                self.cls_planes = pl      # the fp32 backward's weight gradient reads the representation planes
             return ops.linear_fprop(pl, self.s_online.w[u.idx], bias=bias, out_fp32=True)
         return ops.linear_fprop(rep_cat_b, self.w_online.wf[u.idx], bias=bias, out_fp32=True)
 
-    def classifier_backward(self, rep_cat_b, d_logits):
+    def classifier_backward(self, rep_cat_b, d_logits, planes=None):
+        """planes: the representation planes classifier_forward kept (fp32-accurate backward), else None."""
         self.notify_backward()
         u = self.cls
         d = d_logits.contiguous().float()
         ops.col_sum(d, self._gview(u.b_off, u.cout))
+        cpad = (u.cout + 7) // 8 * 8
+        if planes is not None:
+            self._wgrad(u, [planes], [ops.split_planes(d, self.T, cpad=cpad)[0]], planes=True)
+            self._join_side_stream()
+            return
         # any class count: the bf16 gradient gets a 16-byte row pitch, the GEMM reads only the first `cout` columns
-        db = ops.cast_bf16(d) if u.cout % 8 == 0 else ops.cast_bf16_pitched(d, (u.cout + 7) // 8 * 8)
+        db = ops.cast_bf16(d) if u.cout % 8 == 0 else ops.cast_bf16_pitched(d, cpad)
         self._wgrad(u, [rep_cat_b], [db])
         self._join_side_stream()
 

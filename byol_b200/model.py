@@ -130,15 +130,18 @@ class _ClassifierFn(torch.autograd.Function):
     """Stop-gradient linear classifier (main.py:250-252): logits are differentiable w.r.t. its own weights only."""
 
     @staticmethod
-    def forward(ctx, model, rep_cat_b, anchor, logits=None, reps_f32=None):
+    def forward(ctx, model, rep_cat_b, anchor, logits=None, reps_f32=None, planes=None):
         ctx.model = model
         ctx.rep = rep_cat_b
-        return model._engine.classifier_forward(rep_cat_b, reps_f32) if logits is None else logits.detach()
+        out = model._engine.classifier_forward(rep_cat_b, reps_f32) if logits is None else logits.detach()
+        # fp32-accurate backward: the representation planes of this forward (kept by classifier_forward / the graph)
+        ctx.planes = model._engine.cls_planes if logits is None else planes
+        return out
 
     @staticmethod
     def backward(ctx, d_logits):
-        ctx.model._engine.classifier_backward(ctx.rep, d_logits)
-        return None, None, None, None, None
+        ctx.model._engine.classifier_backward(ctx.rep, d_logits, ctx.planes)
+        return None, None, None, None, None, None
 
 
 class BYOL(nn.Module):
@@ -148,7 +151,8 @@ class BYOL(nn.Module):
     are keyword arguments with the reference's defaults (main.py:57,63)."""
 
     def __init__(self, base_network_output_size, projection_output_size, classifier_output_size,
-                 total_training_steps, base_decay=0.996, arch="resnet50", head_latent_size=4096, precision="bf16"):
+                 total_training_steps, base_decay=0.996, arch="resnet50", head_latent_size=4096, precision="bf16",
+                 backward_precision="bf16"):
         super(BYOL, self).__init__()
         self.base_network_output_size = base_network_output_size
         self.arch = arch
@@ -179,11 +183,25 @@ class BYOL(nn.Module):
         self._engine = Engine(self)
         # forward arithmetic: "bf16" = bf16 tensor-core operands (fast path); "fp32" = the reference's fp32 results
         # from exact 3-way bf16 splits of every operand (6 product terms, fp64 statistics; BASELINE configs[1]);
-        # "bf16x2" = 2-way splits (3 terms, ~16 mantissa bits).  The backward pass always uses bf16 operands.
+        # "bf16x2" = 2-way splits (3 terms, ~16 mantissa bits).
+        # backward arithmetic: "bf16" = bf16 operands (fast; the default for every precision); "fp32" (only with
+        # precision="fp32") = the same exact splits on every backward GEMM, fp32 gradients between layers and fp64
+        # BatchNorm-backward sums (per tensor within 2x of fp32 autograd's error given the same ReLU decisions,
+        # DESIGN.md §4).  It keeps fp32 activations for the backward pass instead of bf16 copies, so it needs more
+        # memory and time.
         if precision not in ("bf16", "bf16x2", "fp32"):
             raise ValueError("precision must be 'bf16', 'bf16x2' or 'fp32', got %r" % (precision,))
+        if backward_precision not in ("bf16", "fp32"):
+            raise ValueError("backward_precision must be 'bf16' or 'fp32', got %r" % (backward_precision,))
+        if backward_precision == "fp32" and precision != "fp32":
+            raise ValueError("backward_precision='fp32' needs precision='fp32' (an fp32 backward needs the fp32 "
+                             "activations of the fp32-accurate forward), got precision=%r" % (precision,))
+        if backward_precision == "fp32" and self._engine.fuse3:
+            raise ValueError("backward_precision='fp32' does not support BYOL_B200_FUSE3=1")
         self.precision = precision
+        self.backward_precision = backward_precision
         self._engine.T = {"bf16": 0, "bf16x2": 3, "fp32": 6}[precision]
+        self._engine.bwd32 = backward_precision == "fp32"
         self._anchor = None
         self._rep_cat = None
 
@@ -228,7 +246,7 @@ class BYOL(nn.Module):
             eng.convert_inputs([a1], outs=gs.inputs[0:1])
             eng.convert_inputs([a2], outs=gs.inputs[1:2])
             o = _GraphedOnlineTargetFn.apply(self, gs, self._anchor)
-            linear_preds = _ClassifierFn.apply(self, self._rep_cat, self._anchor, gs.logits)
+            linear_preds = _ClassifierFn.apply(self, self._rep_cat, self._anchor, gs.logits, None, gs.cls_planes)
         else:
             eng.prep_step(self.target_network.mean, self.training)
         if gs is not None:

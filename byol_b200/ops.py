@@ -594,3 +594,89 @@ def avgpool_f32(x):
     y = torch.empty((n, c), dtype=F32, device=x.device)
     check(lib.byol_avgpool_f32(_ptr(x), _ptr(y), n, h * w, c, _stream()), "byol_avgpool_f32")
     return y
+
+
+# ------------------------------------------------------------------------------------------------
+# fp32-accurate backward path (BYOL(backward_precision="fp32"); csrc/split.cu, csrc/conv_igemm.cu)
+# ------------------------------------------------------------------------------------------------
+def prep_weight_dgrad_planes(w, T, out):
+    """fp32 [Cout, Cin, KH, KW] / [out, in] -> bf16 [Cin, taps*T*Cout] (dgrad layout, weight-side plane pattern)."""
+    _chk(w, F32, "w"); _chk(out, BF16, "out")
+    cout, cin = w.shape[0], w.shape[1]
+    taps = w.numel() // (cout * cin)
+    check(lib.byol_prep_weight_dgrad_planes(_ptr(w), _ptr(out), cout, cin, taps, T, _stream()),
+          "byol_prep_weight_dgrad_planes")
+    return out
+
+
+def conv_dgrad_planes(dyp, wdp, h, w, kh, kw, stride, pad, T, resid=None):
+    """dx[N, h, w, Cin] fp32 = conv_transpose(dY, W) (+ resid, fp32 [N, h, w, Cin]).
+    dyp: bf16 planes [N, Ho, Wo, T*Cout]; wdp: [Cin, taps*T*Cout] from prep_weight_dgrad_planes."""
+    _chk(dyp, BF16, "dy"); _chk(wdp, BF16, "wd"); _chk(resid, F32, "resid")
+    n, ho, wo, tc = dyp.shape
+    cin = wdp.shape[0]
+    dx = torch.empty((n, h, w, cin), dtype=F32, device=dyp.device)
+    check(lib.byol_conv_dgrad_planes(_ptr(dyp), _ptr(wdp), _ptr(dx), _ptr(resid), n, ho, wo, tc // T, h, w, cin, kh, kw,
+                                     stride, pad, T, _stream()), "byol_conv_dgrad_planes")
+    return dx
+
+
+def linear_dgrad_planes(dyp, wdp, T):
+    m, tn = dyp.shape
+    return conv_dgrad_planes(dyp.view(m, 1, 1, tn), wdp, 1, 1, 1, 1, 1, 0, T).view(m, -1)
+
+
+def conv_wgrad_planes(xp, dyp, dw, kh, kw, stride, pad, T):
+    """dw[Cout, Cin, KH, KW] (fp32) += dY^T * im2col(X) over the T product terms.  xp: bf16 planes [N, H, W, T*C]
+    (C >= Cin, a multiple of 8); dyp: bf16 planes [N, Ho, Wo, T*ldy] (ldy >= Cout, a multiple of 8)."""
+    _chk(xp, BF16, "x"); _chk(dyp, BF16, "dy"); _chk(dw, F32, "dw")
+    n, h, w, tc = xp.shape
+    _, ho, wo, tl = dyp.shape
+    check(lib.byol_conv_wgrad_planes(_ptr(xp), _ptr(dyp), _ptr(dw), n, h, w, tc // T, dw.shape[1], ho, wo, dw.shape[0],
+                                     tl // T, kh, kw, stride, pad, T, _stream()), "byol_conv_wgrad_planes")
+    return dw
+
+
+def bn_bwd_reduce_f32(g, y, coeffs, s12, mask_mode, mask=None):
+    """s12 (zeroed fp64 [2C]) += [sum dz, sum dz*xhat] of fp32 g, y [M, C]; mask_mode 1: dz = g where
+    y*scale + shift > 0, 3: where the bits of `mask` (bn_apply_f32) are set."""
+    _chk(g, F32, "g"); _chk(y, F32, "y"); _chk(s12, F64, "s12"); _chk(mask, torch.uint8, "mask")
+    m, c = y.shape
+    check(lib.byol_bn_bwd_reduce_f32(_ptr(g), _ptr(y), _ptr(mask), _ptr(coeffs[0]), _ptr(coeffs[1]), _ptr(coeffs[2]),
+                                     _ptr(coeffs[3]), _ptr(s12), m, c, mask_mode, _stream()), "byol_bn_bwd_reduce_f32")
+    return s12
+
+
+def bn_bwd_apply_f32(g, y, coeffs, gamma, s12, count, mask_mode, T, mask=None, want_planes=True, want_f32=False,
+                     want_dz=False, s12_local=None, dgamma=None, dbeta=None):
+    """dy = gamma*invstd*(dz - s1/n - xhat*s2/n) of fp32 [M, C] -> (planes bf16 [M, T*C] | None, fp32 dy | None,
+    fp32 dz | None); dgamma / dbeta += the rank-local sums (s12_local, default s12)."""
+    _chk(g, F32, "g"); _chk(y, F32, "y"); _chk(s12, F64, "s12"); _chk(mask, torch.uint8, "mask")
+    m, c = y.shape
+    dev = y.device
+    planes = torch.empty((m, T * c), dtype=BF16, device=dev) if want_planes else None
+    dy32 = torch.empty((m, c), dtype=F32, device=dev) if want_f32 else None
+    dz = torch.empty((m, c), dtype=F32, device=dev) if want_dz else None
+    check(lib.byol_bn_bwd_apply_f32(_ptr(g), _ptr(y), _ptr(mask), _ptr(coeffs[0]), _ptr(coeffs[1]), _ptr(coeffs[2]),
+                                    _ptr(coeffs[3]), _ptr(gamma), _ptr(s12), _ptr(s12_local), float(count),
+                                    _ptr(planes), _ptr(dy32), _ptr(dz), _ptr(dgamma), _ptr(dbeta), m, c, mask_mode, T,
+                                    _stream()), "byol_bn_bwd_apply_f32")
+    return planes, dy32, dz
+
+
+def maxpool_bwd_f32(dy, idx, h, w, k=3, s=2, p=1):
+    _chk(dy, F32, "dy"); _chk(idx, torch.uint8, "idx")
+    n, _, _, c = dy.shape
+    dx = torch.empty((n, h, w, c), dtype=F32, device=dy.device)
+    check(lib.byol_maxpool_bwd_f32(_ptr(dy), _ptr(idx), _ptr(dx), n, h, w, c, k, s, p, _stream()),
+          "byol_maxpool_bwd_f32")
+    return dx
+
+
+def avgpool_bwd_f32(ga, gb, n, h, w, c):
+    """dx[n, h, w, c] fp32 = (ga + gb)[n, c] / (h*w); ga / gb fp32 [n, c], either may be None."""
+    _chk(ga, F32, "ga"); _chk(gb, F32, "gb")
+    dev = (ga if ga is not None else gb).device
+    dx = torch.empty((n, h, w, c), dtype=F32, device=dev)
+    check(lib.byol_avgpool_bwd_f32(_ptr(ga), _ptr(gb), _ptr(dx), n, h * w, c, _stream()), "byol_avgpool_bwd_f32")
+    return dx

@@ -191,6 +191,33 @@ int byol_maxpool_f32(const float* x, float* y, void* idx, int N, int H, int W, i
                      byol_stream_t stream);
 int byol_avgpool_f32(const float* x, float* y, int N, int HW, int C, byol_stream_t stream);
 
+/* ---- fp32-accurate backward path (BYOL(backward_precision="fp32")): the same exact splits on the backward GEMMs,
+ *      fp32 gradients between layers, fp64 BatchNorm-backward sums (csrc/split.cu, csrc/conv_igemm.cu). ---- */
+int byol_prep_weight_dgrad_planes(const float* w /* [Cout, Cin, taps] */, void* out /* bf16 [Cin, taps*T*Cout] */,
+                                  int Cout, int Cin, int taps, int T, byol_stream_t stream);
+/* dx (fp32 [Nimg, H, W, Cin]) = conv_transpose(dy planes [Nimg, Hs, Ws, T*Cout], wd) (+ resid_f32, optional) */
+int byol_conv_dgrad_planes(const void* dy, const void* wd, float* dx, const float* resid_f32, int Nimg, int Hs, int Ws,
+                           int Cout, int H, int W, int Cin, int KH, int KW, int stride, int pad, int T,
+                           byol_stream_t stream);
+/* dw (fp32 [Cout, Cin_real, KH, KW]) += sum of the T terms dY-plane^T x im2col(src-plane);
+ * src planes [Nimg, Hs, Ws, T*C], dy planes [Nimg, Ho, Wo, T*ldy] */
+int byol_conv_wgrad_planes(const void* src, const void* dy, float* dw, int Nimg, int Hs, int Ws, int C, int Cin_real,
+                           int Ho, int Wo, int Cout, int ldy, int KH, int KW, int stride, int pad, int T,
+                           byol_stream_t stream);
+/* s12 (fp64 [2C]) += [sum dz, sum dz*xhat]; mask_mode 0 none / 1 relu(y*scale+shift) / 3 mask bits */
+int byol_bn_bwd_reduce_f32(const float* g, const float* y, const void* mask, const float* scale, const float* shift,
+                           const float* mean, const float* invstd, double* s12, int64_t M, int C, int mask_mode,
+                           byol_stream_t stream);
+/* dy = gamma*invstd*(dz - s1/n - xhat*s2/n) -> planes bf16 [M, T*C] and / or fp32 [M, C]; dz_out optional fp32;
+ * dgamma / dbeta (optional) += the rank-local sums s12_local (default s12) */
+int byol_bn_bwd_apply_f32(const float* g, const float* y, const void* mask, const float* scale, const float* shift,
+                          const float* mean, const float* invstd, const float* gamma, const double* s12,
+                          const double* s12_local, double count, void* planes, float* dy32, float* dz_out,
+                          float* dgamma, float* dbeta, int64_t M, int C, int mask_mode, int T, byol_stream_t stream);
+int byol_maxpool_bwd_f32(const float* dy, const void* idx, float* dx, int N, int H, int W, int C, int k, int s, int p,
+                         byol_stream_t stream);
+int byol_avgpool_bwd_f32(const float* ga, const float* gb, float* dx, int N, int HW, int C, byol_stream_t stream);
+
 /* ---- projector / predictor MLP forward as ONE cooperative kernel (main.py:194-205, 238-239):
  *      Linear -> BatchNorm1d (batch statistics, grid barrier, optional cross-rank exchange) -> ReLU -> Linear.
  *      x [B, K1] bf16, w1 [H, ldw1], w2 [O, ldw2] bf16 (fprop layouts); stats [2H] and out [B, O] fp32 ZEROED by the
