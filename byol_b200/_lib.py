@@ -53,6 +53,14 @@ _SIGNATURES = {
     "byol_prep_weight_fold": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     "byol_prep_unit_blocks": [c_int, c_int, c_int, c_int, c_int],
     "byol_prep_weights_multi": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p],
+    # grouped 3x3 convolutions (ResNeXt)
+    "byol_prep_weights_grouped": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p],
+    "byol_conv_fprop_grouped": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                c_int, c_int, c_int, c_int, c_int, c_void_p],
+    "byol_conv_dgrad_grouped": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                c_int, c_int, c_void_p],
+    "byol_conv_wgrad_grouped": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                c_int, c_int, c_int, c_void_p],
     "byol_subsample2": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     "byol_cast_f32_bf16": [c_void_p, c_void_p, c_int64, c_void_p],
     "byol_cast_f32_bf16_2d": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],

@@ -65,6 +65,11 @@ struct TileInfo {
   int cls_idx, ph, pw, kh0, kw0, nkw;   // parity mode only
 };
 
+// GROUPED (grouped 3x3 convolutions with Cin == Cout == C and C / groups dividing 64): the weight of a 64-column
+// output tile [n0, n0 + 64) is block-diagonal and needs only the input channels [n0, n0 + 64), so a tile's K loop is
+// one 64-channel k-block per tap, starting at channel n0.  The weight layout is [C][taps * 64], column
+// tap * 64 + (c - n0) (byol_prep_weights_grouped); BN is 64.
+template <bool GROUPED = false>
 __device__ __forceinline__ TileInfo tile_info(const ConvGemmParams& p, int tile, int BN_) {
   TileInfo t;
   t.m0 = (tile / p.tiles_n) * BM;
@@ -80,7 +85,7 @@ __device__ __forceinline__ TileInfo tile_info(const ConvGemmParams& p, int tile,
     t.kw0 = (t.pw + p.base) & 1;
     const int nkh = (p.KH - t.kh0 + 1) >> 1;
     t.nkw = (p.KW - t.kw0 + 1) >> 1;
-    t.nkb = nkh * t.nkw * (p.C / BK);
+    t.nkb = nkh * t.nkw * (GROUPED ? 1 : p.C / BK);
   }
   return t;
 }
@@ -123,10 +128,11 @@ struct SmemLayout {
 // ---------------------------------------------------------------------------------------------
 static constexpr int IG_THREADS = 17 * 32;
 
-template <int BN, int STAGES, bool A_TMA>
+template <int BN, int STAGES, bool A_TMA, bool GROUPED = false>
 __global__ void __launch_bounds__(IG_THREADS, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB,
                   const __grid_constant__ CUtensorMap tmapC, const ConvGemmParams p, const int num_tiles) {
+  static_assert(!GROUPED || (BN == 64 && !A_TMA), "grouped mode: 64-column tiles, gathered A operand");
   using L = SmemLayout<BN, STAGES, A_TMA>;
   constexpr int EW = L::EW;
   constexpr int CPW = L::CPW;
@@ -200,7 +206,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       }
     };
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-      const TileInfo ti = tile_info(p, tile, BN);
+      const TileInfo ti = tile_info<GROUPED>(p, tile, BN);
       const int m0 = ti.m0;
       const int n0 = ti.n0;
       if (do_stats && stat_n0 != n0) {
@@ -356,11 +362,12 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     // "base offset + tap offset", and padding is a per-row bitmask over the taps computed once per tile.
     // The stride-2 dgrad mapping (div == 2) fits too: a tap is valid only if it has the parity of (o + pad), and
     // then src = ((o + pad) >> 1) - (k >> 1), i.e. again "row base + tap offset"; parity goes into the bitmask.
-    const bool fast = (p.C % BK == 0) && (p.KH * p.KW <= 32) && p.small_src;
+    // (grouped mode: the host guarantees the fast-path conditions)
+    const bool fast = GROUPED || ((p.C % BK == 0) && (p.KH * p.KW <= 32) && p.small_src);
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const TileInfo ti = tile_info(p, tile, BN);
+      const TileInfo ti = tile_info<GROUPED>(p, tile, BN);
       const int m0 = ti.m0;
-      if (p.fold) {
+      if (!GROUPED && p.fold) {
         // stem: k-block = kh, this thread's 16-byte chunk = kw: the 8 chunks of a row are 128 contiguous bytes
         uint32_t mask[8];   // bit kh: (kh, this thread's kw) lies inside the image
         int roff[8];
@@ -420,7 +427,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
               if (sh >= 0 && sh < p.Hs && sw >= 0 && sw < p.Ws) mask[i] |= 1u << tapi;
             }
         }
-        int kh = ti.kh0, kw = ti.kw0, cc = 0, tapi = 0;
+        int kh = ti.kh0, kw = ti.kw0, cc = GROUPED ? ti.n0 : 0, tapi = 0;
         for (int kb = 0; kb < ti.nkb; ++kb, ++it) {
           const int s = it % STAGES;
           const uint32_t ph = (it / STAGES) & 1;
@@ -439,9 +446,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
             cp_async16_zfill(stage_base + sw128_offset(row0 + 16 * i, chunk), g, v);
           }
           cp_async_commit();
-          cc += BK;
-          if (cc >= p.C) {
-            cc = 0;
+          if (!GROUPED) cc += BK;
+          if (GROUPED || cc >= p.C) {
+            if (!GROUPED) cc = 0;
             ++tapi;
             kw += 2;
             if (kw >= p.KW) { kw = ti.kw0; kh += 2; }
@@ -473,7 +480,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
               }
           }
         }
-        int kh = 0, kw = 0, cc = 0, tapi = 0;
+        int kh = 0, kw = 0, cc = GROUPED ? ti.n0 : 0, tapi = 0;
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
           const int s = it % STAGES;
           const uint32_t ph = (it / STAGES) & 1;
@@ -493,14 +500,14 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
             cp_async16_zfill(stage_base + sw128_offset(row0 + 16 * i, chunk), g, v);
           }
           cp_async_commit();
-          cc += BK;
-          if (cc >= p.C) {
-            cc = 0;
+          if (!GROUPED) cc += BK;
+          if (GROUPED || cc >= p.C) {
+            if (!GROUPED) cc = 0;
             ++tapi;
             if (++kw == p.KW) { kw = 0; ++kh; }
           }
         }
-      } else {
+      } else if (!GROUPED) {
         int bh[8], bw[8];
         int64_t ioff[8];
 #pragma unroll
@@ -567,7 +574,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     float d[BN / 2];
     int it = 0, local = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-      const int nkb_tile = tile_info(p, tile, BN).nkb;
+      const int nkb_tile = tile_info<GROUPED>(p, tile, BN).nkb;
       int prev_s = -1;
       for (int kb = 0; kb < nkb_tile; ++kb, ++it) {
         const int s = it % STAGES;
@@ -599,7 +606,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       constexpr uint32_t tx = (uint32_t)L::B_STAGE_BYTES + (A_TMA ? (uint32_t)A_STAGE_BYTES : 0u);
       int it = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const TileInfo ti = tile_info(p, tile, BN);
+        const TileInfo ti = tile_info<GROUPED>(p, tile, BN);
         const int n0 = ti.n0;
         const int m0 = ti.m0;
         int kh = ti.kh0, kw = ti.kw0, cc = 0;
@@ -610,9 +617,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
           mbar_arrive_expect_tx(&full_bar[s], tx);
           int kcol = kb * BK;
           if (p.parity) {   // weight columns of the current class tap
-            kcol = (kh * p.KW + kw) * p.C + cc;
-            cc += BK;
-            if (cc >= p.C) { cc = 0; kw += 2; if (kw >= p.KW) { kw = ti.kw0; kh += 2; } }
+            kcol = (kh * p.KW + kw) * (GROUPED ? BK : p.C) + cc;
+            if (!GROUPED) cc += BK;
+            if (GROUPED || cc >= p.C) { cc = 0; kw += 2; if (kw >= p.KW) { kw = ti.kw0; kh += 2; } }
           }
           tma_load_2d(smem_u32(smemB + s * L::B_STAGE_BYTES), &tmapB, &full_bar[s], kcol, n0);
           if (A_TMA) tma_load_2d(smem_u32(smemA + s * A_STAGE_BYTES), &tmapA, &full_bar[s], kb * BK, m0);
@@ -664,11 +671,17 @@ static constexpr int WG_A_STAGE = 2 * WG_KROWS * 128;  // two 64-channel chunks 
 // CTA whose BN spans several taps re-uses its dY tile (A operand) for all of them.
 static constexpr int WG_THREADS = 13 * 32;
 
-template <int BN, int STAGES, bool B_TMA>
+// GROUPED (grouped 3x3 convolutions, Cin == Cout == C, Cin_real = C / groups dividing 64): BN = 128, one tap per
+// N-tile (Cg = 128), and the B chunk of warpgroup wg holds the input channels co0 + 64*wg .. +63, the only ones that
+// share a group with its 64 output channels.  Each warpgroup runs a 64 x 64 MMA on its own chunk; only the in-group
+// entries reach dW[Cout][Cin_real][KH][KW].
+template <int BN, int STAGES, bool B_TMA, bool GROUPED = false>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB,
                   const WgradParams p) {
+  static_assert(!GROUPED || (BN == 128 && !B_TMA), "grouped mode: two 64-channel chunks, gathered B operand");
   constexpr int NCH = BN / 64;                       // 64-channel chunks along N
+  constexpr int NMMA = GROUPED ? 64 : BN;            // MMA width per warpgroup
   constexpr int B_STAGE = NCH * WG_KROWS * 128;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -719,6 +732,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       bool cvalid = group < p.groups;
       if (p.fold_kw) { kh = group; kw = cw >> 3; ci = 0; cvalid = cvalid && kw < p.KW; }
       else           { kh = group / p.KW; kw = group - kh * p.KW; ci = cw; }
+      if (GROUPED) { ci += co0; cvalid = cvalid && ci < p.C; }
       const int dh = kh - p.pad, dw = kw - p.pad;
       const int64_t sC = (int64_t)p.stride * p.ldsrc;
       for (int it = 0; it < nkb; ++it) {
@@ -769,7 +783,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     // ======================= MMA warpgroups (co rows 64*wg .. +63) ========================
     const int wg = (warp - 4) >> 2;
     const bool leader = (threadIdx.x & 127) == 0;
-    float d[BN / 2];
+    float d[NMMA / 2];
     int prev_s = -1;
     for (int it = 0; it < nkb; ++it) {
       const int s = it % STAGES;
@@ -779,12 +793,13 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       // warpgroup's 64 co are the A chunk wg
       const uint64_t adesc =
           make_smem_desc_sw128(smem_u32(smemA + s * WG_A_STAGE + wg * WG_KROWS * 128), WG_KROWS * 128, 1024);
-      const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smemB + s * B_STAGE), WG_KROWS * 128, 1024);
+      const uint64_t bdesc = make_smem_desc_sw128(
+          smem_u32(smemB + s * B_STAGE + (GROUPED ? wg * WG_KROWS * 128 : 0)), WG_KROWS * 128, 1024);
       wg_fence();
 #pragma unroll
       for (int k = 0; k < WG_KROWS / 16; ++k) {
         // advance 16 pixel rows = 2048 bytes: +128 in the (addr >> 4) field
-        wgmma_bf16<BN, 1, 1>(d, adesc + (uint64_t)(128 * k), bdesc + (uint64_t)(128 * k), (uint32_t)((it | k) != 0));
+        wgmma_bf16<NMMA, 1, 1>(d, adesc + (uint64_t)(128 * k), bdesc + (uint64_t)(128 * k), (uint32_t)((it | k) != 0));
       }
       wg_commit();
       wg_wait<1>();
@@ -797,6 +812,25 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     const int t = threadIdx.x & 127;
     const int r0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
     auto add = [&](const float* q, float v) { fix_add(p.fx + (q - p.dw), v); };
+    if (GROUPED) {
+      // column c of warpgroup wg is input channel co0 + 64*wg + c
+      const int gs = p.Cin_real;
+      const int tap = n0 / BN;
+#pragma unroll
+      for (int j = 0; j < NMMA / 8; ++j) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int co = co0 + r0 + 8 * h;
+          if (co >= p.Cout) continue;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int ci = co0 + wg * 64 + 8 * j + 2 * (t & 3) + e;
+            if (co / gs == ci / gs) add(p.dw + ((int64_t)co * gs + ci % gs) * taps + tap, d[4 * j + 2 * h + e]);
+          }
+        }
+      }
+      return;
+    }
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
@@ -906,19 +940,19 @@ bool patch_conv_applicable(int H, int W, int C, int Ndim, int KH, int KW, int st
                            const float* bias, int64_t src_elems);
 int patch_conv_launch(const void* src, const void* wt, void* dst, const void* resid, float* col_sum, float* col_sqsum,
                       int Nimg, int H, int W, int C, int Ndim, int ldw, int ldc, int flip, int relu, int sms,
-                      cudaStream_t stream);
+                      cudaStream_t stream, int grouped = 0);
 
 bool patch_wgrad_applicable(int H, int W, int C, int Cin_real, int Cout, int KH, int KW, int stride, int pad);
 int patch_wgrad_launch(const void* x, const void* dy, float* dw, int Nimg, int H, int W, int C, int Cout, int sms,
-                       cudaStream_t stream);
+                       cudaStream_t stream, int gs = 0);
 
 static int sm_count() { return device_sm_count(); }
 
-template <int BN, int STAGES, bool A_TMA>
+template <int BN, int STAGES, bool A_TMA, bool GROUPED = false>
 static int launch_igemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
                         const ConvGemmParams& p, int tiles_m, cudaStream_t stream) {
   using L = SmemLayout<BN, STAGES, A_TMA>;
-  auto kern = conv_igemm_kernel<BN, STAGES, A_TMA>;
+  auto kern = conv_igemm_kernel<BN, STAGES, A_TMA, GROUPED>;
   static bool attr_set[kMaxDevices] = {};
   const int dev_slot = device_slot();
   if (!attr_set[dev_slot]) {
@@ -949,7 +983,7 @@ static int conv_igemm_impl(const void* src, const void* wt, void* dst, const voi
                            const void* resid_mask, int resid_up, const float* bias, float* col_sum, float* col_sqsum,
                            int Nimg, int Hs, int Ws, int C, int Ho, int Wo, int Ndim, int KH, int KW, int stride,
                            int pad, int mode, int ldw, int ldc, int out_fp32, int relu, int force_gather,
-                           cudaStream_t stream) {
+                           cudaStream_t stream, int grouped = 0) {
   BYOL_CHECK_ARG(src && wt && dst, "byol_conv_igemm: null pointer");
   BYOL_CHECK_ARG(resid_f32 == nullptr || (out_fp32 && resid == nullptr && !resid_up),
                  "byol_conv_igemm: an fp32 residual needs an fp32 output and no other residual");
@@ -978,10 +1012,11 @@ static int conv_igemm_impl(const void* src, const void* wt, void* dst, const voi
       col_sum == nullptr && gemm_fused_applicable((int)M64, C, Ndim, ldw, ldc))
     return gemm_fused_launch(src, wt, dst, resid, resid_mask, nullptr, bias, nullptr, nullptr, nullptr, nullptr,
                              (int)M64, C, Ndim, ldw, ldc, relu, 0, 0, stream);
-  if (!force_gather && resid_f32 == nullptr && resid_mask == nullptr && !resid_up && Hs == Ho && Ws == Wo && ldw >= 9 * C &&
+  if (!force_gather && resid_f32 == nullptr && resid_mask == nullptr && !resid_up && Hs == Ho && Ws == Wo &&
+      ldw >= 9 * (grouped ? BK : C) &&
       patch_conv_applicable(Hs, Ws, C, Ndim, KH, KW, stride, pad, out_fp32, bias, (int64_t)Nimg * Hs * Ws * C))
     return patch_conv_launch(src, wt, dst, resid, col_sum, col_sqsum, Nimg, Hs, Ws, C, Ndim, ldw, ldc, mode, relu,
-                             sm_count(), stream);
+                             sm_count(), stream, grouped);
   ConvGemmParams p;
   memset(&p, 0, sizeof(p));
   p.src = (const bf16*)src;
@@ -998,7 +1033,7 @@ static int conv_igemm_impl(const void* src, const void* wt, void* dst, const voi
   else           { p.mul = 1; p.base = pad; p.dk = -1; p.div = stride; }
   p.M = (int)M64;
   p.Ndim = Ndim;
-  p.Kg = KH * KW * C;
+  p.Kg = KH * KW * (grouped ? BK : C);   // grouped: one 64-channel k-block per tap
   // stem layout (weights made by byol_prep_weight with fold = 1): K = KH * 64, column = kh*64 + kw*8 + c
   p.fold = (mode == 0 && C == 8 && KW > 1 && KW <= 8 && KH <= 32 && ldw == KH * 64 &&
             (int64_t)Nimg * Hs * Ws * C < (1ll << 31) - (1ll << 24)) ? 1 : 0;
@@ -1009,7 +1044,7 @@ static int conv_igemm_impl(const void* src, const void* wt, void* dst, const voi
   p.out_fp32 = out_fp32;
   p.relu = relu;
   p.small_src = ((int64_t)Nimg * Hs * Ws * C < (1ll << 31) - (1ll << 24)) ? 1 : 0;
-  const int BN = (Ndim > 64) ? 128 : 64;
+  const int BN = (Ndim > 64 && !grouped) ? 128 : 64;
   p.tiles_n = (Ndim + BN - 1) / BN;
   int tiles_m = (p.M + BM - 1) / BM;
   if (mode == 1 && stride == 2 && Ho % 2 == 0 && Wo % 2 == 0 && C % BK == 0 && p.small_src && KH <= 3 && KW <= 3 &&
@@ -1050,7 +1085,9 @@ static int conv_igemm_impl(const void* src, const void* wt, void* dst, const voi
     if (p.fx == nullptr) return -2;
   }
   int rc;
-  if (BN == 128) {
+  if (grouped) {
+    rc = launch_igemm<64, 4, false, true>(ta, tb, tc, p, tiles_m, stream);
+  } else if (BN == 128) {
     rc = a_tma ? launch_igemm<128, 3, true>(ta, tb, tc, p, tiles_m, stream)
                : launch_igemm<128, 3, false>(ta, tb, tc, p, tiles_m, stream);
   } else {
@@ -1070,6 +1107,45 @@ extern "C" int byol_conv_igemm(const void* src, const void* wt, void* dst, const
                          Ho, Wo, Ndim, KH, KW, stride, pad, mode, ldw, ldc, out_fp32, relu, force_gather, stream);
 }
 
+// Grouped 3x3 convolutions (ResNeXt conv2): Cin == Cout == C, a multiple of 64; C / groups divides 64; pad 1;
+// stride 1 or 2.  (H, W) is the input size, (Ho, Wo) the output size.  Every check runs before any launch.
+static bool grouped_geometry_ok(const char* what, int Nimg, int H, int W, int C, int Ho, int Wo, int KH, int KW,
+                                int stride, int pad) {
+  if (Nimg <= 0 || H <= 0 || W <= 0 || C < 64 || C % 64 != 0 || KH != 3 || KW != 3 || pad != 1 ||
+      (stride != 1 && stride != 2) || Ho != (H - 1) / stride + 1 || Wo != (W - 1) / stride + 1) {
+    set_last_error("%s: unsupported geometry (N=%d H=%d W=%d C=%d Ho=%d Wo=%d KH=%d KW=%d stride=%d pad=%d): needs "
+                   "C %% 64 == 0, 3x3, pad 1, stride 1 or 2", what, Nimg, H, W, C, Ho, Wo, KH, KW, stride, pad);
+    return false;
+  }
+  const int64_t big = (int64_t)Nimg * (H > Ho ? H : Ho) * (W > Wo ? W : Wo) * C;
+  if (big >= (1ll << 31) - (1ll << 24)) {
+    set_last_error("%s: tensor of %lld elements too large for 32-bit offsets", what, (long long)big);
+    return false;
+  }
+  return true;
+}
+
+// y[Nimg, Ho, Wo, C] = grouped conv(x[Nimg, H, W, C], wt); wt: bf16 [C / 64][64][9 * 64] (byol_prep_weights_grouped);
+// col_sum / col_sqsum (both or none): += per-channel sum / sum of squares of the stored bf16 y
+extern "C" int byol_conv_fprop_grouped(const void* x, const void* wt, void* y, float* col_sum, float* col_sqsum,
+                                       int Nimg, int H, int W, int C, int Ho, int Wo, int KH, int KW, int stride,
+                                       int pad, cudaStream_t stream) {
+  BYOL_CHECK_ARG(x && wt && y, "byol_conv_fprop_grouped: null pointer");
+  if (!grouped_geometry_ok("byol_conv_fprop_grouped", Nimg, H, W, C, Ho, Wo, KH, KW, stride, pad)) return -1;
+  return conv_igemm_impl(x, wt, y, nullptr, nullptr, nullptr, 0, nullptr, col_sum, col_sqsum, Nimg, H, W, C, Ho, Wo,
+                         C, KH, KW, stride, pad, 0, KH * KW * BK, C, 0, 0, 0, stream, 1);
+}
+
+// dx[Nimg, H, W, C] = transpose of the grouped conv applied to dy[Nimg, Ho, Wo, C]; wd: bf16 [C / 64][64][9 * 64]
+// (the dgrad layout of byol_prep_weights_grouped)
+extern "C" int byol_conv_dgrad_grouped(const void* dy, const void* wd, void* dx, int Nimg, int Ho, int Wo, int C,
+                                       int H, int W, int KH, int KW, int stride, int pad, cudaStream_t stream) {
+  BYOL_CHECK_ARG(dy && wd && dx, "byol_conv_dgrad_grouped: null pointer");
+  if (!grouped_geometry_ok("byol_conv_dgrad_grouped", Nimg, H, W, C, Ho, Wo, KH, KW, stride, pad)) return -1;
+  return conv_igemm_impl(dy, wd, dx, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr, Nimg, Ho, Wo, C, H, W,
+                         C, KH, KW, stride, pad, 1, KH * KW * BK, C, 0, 0, 0, stream, 1);
+}
+
 // fp32-accurate dgrad: dx[Nimg, H, W, Cin] (fp32) = conv_transpose(dY, W) (+ resid_f32, fp32 [Nimg, H, W, Cin]).
 // dy: bf16 planes [Nimg, Hs, Ws, T*Cout] (activation pattern), wd: bf16 [Cin, taps*T*Cout] (byol_prep_weight_dgrad_planes).
 // One implicit GEMM over T*Cout channels.  Stride-2 layers take the gather path (the parity mode stores bf16 only).
@@ -1082,12 +1158,12 @@ extern "C" int byol_conv_dgrad_planes(const void* dy, const void* wd, float* dx,
                          H, W, Cin, KH, KW, stride, pad, 1, KH * KW * T * Cout, Cin, 1, 0, 0, stream);
 }
 
-template <int BN, bool B_TMA>
+template <int BN, bool B_TMA, bool GROUPED = false>
 static int launch_wgrad(const CUtensorMap& ta, const CUtensorMap& tb, const WgradParams& p, int grid,
                         cudaStream_t stream) {
   constexpr int STAGES = 4;
   constexpr int SMEM = STAGES * (WG_A_STAGE + (BN / 64) * WG_KROWS * 128) + 256 + 1024;
-  auto kern = conv_wgrad_kernel<BN, STAGES, B_TMA>;
+  auto kern = conv_wgrad_kernel<BN, STAGES, B_TMA, GROUPED>;
   static bool attr_set[kMaxDevices] = {};
   const int dev_slot = device_slot();
   if (!attr_set[dev_slot]) {
@@ -1108,9 +1184,14 @@ static int launch_wgrad(const CUtensorMap& ta, const CUtensorMap& tb, const Wgra
 // T: 0 = plain bf16 operands; 3 / 6 = split-operand planes (byol_conv_wgrad_planes)
 static int conv_wgrad_impl(const void* src, const void* dy, float* dw, int Nimg, int Hs, int Ws, int C, int Cin_real,
                            int Ho, int Wo, int Cout, int ldy, int KH, int KW, int stride, int pad, int force_gather,
-                           int T, cudaStream_t stream) {
+                           int T, cudaStream_t stream, int gs = 0) {
   BYOL_CHECK_ARG(src && dy && dw, "byol_conv_wgrad: null pointer");
   if (ldy == 0) ldy = Cout;
+  // gs > 0: grouped 3x3 convolution with gs = Cin_real input channels per group (byol_conv_wgrad_grouped)
+  if (gs > 0) {
+    if (!force_gather && Hs == Ho && Ws == Wo && patch_wgrad_applicable(Hs, Ws, C, C, Cout, KH, KW, stride, pad))
+      return patch_wgrad_launch(src, dy, dw, Nimg, Hs, Ws, C, Cout, sm_count(), stream, gs);
+  }
   BYOL_CHECK_ARG(C % 8 == 0 && ldy % 8 == 0 && ldy >= Cout && Cout > 0,
                  "byol_conv_wgrad: C=%d and the dy pitch %d must be multiples of 8 (Cout=%d)", C, ldy, Cout);
   BYOL_CHECK_ARG(Cin_real <= C, "byol_conv_wgrad: Cin_real > C");
@@ -1139,7 +1220,7 @@ static int conv_wgrad_impl(const void* src, const void* dy, float* dw, int Nimg,
   p.Cin_real = Cin_real;
   p.fold_kw = (C == 8 && KW <= 8 && KW > 1) ? 1 : 0;
   BYOL_CHECK_ARG(p.fold_kw || C % 64 == 0 || KH * KW == 1, "byol_conv_wgrad: C=%d must be 8 (stem) or a multiple of 64", C);
-  p.Cg = p.fold_kw ? 64 : C;
+  p.Cg = p.fold_kw ? 64 : gs > 0 ? 128 : C;               // grouped: one 128-wide column group (two chunks) per tap
   p.groups = p.fold_kw ? KH : KH * KW;
   const int ncols = p.groups * p.Cg;                       // concatenated (tap, channel) columns
   // (a 128 x 256 tile would need 128 accumulator registers per MMA thread: more than the register file leaves)
@@ -1178,9 +1259,20 @@ static int conv_wgrad_impl(const void* src, const void* dy, float* dw, int Nimg,
   const int64_t ndw = (int64_t)Cout * Cin_real * taps;
   p.fx = fix_scratch(stream, ndw);
   if (p.fx == nullptr) return -2;
-  const int rc = BN == 128 ? (b_tma ? launch_wgrad<128, true>(ta, tb, p, grid, stream) : launch_wgrad<128, false>(ta, tb, p, grid, stream))
+  const int rc = gs > 0 ? launch_wgrad<128, false, true>(ta, tb, p, grid, stream)
+               : BN == 128 ? (b_tma ? launch_wgrad<128, true>(ta, tb, p, grid, stream) : launch_wgrad<128, false>(ta, tb, p, grid, stream))
                            : (b_tma ? launch_wgrad<64, true>(ta, tb, p, grid, stream) : launch_wgrad<64, false>(ta, tb, p, grid, stream));
   return fix_done(stream, rc != 0 ? rc : fix_flush(p.fx, dw, ndw, stream));
+}
+
+// Grouped 3x3 wgrad: dw[C][Cg][KH][KW] (fp32, the real parameter, accumulated) += the in-group entries of
+// dY^T x im2col(x); x [Nimg, H, W, C], dy [Nimg, Ho, Wo, C].  Nothing outside the C * Cg * 9 entries is written.
+extern "C" int byol_conv_wgrad_grouped(const void* x, const void* dy, float* dw, int Nimg, int H, int W, int C, int Cg,
+                                       int Ho, int Wo, int KH, int KW, int stride, int pad, cudaStream_t stream) {
+  BYOL_CHECK_ARG(x && dy && dw, "byol_conv_wgrad_grouped: null pointer");
+  BYOL_CHECK_ARG(Cg >= 1 && Cg <= 64 && 64 % Cg == 0, "byol_conv_wgrad_grouped: Cg=%d must divide 64", Cg);
+  if (!grouped_geometry_ok("byol_conv_wgrad_grouped", Nimg, H, W, C, Ho, Wo, KH, KW, stride, pad)) return -1;
+  return conv_wgrad_impl(x, dy, dw, Nimg, H, W, C, Cg, Ho, Wo, C, C, KH, KW, stride, pad, 0, 0, stream, Cg);
 }
 
 extern "C" int byol_conv_wgrad(const void* src, const void* dy, float* dw, int Nimg, int Hs, int Ws, int C,

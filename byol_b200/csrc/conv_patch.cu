@@ -52,10 +52,14 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst_smem, const CUtensorMap
       : "memory");
 }
 
-template <int BN>
+// GROUPED (grouped convolutions whose group size divides 64, weights [C][9 * 64] from byol_prep_weights_grouped):
+// the block-diagonal weight tile of N-tile n0 needs only the input channels [n0, n0 + 64), so each tile loads the one
+// patch of that chunk (nchunks = 1) and weight tile column tap * 64.
+template <int BN, bool GROUPED = false>
 __global__ void __launch_bounds__(P_THREADS, 1)
 conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_constant__ CUtensorMap tmapB,
                      const PatchParams p) {
+  static_assert(!GROUPED || BN == 64, "grouped mode: 64-column tiles");
   constexpr int B_STAGE = BN * 128;
   constexpr int PATCH_OFF = 0;
   constexpr int B_OFF = P_PSTAGES * 2 * P_PATCH_SLOT;
@@ -283,13 +287,14 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
         const int mt0 = (tile / p.tiles_n) * 2;
         const int npair = (mt0 + 1 < p.num_mt) ? 2 : 1;
         const int ps = g % P_PSTAGES;
+        const int c0 = GROUPED ? (tile % p.tiles_n) * BN : cc * 64;
         mbar_wait(&pempty[ps], (uint32_t)(((g / P_PSTAGES) & 1) ^ 1));
         mbar_arrive_expect_tx(&pfull[ps], p.patch_bytes * (uint32_t)npair);
         for (int jp = 0; jp < npair; ++jp) {
           const int mt = mt0 + jp;
           const int n = mt / p.HB;
           const int h0 = (mt - n * p.HB) * p.TH;
-          tma_load_4d(smem_u32(smemP + (ps * 2 + jp) * P_PATCH_SLOT), &tmapX, &pfull[ps], cc * 64, -1, h0 - 1, n);
+          tma_load_4d(smem_u32(smemP + (ps * 2 + jp) * P_PATCH_SLOT), &tmapX, &pfull[ps], c0, -1, h0 - 1, n);
         }
       };
       int bit = 0;
@@ -328,12 +333,12 @@ static PFN_encodeTiled patch_encode_fn() {
   return fn;
 }
 
-template <int BN>
+template <int BN, bool GROUPED = false>
 static int launch_patch(const CUtensorMap& tx, const CUtensorMap& tb, const PatchParams& p, int sms,
                         cudaStream_t stream) {
   constexpr int SMEM = P_PSTAGES * 2 * P_PATCH_SLOT + P_BSTAGES * BN * 128 + 4 * 2048 + 128 * P_ACC_LD * 4 + 256 + 1024;
   static_assert(SMEM <= 232448, "conv3x3_patch_kernel: shared memory");
-  auto kern = conv3x3_patch_kernel<BN>;
+  auto kern = conv3x3_patch_kernel<BN, GROUPED>;
   static bool attr_set[kMaxDevices] = {};
   const int dev_slot = device_slot();
   if (!attr_set[dev_slot]) {
@@ -364,10 +369,10 @@ bool patch_conv_applicable(int H, int W, int C, int Ndim, int KH, int KW, int st
   return true;
 }
 
-// src: NHWC [Nimg,H,W,C]; wt: [Ndim][9*C] K-major (k = tap*C + c); dst: [Nimg,H,W,Ndim] bf16
+// src: NHWC [Nimg,H,W,C]; wt: [Ndim][9*C] K-major (k = tap*C + c), grouped: [Ndim = C][9*64]; dst: [Nimg,H,W,Ndim] bf16
 int patch_conv_launch(const void* src, const void* wt, void* dst, const void* resid, float* col_sum, float* col_sqsum,
                       int Nimg, int H, int W, int C, int Ndim, int ldw, int ldc, int flip, int relu, int sms,
-                      cudaStream_t stream) {
+                      cudaStream_t stream, int grouped) {
   PFN_encodeTiled fn = patch_encode_fn();
   if (fn == nullptr) { set_last_error("cuTensorMapEncodeTiled entry point unavailable"); return -3; }
   PatchParams p;
@@ -383,7 +388,7 @@ int patch_conv_launch(const void* src, const void* wt, void* dst, const void* re
   p.tiles_n = (Ndim + BN - 1) / BN;
   p.num_mt = Nimg * p.HB;
   p.num_tiles = ((p.num_mt + 1) / 2) * p.tiles_n;
-  p.nchunks = C / 64;
+  p.nchunks = grouped ? 1 : C / 64;
   p.flip = flip;
   p.relu = relu;
   p.patch_bytes = 128u * (uint32_t)p.Wp * (uint32_t)(p.TH + 2);
@@ -400,7 +405,7 @@ int patch_conv_launch(const void* src, const void* wt, void* dst, const void* re
     if (r != CUDA_SUCCESS) { set_last_error("patch conv: 4-D tensor map encode failed (%d)", (int)r); return -3; }
   }
   {
-    cuuint64_t dims[2] = {(cuuint64_t)(9 * C), (cuuint64_t)Ndim};
+    cuuint64_t dims[2] = {(cuuint64_t)(9 * 64 * p.nchunks), (cuuint64_t)Ndim};
     cuuint64_t strides[1] = {(cuuint64_t)ldw * 2};
     cuuint32_t box[2] = {64u, (cuuint32_t)BN};
     cuuint32_t estr[2] = {1u, 1u};
@@ -413,7 +418,7 @@ int patch_conv_launch(const void* src, const void* wt, void* dst, const void* re
     p.fx = fix_scratch(stream, 2 * (int64_t)Ndim);
     if (p.fx == nullptr) return -2;
   }
-  int rc = launch_patch<64>(tx, tb, p, sms, stream);
+  int rc = grouped ? launch_patch<64, true>(tx, tb, p, sms, stream) : launch_patch<64>(tx, tb, p, sms, stream);
   if (rc != 0 || col_sum == nullptr) return rc;
   if ((rc = fix_flush(p.fx, col_sum, Ndim, stream)) != 0) return rc;
   return fix_done(stream, fix_flush(p.fx + Ndim, col_sqsum, Ndim, stream));
@@ -437,7 +442,7 @@ int patch_conv_launch(const void* src, const void* wt, void* dst, const void* re
 namespace byol {
 
 struct WPatchParams {
-  float* dw;            // [Cout][Cin][3][3] fp32
+  float* dw;            // [Cout][Cin][3][3] fp32 (grouped: [Cout][gs][3][3])
   Fix128* fx;        // fixed-point accumulators over the whole dw (fix_scratch)
   int Nimg, H, W, C, Cout;
   int Wp, TH, HB, num_mt;
@@ -445,16 +450,22 @@ struct WPatchParams {
   int splits, mt_per_split;
   uint32_t patch_bytes; // 128 * Wp * (TH + 2)
   uint32_t dy_bytes;    // 128 * Wp * TH
+  int gs;               // grouped mode: input channels per group
 };
 
 static constexpr int WP_STAGES = 2;
 
 static constexpr int WP_THREADS = 9 * 32;
 
-template <int NB>
+// GROUPED (group size gs dividing 64, Cin == Cout): the stage holds the patches of input channels co0 .. co0 + 127;
+// warpgroup wg multiplies its 64 co by chunk wg only (the one channel chunk its groups live in), and only in-group
+// entries reach dW[Cout][gs][3][3].
+template <int NB, bool GROUPED = false>
 __global__ void __launch_bounds__(WP_THREADS, 1)
 conv3x3_wgrad_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_constant__ CUtensorMap tmapDY,
                            const WPatchParams p) {
+  static_assert(!GROUPED || NB == 2, "grouped mode: two 64-channel patches per stage");
+  constexpr int NW = GROUPED ? 64 : 64 * NB;   // MMA width per warpgroup
   constexpr int X_STAGE = NB * P_PATCH_SLOT;
   constexpr int DY_STAGE = 2 * 16384;
   constexpr int DY_OFF = WP_STAGES * X_STAGE;
@@ -474,7 +485,7 @@ conv3x3_wgrad_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __gr
   const int tile_co = bid % p.co_tiles; bid /= p.co_tiles;
   const int split = bid;
   const int co0 = tile_co * 128;
-  const int ci0 = cig * 64 * NB;
+  const int ci0 = GROUPED ? co0 : cig * 64 * NB;
   const int mt_begin = split * p.mt_per_split;
   int mt_end = mt_begin + p.mt_per_split;
   if (mt_end > p.num_mt) mt_end = p.num_mt;
@@ -512,13 +523,13 @@ conv3x3_wgrad_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __gr
   } else {
     const int wg = warp >> 2;
     const bool leader = (threadIdx.x & 127) == 0;
-    float d[3][32 * NB];
+    float d[3][NW / 2];
     int prev_s = -1;
     for (int it = 0; it < ntiles; ++it) {
       const int s = it % WP_STAGES;
       mbar_wait(&full_bar[s], (uint32_t)((it / WP_STAGES) & 1));
       const uint32_t a_base = smem_u32(smemDY + s * DY_STAGE) + (uint32_t)wg * 16384u;   // this warpgroup's 64 co
-      const uint32_t x_base = smem_u32(smemX + s * X_STAGE);
+      const uint32_t x_base = smem_u32(smemX + s * X_STAGE) + (GROUPED ? (uint32_t)wg * P_PATCH_SLOT : 0u);
       wg_fence();
 #pragma unroll
       for (int kw = 0; kw < 3; ++kw) {
@@ -528,8 +539,8 @@ conv3x3_wgrad_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __gr
         const uint64_t bdesc = make_smem_desc_sw128(x_base + shift, P_PATCH_SLOT, 1024);
 #pragma unroll
         for (int k = 0; k < 8; ++k)   // 16 pixel rows = 2048 bytes per step
-          wgmma_bf16<64 * NB, 1, 1>(d[kw], adesc + (uint64_t)(128 * k), bdesc + (uint64_t)(128 * k),
-                                    (uint32_t)((it | k) != 0));
+          wgmma_bf16<NW, 1, 1>(d[kw], adesc + (uint64_t)(128 * k), bdesc + (uint64_t)(128 * k),
+                               (uint32_t)((it | k) != 0));
       }
       wg_commit();
       wg_wait<1>();
@@ -542,6 +553,20 @@ conv3x3_wgrad_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __gr
     // ---------------- epilogue: registers -> L2 reductions into dW[co][ci][kh][kw] ----------------
     const int t = threadIdx.x & 127;
     const int r0 = co0 + wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
+    if (GROUPED) {
+      const int gs = p.gs;
+#pragma unroll
+      for (int kw = 0; kw < 3; ++kw) {
+#pragma unroll
+        for (int i = 0; i < NW / 2; ++i) {
+          const int co = r0 + ((i & 2) ? 8 : 0);
+          const int ci = ci0 + wg * 64 + 8 * (i >> 2) + 2 * (t & 3) + (i & 1);
+          if (co < p.Cout && co / gs == ci / gs)
+            fix_add(p.fx + ((int64_t)co * gs + ci % gs) * 9 + kh * 3 + kw, d[kw][i]);
+        }
+      }
+      return;
+    }
 #pragma unroll
     for (int kw = 0; kw < 3; ++kw) {
 #pragma unroll
@@ -554,11 +579,11 @@ conv3x3_wgrad_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __gr
   }
 }
 
-template <int NB>
+template <int NB, bool GROUPED = false>
 static int launch_wpatch(const CUtensorMap& tx, const CUtensorMap& ty, const WPatchParams& p, int grid,
                          cudaStream_t stream) {
   constexpr int SMEM = WP_STAGES * (NB * P_PATCH_SLOT + 2 * 16384) + 256 + 1024;
-  auto kern = conv3x3_wgrad_patch_kernel<NB>;
+  auto kern = conv3x3_wgrad_patch_kernel<NB, GROUPED>;
   static bool attr_set[kMaxDevices] = {};
   const int dev_slot = device_slot();
   if (!attr_set[dev_slot]) {
@@ -584,8 +609,9 @@ bool patch_wgrad_applicable(int H, int W, int C, int Cin_real, int Cout, int KH,
 }
 
 // x: NHWC [Nimg,H,W,C]; dy: [Nimg,H,W,Cout]; dw: fp32 [Cout][C][3][3] (accumulated)
+// gs > 0: grouped convolution (Cout == C) with gs input channels per group; dw is then [Cout][gs][3][3]
 int patch_wgrad_launch(const void* x, const void* dy, float* dw, int Nimg, int H, int W, int C, int Cout, int sms,
-                       cudaStream_t stream) {
+                       cudaStream_t stream, int gs) {
   PFN_encodeTiled fn = patch_encode_fn();
   if (fn == nullptr) { set_last_error("cuTensorMapEncodeTiled entry point unavailable"); return -3; }
   WPatchParams p;
@@ -598,8 +624,9 @@ int patch_wgrad_launch(const void* x, const void* dy, float* dw, int Nimg, int H
   p.num_mt = Nimg * p.HB;
   // one 64-channel chunk per CTA: 3 taps x 64 x 64 accumulators per warpgroup already take 96 registers per thread
   constexpr int NB = 1;
+  p.gs = gs;
   p.co_tiles = (Cout + 127) / 128;
-  p.ci_groups = C / (64 * NB);
+  p.ci_groups = gs > 0 ? 1 : C / (64 * NB);
   const int base = p.co_tiles * p.ci_groups * 3;
   int splits = sms / base;
   if (splits < 1) splits = 1;
@@ -621,10 +648,10 @@ int patch_wgrad_launch(const void* x, const void* dy, float* dw, int Nimg, int H
     if (r != CUDA_SUCCESS) { set_last_error("patch wgrad: tensor map encode failed (%d)", (int)r); return -3; }
   }
   const int grid = base * p.splits;
-  const int64_t ndw = (int64_t)Cout * C * 9;
+  const int64_t ndw = (int64_t)Cout * (gs > 0 ? gs : C) * 9;
   p.fx = fix_scratch(stream, ndw);
   if (p.fx == nullptr) return -2;
-  const int rc = launch_wpatch<NB>(tx, ty, p, grid, stream);
+  const int rc = gs > 0 ? launch_wpatch<2, true>(tx, ty, p, grid, stream) : launch_wpatch<NB>(tx, ty, p, grid, stream);
   return fix_done(stream, rc != 0 ? rc : fix_flush(p.fx, dw, ndw, stream));
 }
 

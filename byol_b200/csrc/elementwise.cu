@@ -160,6 +160,31 @@ __global__ void prep_weights_multi_kernel(const float* __restrict__ flat, bf16* 
   }
 }
 
+// Grouped 3x3 convolutions (Cin == Cout == C, Cg = C / groups dividing 64), all units of one parameter set in ONE
+// launch; blockIdx.y = unit.  desc[u] = {src_off, dstf_off, dstd_off (-1: none), C, Cg} (int64 each).  The weight of
+// a 64-channel tile [n0, n0 + 64) is block-diagonal, so both layouts keep only that tile's 64 partner channels:
+//   fprop wf[co][tap * 64 + (ci - n0)], n0 = co & ~63   = w[co][ci % Cg][tap] if co, ci share a group, else 0
+//   dgrad wd[ci][tap * 64 + (co - n0)], n0 = ci & ~63   = w[co][ci % Cg][tap] if co, ci share a group, else 0
+__global__ void prep_weights_grouped_kernel(const float* __restrict__ flat, bf16* __restrict__ pool_f,
+                                            bf16* __restrict__ pool_d, const int64_t* __restrict__ desc) {
+  const int64_t* d = desc + (int64_t)blockIdx.y * 5;
+  const float* w = flat + d[0];
+  bf16* wf = pool_f + d[1];
+  bf16* wd = d[2] >= 0 ? pool_d + d[2] : nullptr;
+  const int C = (int)d[3], Cg = (int)d[4];
+  if (C <= 0 || C % 64 != 0 || Cg <= 0 || Cg > 64 || 64 % Cg != 0) return;   // rejected on the host
+  const int64_t total = (int64_t)C * 9 * 64;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int j = (int)(i & 63);
+    const int tap = (int)((i >> 6) % 9);
+    const int r = (int)(i / (9 * 64));
+    const int c = (r & ~63) + j;   // the partner channel: ci of row co (fprop), co of row ci (dgrad)
+    const bool same = r / Cg == c / Cg;
+    wf[i] = __float2bfloat16_rn(same ? __ldg(w + ((int64_t)r * Cg + c % Cg) * 9 + tap) : 0.f);
+    if (wd != nullptr) wd[i] = __float2bfloat16_rn(same ? __ldg(w + ((int64_t)c * Cg + r % Cg) * 9 + tap) : 0.f);
+  }
+}
+
 // y[n, i, j, :] = x[n, 2i, 2j, :]: the pixels a 1x1 / stride-2 convolution reads, compacted so that the downsample
 // branch runs as a plain (TMA-fed) GEMM.  One thread per 16-byte vector.
 __global__ void subsample2_kernel(const bf16* __restrict__ x, bf16* __restrict__ y, int N, int H, int W, int C) {
@@ -570,6 +595,16 @@ extern "C" int byol_prep_weights_multi(const float* flat, void* pool_f, void* po
   // num_blocks = sum over units of byol_prep_unit_blocks(...) (the host knows the shapes; desc lives on the device)
   prep_weights_multi_kernel<<<num_blocks, 256, 0, stream>>>(flat, (bf16*)pool_f, (bf16*)pool_d, desc, num_units);
   return check_launch("prep_weights_multi_kernel");
+}
+
+// desc: device int64 [num_units][5] (see prep_weights_grouped_kernel); max_c: the largest C among the units
+extern "C" int byol_prep_weights_grouped(const float* flat, void* pool_f, void* pool_d, const int64_t* desc,
+                                         int num_units, int max_c, cudaStream_t stream) {
+  BYOL_CHECK_ARG(flat && pool_f && desc && num_units > 0 && num_units <= 65535 && max_c >= 64 && max_c % 64 == 0,
+                 "byol_prep_weights_grouped: bad args (num_units=%d max_c=%d)", num_units, max_c);
+  const dim3 grid((unsigned)grid_for((int64_t)max_c * 9 * 64, 256, 256), (unsigned)num_units);
+  prep_weights_grouped_kernel<<<grid, 256, 0, stream>>>(flat, (bf16*)pool_f, (bf16*)pool_d, desc);
+  return check_launch("prep_weights_grouped_kernel");
 }
 
 extern "C" int byol_subsample2(const void* x, void* y, int N, int H, int W, int C, cudaStream_t stream) {

@@ -32,7 +32,7 @@ F32 = torch.float32
 class _Unit(object):
     """One conv/linear (+ optional BN) layer: static geometry plus offsets into the flat parameter vector."""
     __slots__ = ("idx", "kind", "cin", "cout", "cpad", "k", "stride", "pad", "w_off", "w_numel", "b_off", "bn",
-                 "g_off", "beta_off", "name", "want_dgrad", "fold", "kcols")
+                 "g_off", "beta_off", "name", "want_dgrad", "fold", "kcols", "groups")
 
 
 class _Block(object):
@@ -43,6 +43,7 @@ class _Weights(object):
     """bf16 tensor-core layouts of one weight set (online or target)."""
 
     def __init__(self, units, device, want_dgrad):
+        # grouped units (ResNeXt conv2) keep block-diagonal tiles [C/64, 64, 9*64] in both layouts
         nf = sum(u.cout * u.kcols for u in units)
         self.pool_f = torch.empty(nf, dtype=BF16, device=device)
         self.pool_d = None
@@ -51,17 +52,21 @@ class _Weights(object):
         off = 0
         for u in units:
             n = u.cout * u.kcols
-            self.wf.append(self.pool_f[off:off + n].view(u.cout, u.kcols))
+            shape = (u.cout // 64, 64, u.kcols) if u.groups > 1 else (u.cout, u.kcols)
+            self.wf.append(self.pool_f[off:off + n].view(shape))
             self.off_f.append(off)
             off += n
         if want_dgrad:
-            nd = sum(u.cin * u.k * u.k * u.cout for u in units if u.want_dgrad)
+            nd = sum(u.cin * (u.kcols if u.groups > 1 else u.k * u.k * u.cout) for u in units if u.want_dgrad)
             self.pool_d = torch.empty(nd, dtype=BF16, device=device)
             off = 0
             for u in units:
                 if u.want_dgrad:
-                    n = u.cin * u.k * u.k * u.cout
-                    self.wd.append(self.pool_d[off:off + n].view(u.cin, u.k * u.k * u.cout))
+                    if u.groups > 1:
+                        n, shape = u.cin * u.kcols, (u.cin // 64, 64, u.kcols)
+                    else:
+                        n, shape = u.cin * u.k * u.k * u.cout, (u.cin, u.k * u.k * u.cout)
+                    self.wd.append(self.pool_d[off:off + n].view(shape))
                     self.off_d.append(off)
                     off += n
                 else:
@@ -70,9 +75,21 @@ class _Weights(object):
         else:
             self.wd = [None] * len(units)
             self.off_d = [-1] * len(units)
+        # descriptor tables of the grouped units' one-launch conversion (with and without the dgrad layouts)
+        grouped = [u for u in units if u.groups > 1]
+        self.grouped_max_c = max([u.cout for u in grouped] or [0])
+        self.gdesc_with_dgrad = self.gdesc_fprop_only = None
+        if grouped:
+            rows = [[u.w_off, self.off_f[u.idx], -1, u.cout, u.cin // u.groups] for u in grouped]
+            self.gdesc_fprop_only = torch.tensor(rows, dtype=torch.int64, device=device)
+            for r, u in zip(rows, grouped):
+                r[2] = self.off_d[u.idx]
+            self.gdesc_with_dgrad = torch.tensor(rows, dtype=torch.int64, device=device)
         # descriptor tables for the one-launch weight conversion (with and without the dgrad layouts)
         rows_d, rows_n = [], []
         for u in units:
+            if u.groups > 1:
+                continue
             fold = (u.k * 16 + u.k) if u.fold else 0
             base = [u.w_off, self.off_f[u.idx], -1, u.cout, u.cin, u.cpad, u.k * u.k, fold]
             rows_n.append(list(base))
@@ -239,17 +256,20 @@ class Engine(object):
         u.name = name
         if isinstance(mod, nn.Conv2d):
             assert mod.kernel_size[0] == mod.kernel_size[1] and mod.stride[0] == mod.stride[1]
-            assert mod.groups == 1 and mod.dilation[0] == 1 and mod.bias is None, "unsupported conv: %s" % name
+            assert mod.dilation[0] == 1 and mod.bias is None, "unsupported conv: %s" % name
             u.kind, u.cin, u.cout = "conv", mod.in_channels, mod.out_channels
             u.k, u.stride, u.pad = mod.kernel_size[0], mod.stride[0], mod.padding[0]
+            u.groups = mod.groups     # > 1: grouped 3x3 (model.check_grouped_convs ran at construction)
             u.b_off = -1
         else:
             u.kind, u.cin, u.cout, u.k, u.stride, u.pad = "linear", mod.in_features, mod.out_features, 1, 1, 0
+            u.groups = 1
             u.b_off = self.offsets[id(mod.bias)] if mod.bias is not None else -1
         u.cpad = (u.cin + 7) // 8 * 8
         # stem (3 input channels, 7x7): folded weight layout [Cout][KH*64] (see byol_prep_weight_fold)
         u.fold = u.kind == "conv" and u.cpad == 8 and 1 < u.k <= 8
-        u.kcols = u.k * 64 if u.fold else u.k * u.k * u.cpad
+        # grouped: one 64-channel k-block per tap (byol_prep_weights_grouped)
+        u.kcols = u.k * 64 if u.fold else u.k * u.k * (64 if u.groups > 1 else u.cpad)
         u.w_off = self.offsets[id(mod.weight)]
         u.w_numel = mod.weight.numel()
         u.bn = bn
@@ -332,8 +352,12 @@ class Engine(object):
 
     def prep_weights(self, flat, wset, want_dgrad):
         """fp32 master (flat vector) -> bf16 tensor-core layouts of every conv / linear, one launch."""
-        desc = wset.desc_with_dgrad if (want_dgrad and wset.pool_d is not None) else wset.desc_fprop_only
+        with_d = want_dgrad and wset.pool_d is not None
+        desc = wset.desc_with_dgrad if with_d else wset.desc_fprop_only
         ops.prep_weights_multi(flat, wset.pool_f, wset.pool_d, desc, wset.prep_blocks)
+        if wset.grouped_max_c:
+            ops.prep_weights_grouped(flat, wset.pool_f, wset.pool_d,
+                                     wset.gdesc_with_dgrad if with_d else wset.gdesc_fprop_only, wset.grouped_max_c)
         if wset.stem4_ok:
             st = self.stem
             ops.prep_weight_stem4(flat[st.w_off:st.w_off + st.w_numel].view(st.cout, st.cin, st.k, st.k),
@@ -842,7 +866,7 @@ class Engine(object):
         """dW += dY^T * im2col(X) on the side stream: the weight-gradient GEMMs only feed the flat gradient buffer, so
         they overlap with the HBM-bound BatchNorm-backward kernels of the next layer on the main stream.
         planes: xs / dys are split-operand planes (fp32-accurate backward)."""
-        dw = self._gview(u.w_off, u.w_numel).view(u.cout, u.cin, u.k, u.k)
+        dw = self._gview(u.w_off, u.w_numel).view(u.cout, u.cin // u.groups, u.k, u.k)
         launch = self._launch_wgrad_planes if planes else self._launch_wgrad
         main = torch.cuda.current_stream()
         side = self._side_stream

@@ -57,7 +57,32 @@ def _resnet(arch):
     if arch.startswith("resnet:"):   # custom depth: "resnet:<basic|bottleneck>:d1,d2,d3,d4"
         _, kind, depths = arch.split(":")
         return ResNet(Bottleneck if kind == "bottleneck" else BasicBlock, [int(d) for d in depths.split(",")])
+    if arch.startswith("resnext:"):  # custom ResNeXt: "resnext:<groups>x<width per group>:d1,d2,d3,d4"
+        _, gw, depths = arch.split(":")
+        g, w = gw.split("x")
+        return ResNet(Bottleneck, [int(d) for d in depths.split(",")], groups=int(g), width_per_group=int(w))
     raise ValueError("unknown arch %r" % arch)
+
+
+def check_grouped_convs(module, precision):
+    """Grouped convolutions run on the block-diagonal tile kernels only (3x3, pad 1, stride 1 or 2, Cin == Cout ==
+    C with C % 64 == 0, C / groups dividing 64) and only with bf16 operands.  Raises ValueError naming the first
+    layer that does not fit."""
+    for name, m in module.named_modules():
+        if not isinstance(m, nn.Conv2d) or m.groups == 1:
+            continue
+        c, g = m.in_channels, m.groups
+        ok = (m.kernel_size == (3, 3) and m.padding == (1, 1) and m.stride in ((1, 1), (2, 2)) and
+              m.dilation == (1, 1) and m.bias is None and m.out_channels == c and c % 64 == 0 and
+              64 % (c // g) == 0)
+        if not ok:
+            raise ValueError("byol_b200: grouped conv %s (%d -> %d, groups %d, kernel %s, stride %s, padding %s) is not "
+                             "supported: grouped convs must be 3x3 / pad 1 / stride 1 or 2 with Cin == Cout, a multiple "
+                             "of 64, and Cin / groups dividing 64" % (name, c, m.out_channels, g, m.kernel_size,
+                                                                     m.stride, m.padding))
+        if precision != "bf16":
+            raise ValueError("byol_b200: grouped conv %s: precision=%r is not supported for grouped convolutions "
+                             "(only 'bf16')" % (name, precision))
 
 
 class _OnlineTargetFn(torch.autograd.Function):
@@ -198,6 +223,7 @@ class BYOL(nn.Module):
                              "activations of the fp32-accurate forward), got precision=%r" % (precision,))
         if backward_precision == "fp32" and self._engine.fuse3:
             raise ValueError("backward_precision='fp32' does not support BYOL_B200_FUSE3=1")
+        check_grouped_convs(self, precision)
         self.precision = precision
         self.backward_precision = backward_precision
         self._engine.T = {"bf16": 0, "bf16x2": 3, "fp32": 6}[precision]

@@ -143,6 +143,28 @@ def prep_weights_multi(flat, pool_f, pool_d, desc, num_blocks=None):
                                       _stream()), "byol_prep_weights_multi")
 
 
+def prep_weights_grouped(flat, pool_f, pool_d, desc, max_c):
+    """All grouped 3x3 weights of one parameter set -> block-diagonal tile layouts, one launch.
+    desc: device int64 [units, 5] = [src offset, fprop offset, dgrad offset or -1, C, Cg]; max_c: the largest C."""
+    check(lib.byol_prep_weights_grouped(_ptr(flat), _ptr(pool_f), _ptr(pool_d), _ptr(desc), desc.shape[0], max_c,
+                                        _stream()), "byol_prep_weights_grouped")
+
+
+def prep_weight_grouped(w, want_dgrad=True):
+    """fp32 [C, Cg, 3, 3] -> (w_fprop, w_dgrad) bf16 [C/64, 64, 9*64] block-diagonal tiles (w_dgrad None unless
+    want_dgrad)."""
+    _chk(w, F32, "w")
+    c, cg = w.shape[0], w.shape[1]
+    if tuple(w.shape[2:]) != (3, 3) or c % 64 != 0 or 64 % cg != 0:
+        raise ValueError("prep_weight_grouped: need a [C, Cg, 3, 3] weight, C a multiple of 64 and Cg dividing 64, got %s"
+                         % (tuple(w.shape),))
+    wf = torch.empty((c // 64, 64, 9 * 64), dtype=BF16, device=w.device)
+    wd = torch.empty_like(wf) if want_dgrad else None
+    desc = torch.tensor([[0, 0, 0 if want_dgrad else -1, c, cg]], dtype=torch.int64, device=w.device)
+    prep_weights_grouped(w.reshape(-1), wf, wd, desc, c)
+    return wf, wd
+
+
 def prep_blocks(rows):
     """Grid size for prep_weights_multi: rows = [[src, dstf, dstd, Cout, Cin, Cpad, taps, fold], ...]."""
     return sum(lib.byol_prep_unit_blocks(int(r[3]), int(r[4]), int(r[5]), int(r[6]), int(r[7])) for r in rows)
@@ -170,12 +192,28 @@ def cast_bf16(x, out=None):
 # ------------------------------------------------------------------------------------------------
 # tensor-core convolution / linear
 # ------------------------------------------------------------------------------------------------
+def _grouped_unsupported(**options):
+    bad = sorted(k for k, v in options.items() if v is not None and v is not False)
+    if bad:
+        raise ValueError("grouped convolutions do not support %s" % ", ".join(bad))
+
+
 def conv_fprop(x, w_f, kh, kw, stride, pad, bias=None, resid=None, stats=None, relu=False, out_fp32=False,
                out=None, force_gather=False):
-    """y[N,Ho,Wo,Cout] = conv(x[N,H,W,C], w).  stats: optional zeroed fp32 [2*Cout] receiving column sum / sqsum."""
+    """y[N,Ho,Wo,Cout] = conv(x[N,H,W,C], w).  stats: optional zeroed fp32 [2*Cout] receiving column sum / sqsum.
+    A 3-D w_f is the grouped tile layout [C/64, 64, 9*64] of :func:`prep_weights_grouped` (grouped 3x3 conv)."""
     _chk(x, BF16, "x"); _chk(w_f, BF16, "w_f"); _chk(bias, F32, "bias"); _chk(resid, BF16, "resid")
     _chk(stats, F32, "stats")
     n, h, w, c = x.shape
+    if w_f.dim() == 3:
+        _grouped_unsupported(bias=bias, resid=resid, relu=relu, out_fp32=out_fp32, force_gather=force_gather)
+        ho, wo = conv_out_size(h, kh, stride, pad), conv_out_size(w, kw, stride, pad)
+        if out is None:
+            out = torch.empty((n, ho, wo, c), dtype=BF16, device=x.device)
+        cq = (stats.data_ptr() + 4 * c) if stats is not None else 0
+        check(lib.byol_conv_fprop_grouped(_ptr(x), _ptr(w_f), _ptr(out), _ptr(stats), cq, n, h, w, c, ho, wo, kh, kw,
+                                          stride, pad, _stream()), "byol_conv_fprop_grouped")
+        return out
     cout, ldw = w_f.shape
     ho, wo = conv_out_size(h, kh, stride, pad), conv_out_size(w, kw, stride, pad)
     if out is None:
@@ -192,9 +230,17 @@ def conv_dgrad(dy, w_d, h, w, kh, kw, stride, pad, resid=None, out=None, force_g
                resid_up=False):
     """dx[N,H,W,Cin] = conv_transpose(dy[N,Ho,Wo,Cout], w) (+ resid, optionally only where the bits of resid_mask,
     the uint8 ReLU mask written by bn_apply, are set; resid_up: resid is the compact [N, h/2, w/2, Cin] gradient of a
-    stride-2 branch, added to the even pixels);  w_d is the dgrad layout [Cin, taps*Cout]."""
+    stride-2 branch, added to the even pixels);  w_d is the dgrad layout [Cin, taps*Cout], or the grouped tile
+    layout [C/64, 64, 9*64] (3-D) of :func:`prep_weights_grouped`."""
     _chk(dy, BF16, "dy"); _chk(w_d, BF16, "w_d"); _chk(resid, BF16, "resid"); _chk(resid_mask, torch.uint8, "mask")
     n, ho, wo, cout = dy.shape
+    if w_d.dim() == 3:
+        _grouped_unsupported(resid=resid, resid_mask=resid_mask, resid_up=resid_up, force_gather=force_gather)
+        if out is None:
+            out = torch.empty((n, h, w, cout), dtype=BF16, device=dy.device)
+        check(lib.byol_conv_dgrad_grouped(_ptr(dy), _ptr(w_d), _ptr(out), n, ho, wo, cout, h, w, kh, kw, stride, pad,
+                                          _stream()), "byol_conv_dgrad_grouped")
+        return out
     cin, ldw = w_d.shape
     if out is None:
         out = torch.empty((n, h, w, cin), dtype=BF16, device=dy.device)
@@ -206,11 +252,21 @@ def conv_dgrad(dy, w_d, h, w, kh, kw, stride, pad, resid=None, out=None, force_g
 
 def conv_wgrad(x, dy, dw, kh, kw, stride, pad, force_gather=False):
     """dw[Cout,Cin,KH,KW] (fp32, reference layout) += dy^T * im2col(x).  x: [N,H,W,Cpad], dy: [N,Ho,Wo,ldy] whose
-    first Cout = dw.shape[0] columns are the gradient (ldy > Cout: pitched rows, e.g. a 10-class classifier)."""
+    first Cout = dw.shape[0] columns are the gradient (ldy > Cout: pitched rows, e.g. a 10-class classifier).
+    dw.shape[1] < C (C a multiple of 64, so not channel padding): a grouped 3x3 convolution with dw.shape[1] input
+    channels per group; only the in-group entries of dw are accumulated."""
     _chk(x, BF16, "x"); _chk(dy, BF16, "dy"); _chk(dw, F32, "dw")
     n, h, w, c = x.shape
     _, ho, wo, ldy = dy.shape
     cout, cin_real = dw.shape[0], dw.shape[1]
+    if cin_real < c and c % 64 == 0:
+        _grouped_unsupported(force_gather=force_gather)
+        if cout != c or ldy != c:
+            raise ValueError("grouped conv_wgrad: dw [%d, %d] and dy with %d channels do not match x with %d channels"
+                             % (cout, cin_real, ldy, c))
+        check(lib.byol_conv_wgrad_grouped(_ptr(x), _ptr(dy), _ptr(dw), n, h, w, c, cin_real, ho, wo, kh, kw, stride,
+                                          pad, _stream()), "byol_conv_wgrad_grouped")
+        return dw
     check(lib.byol_conv_wgrad(_ptr(x), _ptr(dy), _ptr(dw), n, h, w, c, cin_real, ho, wo, cout, ldy, kh, kw, stride,
                               pad, int(force_gather), _stream()), "byol_conv_wgrad")
     return dw

@@ -122,6 +122,24 @@ int byol_prep_weight_fold(const float* w, void* w_fprop, int Cout, int Cin, int 
 int byol_prep_unit_blocks(int Cout, int Cin, int Cpad, int taps, int fold);   /* blocks one unit needs */
 int byol_prep_weights_multi(const float* flat, void* pool_f, void* pool_d, const int64_t* desc, int num_units,
                             int num_blocks /* sum of byol_prep_unit_blocks over the units */, byol_stream_t stream);
+/* ---- grouped 3x3 convolutions (ResNeXt conv2, torchvision Bottleneck with groups > 1): Cin == Cout == C with
+ *      C % 64 == 0, Cg = C / groups dividing 64, 3x3, pad 1, stride 1 or 2.  A 64-channel output tile only meets its
+ *      own 64 input channels, so the weights are kept as block-diagonal tiles [C / 64][64][9 * 64]; each tile runs
+ *      9 k-blocks of 64 channels (64 / Cg times the algorithmic FLOPs).  Arguments are validated before any launch. */
+/* desc: device int64 [num_units][5] = {src offset in flat (fp32 [C][Cg][3][3]), fprop offset in pool_f,
+ * dgrad offset in pool_d or -1, C, Cg}; max_c: the largest C.  fprop column tap*64 + (ci - n0) for row co,
+ * dgrad column tap*64 + (co - n0) for row ci (n0 = the row's 64-aligned tile start); off-group entries are 0. */
+int byol_prep_weights_grouped(const float* flat, void* pool_f, void* pool_d, const int64_t* desc, int num_units,
+                              int max_c, byol_stream_t stream);
+/* y [Nimg, Ho, Wo, C] bf16; col_sum / col_sqsum (both or none): += per-channel sum / sum of squares of y */
+int byol_conv_fprop_grouped(const void* x, const void* wt, void* y, float* col_sum, float* col_sqsum, int Nimg, int H,
+                            int W, int C, int Ho, int Wo, int KH, int KW, int stride, int pad, byol_stream_t stream);
+/* dx [Nimg, H, W, C] bf16 from dy [Nimg, Ho, Wo, C] and the dgrad tiles */
+int byol_conv_dgrad_grouped(const void* dy, const void* wd, void* dx, int Nimg, int Ho, int Wo, int C, int H, int W,
+                            int KH, int KW, int stride, int pad, byol_stream_t stream);
+/* dw (fp32 [C][Cg][KH][KW], the parameter itself) += its in-group entries of dY^T x im2col(x); nothing else is written */
+int byol_conv_wgrad_grouped(const void* x, const void* dy, float* dw, int Nimg, int H, int W, int C, int Cg, int Ho,
+                            int Wo, int KH, int KW, int stride, int pad, byol_stream_t stream);
 /* y[n,i,j,:] = x[n,2i,2j,:] (input of a 1x1 / stride-2 downsample conv, compacted for the TMA-fed GEMM) */
 int byol_subsample2(const void* x, void* y, int N, int H, int W, int C, byol_stream_t stream);
 int byol_cast_f32_bf16(const float* x, void* y, int64_t n, byol_stream_t stream);
