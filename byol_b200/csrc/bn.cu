@@ -562,10 +562,7 @@ extern "C" int byol_bn_stats(const void* x, float* stats, int M, int C, cudaStre
   if (rows_per_block < 32) rows_per_block = 32;
   const int blocks = (M + rows_per_block - 1) / rows_per_block;
   const size_t red_bytes = 2 * (size_t)C * sizeof(Fix128);
-  if (red_bytes > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(bn_stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
-    if (e != cudaSuccess) { set_last_error("byol_bn_stats: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e)); return -2; }
-  }
+  if (smem_opt_in((const void*)bn_stats_kernel, (int)red_bytes, "bn_stats_kernel") != 0) return -2;
   Fix128* fx = fix_scratch(stream, 2 * (int64_t)C);
   if (fx == nullptr) return -2;
   bn_stats_kernel<<<blocks, 256, red_bytes, stream>>>((const bf16*)x, fx, fx + C, M, C, rows_per_block);
@@ -640,41 +637,20 @@ extern "C" int byol_bn_bwd_reduce(const void* g, const void* x, const void* act,
   BYOL_CHECK_ARG(red_bytes <= 226 * 1024, "byol_bn_bwd_reduce: C=%d too wide (at most 4800 channels)", C);
   const int fg = fixed_grid(nvec, C / 8);
   if (fg > 0) {
-    if (red_bytes > 48 * 1024) {   // wide layers: opt in to > 48 KB of dynamic smem for the per-block accumulators
-      cudaError_t e = cudaSuccess;
-      if (mask_mode == 0) e = cudaFuncSetAttribute(bn_bwd_reduce_fixed_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
-      else if (mask_mode == 1) e = cudaFuncSetAttribute(bn_bwd_reduce_fixed_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
-      else if (mask_mode == 2) e = cudaFuncSetAttribute(bn_bwd_reduce_fixed_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
-      else e = cudaFuncSetAttribute(bn_bwd_reduce_fixed_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
-      if (e != cudaSuccess) { set_last_error("byol_bn_bwd_reduce: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e)); return -2; }
-    }
-    if (mask_mode == 0)
-      bn_bwd_reduce_fixed_kernel<0><<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, nvec, C);
-    else if (mask_mode == 1)
-      bn_bwd_reduce_fixed_kernel<1><<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, nvec, C);
-    else if (mask_mode == 2)
-      bn_bwd_reduce_fixed_kernel<2><<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, nvec, C);
-    else
-      bn_bwd_reduce_fixed_kernel<3><<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, nvec, C);
+    static const decltype(&bn_bwd_reduce_fixed_kernel<0>) fixed_kernels[4] = {
+        bn_bwd_reduce_fixed_kernel<0>, bn_bwd_reduce_fixed_kernel<1>, bn_bwd_reduce_fixed_kernel<2>,
+        bn_bwd_reduce_fixed_kernel<3>};
+    const auto kern = fixed_kernels[mask_mode];
+    if (smem_opt_in((const void*)kern, (int)red_bytes, "bn_bwd_reduce_fixed_kernel") != 0) return -2;
+    kern<<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, nvec, C);
     if (check_launch("bn_bwd_reduce_fixed_kernel") != 0) return -100;
     return fix_done(stream, fix_flush(fx, s12, 2 * (int64_t)C, stream));
   }
-  if (red_bytes > 48 * 1024) {   // very wide BatchNorm1d (head_latent_size >= 6144): opt in to > 48 KB of dynamic smem
-    cudaError_t e = cudaSuccess;
-    if (mask_mode == 0) e = cudaFuncSetAttribute(bn_bwd_reduce_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
-    else if (mask_mode == 1) e = cudaFuncSetAttribute(bn_bwd_reduce_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
-    else if (mask_mode == 2) e = cudaFuncSetAttribute(bn_bwd_reduce_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
-    else e = cudaFuncSetAttribute(bn_bwd_reduce_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red_bytes);
-    if (e != cudaSuccess) { set_last_error("byol_bn_bwd_reduce: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e)); return -2; }
-  }
-  if (mask_mode == 0)
-    bn_bwd_reduce_kernel<0><<<blocks, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, M, C, rows_per_block);
-  else if (mask_mode == 1)
-    bn_bwd_reduce_kernel<1><<<blocks, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, M, C, rows_per_block);
-  else if (mask_mode == 2)
-    bn_bwd_reduce_kernel<2><<<blocks, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, M, C, rows_per_block);
-  else
-    bn_bwd_reduce_kernel<3><<<blocks, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, M, C, rows_per_block);
+  static const decltype(&bn_bwd_reduce_kernel<0>) kernels[4] = {bn_bwd_reduce_kernel<0>, bn_bwd_reduce_kernel<1>,
+                                                                 bn_bwd_reduce_kernel<2>, bn_bwd_reduce_kernel<3>};
+  const auto kern = kernels[mask_mode];
+  if (smem_opt_in((const void*)kern, (int)red_bytes, "bn_bwd_reduce_kernel") != 0) return -2;
+  kern<<<blocks, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, M, C, rows_per_block);
   if (check_launch("bn_bwd_reduce_kernel") != 0) return -100;
   return fix_done(stream, fix_flush(fx, s12, 2 * (int64_t)C, stream));
 }

@@ -1,6 +1,12 @@
-// byol_b200 — C-ABI plumbing shared by every entry point: thread-local error string, launch checks, version.
+// byol_b200 — C-ABI plumbing shared by every entry point: thread-local error string, launch checks, version, and the
+// host-side launch helpers (shared-memory opt-in, tensor maps, fixed-point scratch).
 #include <stdarg.h>
 #include <stdio.h>
+
+#include <atomic>
+#include <map>
+#include <mutex>
+#include <utility>
 
 #include "common.cuh"
 
@@ -32,15 +38,72 @@ int device_slot() {
 }
 
 int device_sm_count() {
-  static int n[kMaxDevices] = {};
+  static std::atomic<int> n[kMaxDevices] = {};
   const int slot = device_slot();
-  if (n[slot] == 0) {
-    int dev = 0, v = 0;
+  int v = n[slot].load(std::memory_order_relaxed);
+  if (v == 0) {
+    int dev = 0;
     cudaGetDevice(&dev);
     if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
-    n[slot] = v;
+    n[slot].store(v, std::memory_order_relaxed);
   }
-  return n[slot];
+  return v;
+}
+
+int smem_opt_in(const void* kernel, int bytes, const char* what) {
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, int> granted;   // (kernel, device slot) -> bytes
+  const std::lock_guard<std::mutex> lock(mu);
+  int& have = granted.emplace(std::make_pair(kernel, device_slot()), 48 * 1024).first->second;
+  if (bytes <= have) return 0;
+  const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) {
+    set_last_error("%s: cudaFuncSetAttribute(%d bytes of shared memory) failed: %s", what, bytes,
+                   cudaGetErrorString(e));
+    return -2;
+  }
+  have = bytes;
+  return 0;
+}
+
+int tmap_bf16(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims, const uint64_t* byte_strides,
+              const uint32_t* box, CUtensorMapSwizzle swizzle, const char* what) {
+  // decltype only names the driver function's type: the library resolves it at run time and does not link libcuda
+  static const auto encode = []() -> decltype(&cuTensorMapEncodeTiled) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess)
+      return nullptr;
+    return reinterpret_cast<decltype(&cuTensorMapEncodeTiled)>(fn);
+  }();
+  if (encode == nullptr) {
+    set_last_error("%s: cuTensorMapEncodeTiled entry point unavailable", what);
+    return -3;
+  }
+  const cuuint32_t elem_strides[5] = {1u, 1u, 1u, 1u, 1u};
+  const CUresult r = encode(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims,
+                            byte_strides, box, elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    char shape[384];   // at most 5 entries of < 72 characters
+    int len = snprintf(shape, sizeof(shape), "%llu (box %u)", (unsigned long long)dims[0], box[0]);
+    for (int i = 1; i < rank; ++i)
+      len += snprintf(shape + len, sizeof(shape) - len, ", %llu (box %u, stride %llu B)", (unsigned long long)dims[i],
+                      box[i], (unsigned long long)byte_strides[i - 1]);
+    set_last_error("%s: cuTensorMapEncodeTiled failed (%d): dims %s, base %p", what, (int)r, shape, base);
+    return -3;
+  }
+  return 0;
+}
+
+int tmap_2d(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
+            uint32_t box_cols, const char* what) {
+  const uint64_t dims[2] = {cols, rows};
+  const uint64_t strides[1] = {ld * sizeof(bf16)};
+  const uint32_t box[2] = {box_cols, box_rows};
+  return tmap_bf16(tm, base, 2, dims, strides, box,
+                   box_cols == 64u ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, what);
 }
 
 // Per-(device, stream) scratch for the fixed-point accumulators.  It only grows; a buffer that a captured CUDA graph
@@ -117,6 +180,12 @@ int fix_flush(Fix128* acc, float* dst, int64_t n, cudaStream_t stream) {
   if (blocks > 4 * 1024) blocks = 4 * 1024;
   fix_flush_kernel<<<(int)blocks, 256, 0, stream>>>(acc, dst, n);
   return check_launch("fix_flush_kernel");
+}
+
+int fix_flush_stats(Fix128* acc, float* col_sum, float* col_sqsum, int64_t n, cudaStream_t stream) {
+  const int rc = fix_flush(acc, col_sum, n, stream);
+  if (rc != 0) return rc;
+  return fix_done(stream, fix_flush(acc + n, col_sqsum, n, stream));
 }
 
 }  // namespace byol

@@ -17,11 +17,25 @@ typedef __nv_bfloat16 bf16;
 void set_last_error(const char* fmt, ...);
 int check_launch(const char* what);
 
-// One process may drive several GPUs: per-kernel attributes (cudaFuncSetAttribute) and the SM count are per device,
-// so the host wrappers cache them per device slot (capi.cu).
+// One process may drive several GPUs: per-kernel attributes (the shared-memory opt-in) and the SM count are per
+// device, so capi.cu caches them per device slot.
 static constexpr int kMaxDevices = 64;
 int device_slot();       // current CUDA device index, clamped to [0, kMaxDevices)
 int device_sm_count();   // SM count of the current device (cached per device; 132 if the query fails)
+
+// Lets `kernel` launch with `bytes` of dynamic shared memory on the current device.  The attribute is raised only
+// when a launch needs more than the kernel was granted there so far (48 KB need no opt-in).  0, or -2 on failure.
+int smem_opt_in(const void* kernel, int bytes, const char* what);
+
+// Tensor maps: every operand the kernels move by TMA is bf16, uninterleaved, promoted to L2 in 256-byte lines and
+// not OOB-filled (out-of-bounds elements load as zero).  dims[0] is the contiguous dimension; byte_strides holds the
+// rank - 1 strides of dims[1..].  0, or -3 when the map can not be encoded.
+int tmap_bf16(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims, const uint64_t* byte_strides,
+              const uint32_t* box, CUtensorMapSwizzle swizzle, const char* what);
+// 2-D map of `rows` x `cols` (cols contiguous, row pitch `ld` elements), box = box_rows x box_cols with box_cols = 64
+// (128-byte swizzle, operand loads) or 32 (64-byte swizzle, output stores)
+int tmap_2d(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
+            uint32_t box_cols, const char* what);
 
 // ----------------------------------------------------------------------------
 // Deterministic reductions.  Partial sums from many blocks are accumulated in fixed point: an addend x = v * 2^50
@@ -51,6 +65,9 @@ Fix128* fix_scratch(cudaStream_t stream, int64_t n);
 int fix_done(cudaStream_t stream, int rc);   // marks the stream's scratch clean when rc == 0; returns rc
 // dst[i] += value(acc[i]) for i < n (one fp32 addition per element); acc[i] is reset to zero
 int fix_flush(Fix128* acc, float* dst, int64_t n, cudaStream_t stream);
+// the fused column statistics: col_sum += acc[0, n), col_sqsum += acc[n, 2n), then fix_done.  A failed flush returns
+// without fix_done, so the next fix_scratch on the stream zeroes the accumulators again.
+int fix_flush_stats(Fix128* acc, float* col_sum, float* col_sqsum, int64_t n, cudaStream_t stream);
 
 __device__ __forceinline__ void fix_add_words(Fix128* acc, unsigned long long lo, long long hi) {
   atomicAdd(&acc->lo, lo);   // results unused: both compile to reductions

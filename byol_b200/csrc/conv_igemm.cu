@@ -887,47 +887,6 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_encodeTiled get_encode_fn() {
-  static PFN_encodeTiled fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres);
-    if (e != cudaSuccess || qres != cudaDriverEntryPointSuccess || ptr == nullptr) {
-      set_last_error("cuTensorMapEncodeTiled entry point unavailable (%s)", cudaGetErrorString(e));
-      return nullptr;
-    }
-    fn = (PFN_encodeTiled)ptr;
-  }
-  return fn;
-}
-
-// 2-D bf16 tensor map: `rows` x `cols` (cols contiguous), row pitch `ld` elements.
-// box = box_rows x box_cols with box_cols = 64 (128-byte swizzle, operand loads) or 32 (64-byte swizzle, output stores)
-static int make_tmap_2d(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
-                        uint32_t box_rows, uint32_t box_cols = 64u) {
-  PFN_encodeTiled fn = get_encode_fn();
-  if (fn == nullptr) return -1;
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * sizeof(bf16)};
-  cuuint32_t box[2] = {box_cols, box_rows};
-  cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  box_cols == 64u ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("cuTensorMapEncodeTiled failed (%d): rows=%llu cols=%llu ld=%llu box_rows=%u base=%p", (int)r,
-                   (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld, box_rows, base);
-    return -1;
-  }
-  return 0;
-}
-
 // gemm_fused.cu: plain GEMM with TMA-staged residual tile / per-column vectors in the epilogue
 bool gemm_fused_applicable(int M, int C, int Ndim, int ldw, int ldc);
 int gemm_fused_launch(const void* src, const void* wt, void* dst, const void* resid, const void* resid_mask,
@@ -946,25 +905,14 @@ bool patch_wgrad_applicable(int H, int W, int C, int Cin_real, int Cout, int KH,
 int patch_wgrad_launch(const void* x, const void* dy, float* dw, int Nimg, int H, int W, int C, int Cout, int sms,
                        cudaStream_t stream, int gs = 0);
 
-static int sm_count() { return device_sm_count(); }
-
 template <int BN, int STAGES, bool A_TMA, bool GROUPED = false>
 static int launch_igemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
                         const ConvGemmParams& p, int tiles_m, cudaStream_t stream) {
   using L = SmemLayout<BN, STAGES, A_TMA>;
   auto kern = conv_igemm_kernel<BN, STAGES, A_TMA, GROUPED>;
-  static bool attr_set[kMaxDevices] = {};
-  const int dev_slot = device_slot();
-  if (!attr_set[dev_slot]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
-    if (e != cudaSuccess) {
-      set_last_error("cudaFuncSetAttribute(conv_igemm) failed: %s", cudaGetErrorString(e));
-      return -2;
-    }
-    attr_set[dev_slot] = true;
-  }
+  if (smem_opt_in((const void*)kern, L::TOTAL, "conv_igemm_kernel") != 0) return -2;
   const int num_tiles = tiles_m * p.tiles_n;
-  int grid = sm_count();               // persistent: one CTA per SM (shared memory sized for it)
+  int grid = device_sm_count();        // persistent: one CTA per SM (shared memory sized for it)
   if (grid > num_tiles) grid = num_tiles;
   kern<<<grid, IG_THREADS, L::TOTAL, stream>>>(ta, tb, tc, p, num_tiles);
   return check_launch("conv_igemm_kernel");
@@ -1016,7 +964,7 @@ static int conv_igemm_impl(const void* src, const void* wt, void* dst, const voi
       ldw >= 9 * (grouped ? BK : C) &&
       patch_conv_applicable(Hs, Ws, C, Ndim, KH, KW, stride, pad, out_fp32, bias, (int64_t)Nimg * Hs * Ws * C))
     return patch_conv_launch(src, wt, dst, resid, col_sum, col_sqsum, Nimg, Hs, Ws, C, Ndim, ldw, ldc, mode, relu,
-                             sm_count(), stream, grouped);
+                             device_sm_count(), stream, grouped);
   ConvGemmParams p;
   memset(&p, 0, sizeof(p));
   p.src = (const bf16*)src;
@@ -1069,14 +1017,14 @@ static int conv_igemm_impl(const void* src, const void* wt, void* dst, const voi
 
   CUtensorMap ta, tb, tc;
   memset(&ta, 0, sizeof(ta));
-  if (make_tmap_2d(&tb, wt, (uint64_t)Ndim, (uint64_t)p.Kg, (uint64_t)ldw, (uint32_t)BN) != 0) return -3;
+  if (tmap_2d(&tb, wt, (uint64_t)Ndim, (uint64_t)p.Kg, (uint64_t)ldw, (uint32_t)BN, 64u, "conv_igemm B") != 0) return -3;
   if (!out_fp32) {
-    if (make_tmap_2d(&tc, dst, (uint64_t)p.M, (uint64_t)Ndim, (uint64_t)ldc, 32u, 32u) != 0) return -3;
+    if (tmap_2d(&tc, dst, (uint64_t)p.M, (uint64_t)Ndim, (uint64_t)ldc, 32u, 32u, "conv_igemm C") != 0) return -3;
   } else {
     tc = tb;
   }
   if (a_tma) {
-    if (make_tmap_2d(&ta, src, (uint64_t)p.M, (uint64_t)C, (uint64_t)C, (uint32_t)BM) != 0) return -3;
+    if (tmap_2d(&ta, src, (uint64_t)p.M, (uint64_t)C, (uint64_t)C, (uint32_t)BM, 64u, "conv_igemm A") != 0) return -3;
   } else {
     ta = tb;
   }
@@ -1095,8 +1043,7 @@ static int conv_igemm_impl(const void* src, const void* wt, void* dst, const voi
                : launch_igemm<64, 4, false>(ta, tb, tc, p, tiles_m, stream);
   }
   if (rc != 0 || col_sum == nullptr) return rc;
-  if ((rc = fix_flush(p.fx, col_sum, Ndim, stream)) != 0) return rc;
-  return fix_done(stream, fix_flush(p.fx + Ndim, col_sqsum, Ndim, stream));
+  return fix_flush_stats(p.fx, col_sum, col_sqsum, Ndim, stream);
 }
 
 extern "C" int byol_conv_igemm(const void* src, const void* wt, void* dst, const void* resid,
@@ -1164,16 +1111,7 @@ static int launch_wgrad(const CUtensorMap& ta, const CUtensorMap& tb, const Wgra
   constexpr int STAGES = 4;
   constexpr int SMEM = STAGES * (WG_A_STAGE + (BN / 64) * WG_KROWS * 128) + 256 + 1024;
   auto kern = conv_wgrad_kernel<BN, STAGES, B_TMA, GROUPED>;
-  static bool attr_set[kMaxDevices] = {};
-  const int dev_slot = device_slot();
-  if (!attr_set[dev_slot]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (e != cudaSuccess) {
-      set_last_error("cudaFuncSetAttribute(conv_wgrad) failed: %s", cudaGetErrorString(e));
-      return -2;
-    }
-    attr_set[dev_slot] = true;
-  }
+  if (smem_opt_in((const void*)kern, SMEM, "conv_wgrad_kernel") != 0) return -2;
   kern<<<grid, WG_THREADS, SMEM, stream>>>(ta, tb, p);
   return check_launch("conv_wgrad_kernel");
 }
@@ -1190,7 +1128,7 @@ static int conv_wgrad_impl(const void* src, const void* dy, float* dw, int Nimg,
   // gs > 0: grouped 3x3 convolution with gs = Cin_real input channels per group (byol_conv_wgrad_grouped)
   if (gs > 0) {
     if (!force_gather && Hs == Ho && Ws == Wo && patch_wgrad_applicable(Hs, Ws, C, C, Cout, KH, KW, stride, pad))
-      return patch_wgrad_launch(src, dy, dw, Nimg, Hs, Ws, C, Cout, sm_count(), stream, gs);
+      return patch_wgrad_launch(src, dy, dw, Nimg, Hs, Ws, C, Cout, device_sm_count(), stream, gs);
   }
   BYOL_CHECK_ARG(C % 8 == 0 && ldy % 8 == 0 && ldy >= Cout && Cout > 0,
                  "byol_conv_wgrad: C=%d and the dy pitch %d must be multiples of 8 (Cout=%d)", C, ldy, Cout);
@@ -1200,7 +1138,7 @@ static int conv_wgrad_impl(const void* src, const void* dy, float* dw, int Nimg,
   BYOL_CHECK_ARG(M64 > 0 && M64 < (1ll << 31), "byol_conv_wgrad: M out of range");
   // 3x3 / stride 1 / pad 1: shifted-window kernel over TMA patches (no gather)
   if (T == 0 && !force_gather && ldy == Cout && Hs == Ho && Ws == Wo && patch_wgrad_applicable(Hs, Ws, C, Cin_real, Cout, KH, KW, stride, pad))
-    return patch_wgrad_launch(src, dy, dw, Nimg, Hs, Ws, C, Cout, sm_count(), stream);
+    return patch_wgrad_launch(src, dy, dw, Nimg, Hs, Ws, C, Cout, device_sm_count(), stream);
   const int terms = T == 0 ? 1 : T;
   WgradParams p;
   memset(&p, 0, sizeof(p));
@@ -1235,7 +1173,7 @@ static int conv_wgrad_impl(const void* src, const void* dy, float* dw, int Nimg,
   // The epilogue adds 128 x BN values per CTA to the gradient with L2 reductions, so the split count trades
   // parallelism against reduction traffic: exactly one resident wave (one CTA per SM), rounded DOWN so that no
   // second, nearly empty wave appears.
-  const int target_ctas = sm_count();
+  const int target_ctas = device_sm_count();
   int splits = target_ctas / base_ctas;
   int max_splits = (p.num_kb_total + 7) / 8;                // at least 8 k-blocks (512 pixels) per CTA
   if (max_splits < 1) max_splits = 1;
@@ -1250,9 +1188,11 @@ static int conv_wgrad_impl(const void* src, const void* dy, float* dw, int Nimg,
   CUtensorMap ta, tb;
   // plain operands: the map ends at column Cout (TMA zero-fills a co tile past it); planes: all terms side by side
   const uint64_t dy_cols = T == 0 ? (uint64_t)Cout : (uint64_t)terms * ldy;
-  if (make_tmap_2d(&ta, dy, (uint64_t)p.M, dy_cols, (uint64_t)terms * ldy, (uint32_t)WG_KROWS) != 0) return -3;
+  if (tmap_2d(&ta, dy, (uint64_t)p.M, dy_cols, (uint64_t)terms * ldy, (uint32_t)WG_KROWS, 64u, "conv_wgrad dY") != 0)
+    return -3;
   if (b_tma) {
-    if (make_tmap_2d(&tb, src, (uint64_t)p.M, (uint64_t)p.ldsrc, (uint64_t)p.ldsrc, (uint32_t)WG_KROWS) != 0) return -3;
+    if (tmap_2d(&tb, src, (uint64_t)p.M, (uint64_t)p.ldsrc, (uint64_t)p.ldsrc, (uint32_t)WG_KROWS, 64u, "conv_wgrad X") != 0)
+      return -3;
   } else {
     tb = ta;
   }

@@ -316,42 +316,25 @@ conv3x3_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
   }
 }
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_encodeTiled patch_encode_fn() {
-  static PFN_encodeTiled fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = (PFN_encodeTiled)ptr;
-  }
-  return fn;
-}
-
 template <int BN, bool GROUPED = false>
 static int launch_patch(const CUtensorMap& tx, const CUtensorMap& tb, const PatchParams& p, int sms,
                         cudaStream_t stream) {
   constexpr int SMEM = P_PSTAGES * 2 * P_PATCH_SLOT + P_BSTAGES * BN * 128 + 4 * 2048 + 128 * P_ACC_LD * 4 + 256 + 1024;
   static_assert(SMEM <= 232448, "conv3x3_patch_kernel: shared memory");
   auto kern = conv3x3_patch_kernel<BN, GROUPED>;
-  static bool attr_set[kMaxDevices] = {};
-  const int dev_slot = device_slot();
-  if (!attr_set[dev_slot]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (e != cudaSuccess) {
-      set_last_error("cudaFuncSetAttribute(conv3x3_patch) failed: %s", cudaGetErrorString(e));
-      return -2;
-    }
-    attr_set[dev_slot] = true;
-  }
+  if (smem_opt_in((const void*)kern, SMEM, "conv3x3_patch_kernel") != 0) return -2;
   int grid = sms < p.num_tiles ? sms : p.num_tiles;
   kern<<<grid, P_THREADS, SMEM, stream>>>(tx, tb, p);
   return check_launch("conv3x3_patch_kernel");
+}
+
+// NHWC activation [Nimg][H][W][C] as a 4-D map; box = 64 channels x box_w pixels x box_h rows of one image
+static int tmap_nhwc(CUtensorMap* tm, const void* base, int Nimg, int H, int W, int C, int box_w, int box_h,
+                     const char* what) {
+  const uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)Nimg};
+  const uint64_t strides[3] = {(uint64_t)C * 2, (uint64_t)W * C * 2, (uint64_t)H * W * C * 2};
+  const uint32_t box[4] = {64u, (uint32_t)box_w, (uint32_t)box_h, 1u};
+  return tmap_bf16(tm, base, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, what);
 }
 
 // Is the patch formulation applicable / worthwhile for this geometry?
@@ -373,8 +356,6 @@ bool patch_conv_applicable(int H, int W, int C, int Ndim, int KH, int KW, int st
 int patch_conv_launch(const void* src, const void* wt, void* dst, const void* resid, float* col_sum, float* col_sqsum,
                       int Nimg, int H, int W, int C, int Ndim, int ldw, int ldc, int flip, int relu, int sms,
                       cudaStream_t stream, int grouped) {
-  PFN_encodeTiled fn = patch_encode_fn();
-  if (fn == nullptr) { set_last_error("cuTensorMapEncodeTiled entry point unavailable"); return -3; }
   PatchParams p;
   memset(&p, 0, sizeof(p));
   p.dst = dst; p.resid = (const bf16*)resid; p.col_sum = col_sum; p.col_sqsum = col_sqsum;
@@ -394,34 +375,17 @@ int patch_conv_launch(const void* src, const void* wt, void* dst, const void* re
   p.patch_bytes = 128u * (uint32_t)p.Wp * (uint32_t)(p.TH + 2);
 
   CUtensorMap tx, tb;
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)Nimg};
-    cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-    cuuint32_t box[4] = {64u, (cuuint32_t)p.Wp, (cuuint32_t)(p.TH + 2), 1u};
-    cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
-    CUresult r = fn(&tx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(src), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_last_error("patch conv: 4-D tensor map encode failed (%d)", (int)r); return -3; }
-  }
-  {
-    cuuint64_t dims[2] = {(cuuint64_t)(9 * 64 * p.nchunks), (cuuint64_t)Ndim};
-    cuuint64_t strides[1] = {(cuuint64_t)ldw * 2};
-    cuuint32_t box[2] = {64u, (cuuint32_t)BN};
-    cuuint32_t estr[2] = {1u, 1u};
-    CUresult r = fn(&tb, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(wt), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_last_error("patch conv: weight tensor map encode failed (%d)", (int)r); return -3; }
-  }
+  if (tmap_nhwc(&tx, src, Nimg, H, W, C, p.Wp, p.TH + 2, "conv3x3_patch X") != 0) return -3;
+  if (tmap_2d(&tb, wt, (uint64_t)Ndim, (uint64_t)(9 * 64 * p.nchunks), (uint64_t)ldw, (uint32_t)BN, 64u,
+              "conv3x3_patch B") != 0)
+    return -3;
   if (col_sum != nullptr) {
     p.fx = fix_scratch(stream, 2 * (int64_t)Ndim);
     if (p.fx == nullptr) return -2;
   }
   int rc = grouped ? launch_patch<64, true>(tx, tb, p, sms, stream) : launch_patch<64>(tx, tb, p, sms, stream);
   if (rc != 0 || col_sum == nullptr) return rc;
-  if ((rc = fix_flush(p.fx, col_sum, Ndim, stream)) != 0) return rc;
-  return fix_done(stream, fix_flush(p.fx + Ndim, col_sqsum, Ndim, stream));
+  return fix_flush_stats(p.fx, col_sum, col_sqsum, Ndim, stream);
 }
 
 }  // namespace byol
@@ -584,16 +548,7 @@ static int launch_wpatch(const CUtensorMap& tx, const CUtensorMap& ty, const WPa
                          cudaStream_t stream) {
   constexpr int SMEM = WP_STAGES * (NB * P_PATCH_SLOT + 2 * 16384) + 256 + 1024;
   auto kern = conv3x3_wgrad_patch_kernel<NB, GROUPED>;
-  static bool attr_set[kMaxDevices] = {};
-  const int dev_slot = device_slot();
-  if (!attr_set[dev_slot]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (e != cudaSuccess) {
-      set_last_error("cudaFuncSetAttribute(conv3x3_wgrad_patch) failed: %s", cudaGetErrorString(e));
-      return -2;
-    }
-    attr_set[dev_slot] = true;
-  }
+  if (smem_opt_in((const void*)kern, SMEM, "conv3x3_wgrad_patch_kernel") != 0) return -2;
   kern<<<grid, WP_THREADS, SMEM, stream>>>(tx, ty, p);
   return check_launch("conv3x3_wgrad_patch_kernel");
 }
@@ -612,8 +567,6 @@ bool patch_wgrad_applicable(int H, int W, int C, int Cin_real, int Cout, int KH,
 // gs > 0: grouped convolution (Cout == C) with gs input channels per group; dw is then [Cout][gs][3][3]
 int patch_wgrad_launch(const void* x, const void* dy, float* dw, int Nimg, int H, int W, int C, int Cout, int sms,
                        cudaStream_t stream, int gs) {
-  PFN_encodeTiled fn = patch_encode_fn();
-  if (fn == nullptr) { set_last_error("cuTensorMapEncodeTiled entry point unavailable"); return -3; }
   WPatchParams p;
   memset(&p, 0, sizeof(p));
   p.dw = dw; p.Nimg = Nimg; p.H = H; p.W = W; p.C = C; p.Cout = Cout;
@@ -636,17 +589,8 @@ int patch_wgrad_launch(const void* x, const void* dy, float* dw, int Nimg, int H
   p.patch_bytes = 128u * (uint32_t)p.Wp * (uint32_t)(p.TH + 2);
   p.dy_bytes = 128u * (uint32_t)p.Wp * (uint32_t)p.TH;
   CUtensorMap tx, ty;
-  for (int which = 0; which < 2; ++which) {
-    const int ch = which == 0 ? C : Cout;
-    cuuint64_t dims[4] = {(cuuint64_t)ch, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)Nimg};
-    cuuint64_t strides[3] = {(cuuint64_t)ch * 2, (cuuint64_t)W * ch * 2, (cuuint64_t)H * W * ch * 2};
-    cuuint32_t box[4] = {64u, (cuuint32_t)p.Wp, (cuuint32_t)(which == 0 ? p.TH + 2 : p.TH), 1u};
-    cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
-    CUresult r = fn(which == 0 ? &tx : &ty, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4,
-                    const_cast<void*>(which == 0 ? x : dy), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_last_error("patch wgrad: tensor map encode failed (%d)", (int)r); return -3; }
-  }
+  if (tmap_nhwc(&tx, x, Nimg, H, W, C, p.Wp, p.TH + 2, "conv3x3_wgrad_patch X") != 0) return -3;
+  if (tmap_nhwc(&ty, dy, Nimg, H, W, Cout, p.Wp, p.TH, "conv3x3_wgrad_patch dY") != 0) return -3;
   const int grid = base * p.splits;
   const int64_t ndw = (int64_t)Cout * (gs > 0 ? gs : C) * 9;
   p.fx = fix_scratch(stream, ndw);

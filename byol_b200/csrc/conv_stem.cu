@@ -433,25 +433,6 @@ __global__ void prep_weight_stem4_kernel(const float* __restrict__ w, bf16* __re
 
 using namespace byol;
 
-typedef CUresult (*PFN_encodeTiledStem)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                        const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                        CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_encodeTiledStem stem_encode_fn() {
-  static PFN_encodeTiledStem fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = (PFN_encodeTiledStem)ptr;
-  }
-  return fn;
-}
-
-static int stem_sm_count() { return device_sm_count(); }
-
 // 1 if the stem kernels handle this geometry (otherwise use byol_conv_igemm / byol_conv_wgrad with the NHWC8 input)
 extern "C" int byol_stem4_supported(int Cin, int Cout, int H, int W, int k, int stride, int pad) {
   return (Cin >= 1 && Cin <= 4 && Cout == 64 && k == 7 && stride == 2 && pad == 3 && H >= 2 && H % 2 == 0 &&
@@ -492,34 +473,22 @@ extern "C" int byol_stem_conv_fprop(const void* xs, const void* ws, void* y, flo
   p.N = N; p.Ho = Ho; p.Wo = Wo;
   p.pairs_per_img = (H + 6) / 2;
   p.num_tiles = N * Ho;
-  PFN_encodeTiledStem fn = stem_encode_fn();
-  if (fn == nullptr) { set_last_error("byol_stem_conv_fprop: cuTensorMapEncodeTiled unavailable"); return -3; }
   CUtensorMap tmY;
-  cuuint64_t dims[3] = {64, (cuuint64_t)Wo, (cuuint64_t)N * Ho};
-  cuuint64_t strides[2] = {128, (cuuint64_t)Wo * 128};
-  cuuint32_t box[3] = {32, 32, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(&tmY, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, y, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_last_error("byol_stem_conv_fprop: tensor map encode failed (%d)", (int)r); return -3; }
-  static bool attr_set[kMaxDevices] = {};
-  const int dev_slot = device_slot();
-  if (!attr_set[dev_slot]) {
-    cudaError_t e = cudaFuncSetAttribute(stem_fprop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ST_TOTAL);
-    if (e != cudaSuccess) { set_last_error("cudaFuncSetAttribute(stem_fprop) failed: %s", cudaGetErrorString(e)); return -2; }
-    attr_set[dev_slot] = true;
-  }
-  int grid = stem_sm_count();
+  const uint64_t dims[3] = {64, (uint64_t)Wo, (uint64_t)N * Ho};
+  const uint64_t strides[2] = {128, (uint64_t)Wo * 128};
+  const uint32_t box[3] = {32, 32, 1};
+  if (tmap_bf16(&tmY, y, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B, "byol_stem_conv_fprop Y") != 0) return -3;
+  if (smem_opt_in((const void*)stem_fprop_kernel, ST_TOTAL, "stem_fprop_kernel") != 0) return -2;
+  int grid = device_sm_count();
   if (grid > p.num_tiles) grid = p.num_tiles;
   if (col_sum != nullptr) {
     p.fx = fix_scratch(stream, 128);
     if (p.fx == nullptr) return -2;
   }
   stem_fprop_kernel<<<grid, ST_THREADS, ST_TOTAL, stream>>>(tmY, p);
-  int rc = check_launch("stem_fprop_kernel");
+  const int rc = check_launch("stem_fprop_kernel");
   if (rc != 0 || col_sum == nullptr) return rc;
-  if ((rc = fix_flush(p.fx, col_sum, 64, stream)) != 0) return rc;
-  return fix_done(stream, fix_flush(p.fx + 64, col_sqsum, 64, stream));
+  return fix_flush_stats(p.fx, col_sum, col_sqsum, 64, stream);
 }
 
 // dw[64][Cin][7][7] (fp32) += dY^T * im2col(xs); dy: [N, H/2, W/2, 64] bf16
@@ -539,25 +508,13 @@ extern "C" int byol_stem_conv_wgrad(const void* xs, const void* dy, float* dw, i
   // (for no-swizzle MN-major operands the roles are swapped w.r.t. K-major)
   p.b_lbo = 128u;
   p.b_sbo = 16u;
-  PFN_encodeTiledStem fn = stem_encode_fn();
-  if (fn == nullptr) { set_last_error("byol_stem_conv_wgrad: cuTensorMapEncodeTiled unavailable"); return -3; }
   CUtensorMap tmDY;
-  cuuint64_t dims[4] = {64, (cuuint64_t)Wo, (cuuint64_t)Ho, (cuuint64_t)N};
-  cuuint64_t strides[3] = {128, (cuuint64_t)Wo * 128, (cuuint64_t)Ho * Wo * 128};
-  cuuint32_t box[4] = {64, 128, 1, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = fn(&tmDY, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(dy), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_last_error("byol_stem_conv_wgrad: tensor map encode failed (%d)", (int)r); return -3; }
-  static bool attr_set[kMaxDevices] = {};
-  const int dev_slot = device_slot();
-  if (!attr_set[dev_slot]) {
-    cudaError_t e = cudaFuncSetAttribute(stem_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SW_TOTAL);
-    if (e != cudaSuccess) { set_last_error("cudaFuncSetAttribute(stem_wgrad) failed: %s", cudaGetErrorString(e)); return -2; }
-    attr_set[dev_slot] = true;
-  }
-  int grid = stem_sm_count();
+  const uint64_t dims[4] = {64, (uint64_t)Wo, (uint64_t)Ho, (uint64_t)N};
+  const uint64_t strides[3] = {128, (uint64_t)Wo * 128, (uint64_t)Ho * Wo * 128};
+  const uint32_t box[4] = {64, 128, 1, 1};
+  if (tmap_bf16(&tmDY, dy, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, "byol_stem_conv_wgrad dY") != 0) return -3;
+  if (smem_opt_in((const void*)stem_wgrad_kernel, SW_TOTAL, "stem_wgrad_kernel") != 0) return -2;
+  int grid = device_sm_count();
   if (grid > p.num_units) grid = p.num_units;
   const int64_t ndw = (int64_t)64 * Cin * 49;
   p.fx = fix_scratch(stream, ndw);

@@ -379,42 +379,6 @@ gemm_fused_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
 }
 
 // ---------------------------------------------------------------------------------------------
-typedef CUresult (*PFN_encodeTiledGF)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                      const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                      CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_encodeTiledGF gf_encode_fn() {
-  static PFN_encodeTiledGF fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = (PFN_encodeTiledGF)ptr;
-  }
-  return fn;
-}
-
-static int gf_tmap(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,
-                   uint32_t box_cols) {
-  PFN_encodeTiledGF fn = gf_encode_fn();
-  if (fn == nullptr) { set_last_error("cuTensorMapEncodeTiled entry point unavailable"); return -1; }
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * sizeof(bf16)};
-  cuuint32_t box[2] = {box_cols, box_rows};
-  cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, box_cols == 64u ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("gemm_fused: cuTensorMapEncodeTiled failed (%d): rows=%llu cols=%llu ld=%llu", (int)r,
-                   (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld);
-    return -1;
-  }
-  return 0;
-}
-
 // true if the rich-epilogue kernel can run this GEMM (the caller falls back to conv_igemm_kernel otherwise)
 bool gemm_fused_applicable(int M, int C, int Ndim, int ldw, int ldc) {
   return M > 0 && C % 8 == 0 && Ndim > 64 && Ndim % 8 == 0 && ldc % 8 == 0 && ldc >= Ndim && ldw % 8 == 0 && ldw >= C;
@@ -452,19 +416,13 @@ int gemm_fused_launch(const void* src, const void* wt, void* dst, const void* re
   const int tiles_m = (M + GF_BM - 1) / GF_BM;
   const int num_tiles = tiles_m * p.tiles_n;
   CUtensorMap ta, tb, tc, tr;
-  if (gf_tmap(&ta, src, (uint64_t)M, (uint64_t)C, (uint64_t)C, GF_BM, 64u) != 0) return -3;
-  if (gf_tmap(&tb, wt, (uint64_t)Ndim, (uint64_t)C, (uint64_t)ldw, GF_BN, 64u) != 0) return -3;
-  if (!no_dst) { if (gf_tmap(&tc, dst, (uint64_t)M, (uint64_t)Ndim, (uint64_t)ldc, 32u, 32u) != 0) return -3; }
+  if (tmap_2d(&ta, src, (uint64_t)M, (uint64_t)C, (uint64_t)C, GF_BM, 64u, "gemm_fused A") != 0) return -3;
+  if (tmap_2d(&tb, wt, (uint64_t)Ndim, (uint64_t)C, (uint64_t)ldw, GF_BN, 64u, "gemm_fused B") != 0) return -3;
+  if (!no_dst) { if (tmap_2d(&tc, dst, (uint64_t)M, (uint64_t)Ndim, (uint64_t)ldc, 32u, 32u, "gemm_fused C") != 0) return -3; }
   else tc = tb;
-  if (resid != nullptr) { if (gf_tmap(&tr, resid, (uint64_t)M, (uint64_t)Ndim, (uint64_t)ldc, 32u, 32u) != 0) return -3; }
+  if (resid != nullptr) { if (tmap_2d(&tr, resid, (uint64_t)M, (uint64_t)Ndim, (uint64_t)ldc, 32u, 32u, "gemm_fused R") != 0) return -3; }
   else tr = tb;
-  static bool attr_set[kMaxDevices] = {};
-  const int dev_slot = device_slot();
-  if (!attr_set[dev_slot]) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GF_TOTAL);
-    if (e != cudaSuccess) { set_last_error("cudaFuncSetAttribute(gemm_fused) failed: %s", cudaGetErrorString(e)); return -2; }
-    attr_set[dev_slot] = true;
-  }
+  if (smem_opt_in((const void*)gemm_fused_kernel, GF_TOTAL, "gemm_fused_kernel") != 0) return -2;
   int grid = device_sm_count();
   if (grid > num_tiles) grid = num_tiles;
   if (col_sum != nullptr) {
@@ -474,8 +432,7 @@ int gemm_fused_launch(const void* src, const void* wt, void* dst, const void* re
   gemm_fused_kernel<<<grid, GF_THREADS, GF_TOTAL, stream>>>(ta, tb, tc, tr, p, num_tiles);
   int rc = check_launch("gemm_fused_kernel");
   if (rc != 0 || col_sum == nullptr) return rc;
-  if ((rc = fix_flush(p.fx, col_sum, Ndim, stream)) != 0) return rc;
-  return fix_done(stream, fix_flush(p.fx + Ndim, col_sqsum, Ndim, stream));
+  return fix_flush_stats(p.fx, col_sum, col_sqsum, Ndim, stream);
 }
 
 }  // namespace byol

@@ -387,37 +387,6 @@ mlp_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmapX, const __grid_con
   }
 }
 
-typedef CUresult (*PFN_encodeTiledMF)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                      const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                      CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static int mf_tmap(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
-  static PFN_encodeTiledMF fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess) {
-      set_last_error("cuTensorMapEncodeTiled entry point unavailable");
-      return -1;
-    }
-    fn = (PFN_encodeTiledMF)ptr;
-  }
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * sizeof(bf16)};
-  cuuint32_t box[2] = {64u, box_rows};
-  cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("mlp_fused: cuTensorMapEncodeTiled failed (%d): rows=%llu cols=%llu ld=%llu box_rows=%u", (int)r,
-                   (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld, box_rows);
-    return -1;
-  }
-  return 0;
-}
-
 }  // namespace byol
 
 using namespace byol;
@@ -463,22 +432,16 @@ extern "C" int byol_mlp_fused_fwd(const void* x, const void* w1, const float* b1
   p.peer.counter = (uint32_t*)counter;
   for (int r = 0; r < 8; ++r) p.peer.p[r] = (world > 1 && r < world) ? peer_ptrs[r] : 0ull;
   CUtensorMap tx, tw1, tw2, th, ta;
-  if (mf_tmap(&tx, x, (uint64_t)B, (uint64_t)K1, (uint64_t)K1, 128u) != 0) return -3;
-  if (mf_tmap(&tw1, w1, (uint64_t)H, (uint64_t)K1, (uint64_t)ldw1, 128u) != 0) return -3;
-  if (mf_tmap(&tw2, w2, (uint64_t)O, (uint64_t)H, (uint64_t)ldw2, (uint32_t)O) != 0) return -3;
+  if (tmap_2d(&tx, x, (uint64_t)B, (uint64_t)K1, (uint64_t)K1, 128u, 64u, "mlp_fused X") != 0) return -3;
+  if (tmap_2d(&tw1, w1, (uint64_t)H, (uint64_t)K1, (uint64_t)ldw1, 128u, 64u, "mlp_fused W1") != 0) return -3;
+  if (tmap_2d(&tw2, w2, (uint64_t)O, (uint64_t)H, (uint64_t)ldw2, (uint32_t)O, 64u, "mlp_fused W2") != 0) return -3;
   if (p.save) {
-    if (mf_tmap(&th, h_save, (uint64_t)B, (uint64_t)H, (uint64_t)H, 128u) != 0) return -3;
-    if (mf_tmap(&ta, a_save, (uint64_t)B, (uint64_t)H, (uint64_t)H, 128u) != 0) return -3;
+    if (tmap_2d(&th, h_save, (uint64_t)B, (uint64_t)H, (uint64_t)H, 128u, 64u, "mlp_fused h_save") != 0) return -3;
+    if (tmap_2d(&ta, a_save, (uint64_t)B, (uint64_t)H, (uint64_t)H, 128u, 64u, "mlp_fused a_save") != 0) return -3;
   } else {
     th = tx; ta = tx;
   }
-  static bool attr_set[kMaxDevices] = {};
-  const int dev_slot = device_slot();
-  if (!attr_set[dev_slot]) {
-    cudaError_t e = cudaFuncSetAttribute(mlp_fused_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MF_TOTAL);
-    if (e != cudaSuccess) { set_last_error("cudaFuncSetAttribute(mlp_fused) failed: %s", cudaGetErrorString(e)); return -2; }
-    attr_set[dev_slot] = true;
-  }
+  if (smem_opt_in((const void*)mlp_fused_fwd_kernel, MF_TOTAL, "mlp_fused_fwd_kernel") != 0) return -2;
   const int grid = ((B + 127) / 128) * p.tiles_h;
   // cooperative launch: every CTA must be resident for the grid barrier
   cudaLaunchConfig_t cfg;
