@@ -36,7 +36,7 @@ class _Unit(object):
 
 
 class _Block(object):
-    __slots__ = ("kind", "c1", "c2", "c3", "down")
+    __slots__ = ("kind", "c1", "c2", "c3", "down", "idx")
 
 
 class _Weights(object):
@@ -192,6 +192,11 @@ class Engine(object):
         # projector / predictor forward as one cooperative kernel per lane (csrc/mlp_fused.cu); =0: four launches
         self.fused_mlp = os.environ.get("BYOL_B200_FUSED_MLP", "1") != "0"
         self._mlp_bar = None
+        # activation recomputation (recompute_plan): per geometry the set of blocks whose online lanes keep only the
+        # block input, the BN coefficients and the output mask; _recompute_now is the set of the running forward
+        self._plans = {}
+        self._recompute_now = frozenset()
+        self._mem_budget = None     # bytes: replaces the device's free memory in recompute_plan (tests)
 
     # ------------------------------------------------------------------------------------------
     # flat buffers
@@ -281,7 +286,35 @@ class Engine(object):
         return u
 
     def build_plan(self):
+        self.walk_layers()
+        self.module_key = self._module_key()
+        self.bn_modules = [u.bn for u in self.units if u.bn is not None]
+        self.bn_channels = sum(u.cout for u in self.units if u.bn is not None)
+        self.sync = any(isinstance(b, nn.SyncBatchNorm) for b in self.bn_modules)
+        self._side_stream = torch.cuda.Stream(device=self.device) if self.overlap_wgrad else None
+        # the same two streams serve the forward lane pairs and the backward views: every extra stream is an extra
+        # caching-allocator pool, and pools do not share their cached blocks
+        self._fwd_streams = [torch.cuda.Stream(device=self.device) for _ in range(2)]
+        self._bwd_streams = self._fwd_streams
+        self.w_online = _Weights(self.units, self.device, True)
+        self.w_target = _Weights(self.units, self.device, False)
+        self.graphs = {}           # captured steps point into the old buffers
+        self._plans = {}
+        self.s_online = self.s_target = None
+        if self.T:
+            self.s_online = _SplitWeights(self.units, self.device, self.T, want_dgrad=self.bwd32)
+            self.s_target = _SplitWeights(self.units, self.device, self.T)
+        self.ready = True
+
+    def walk_layers(self):
+        """Units and blocks of the module tree (geometry and flat offsets).  Needs no device: before flatten() the
+        offsets are those flatten() will assign."""
         model = self.model
+        if not self.is_flat():
+            self.offsets, off = {}, 0
+            for p in model.parameters():
+                self.offsets[id(p)] = off
+                off += p.numel()
         self.units, self.blocks = [], []
         children = list(model.base_network.children())
         convs = [c for c in children if isinstance(c, nn.Conv2d)]
@@ -303,6 +336,7 @@ class Engine(object):
                 if blk.downsample is not None:
                     d = list(blk.downsample.children())
                     b.down = self._unit(d[0], d[1], "down")
+                b.idx = len(self.blocks)
                 self.blocks.append(b)
         self.rep_dim = (self.blocks[-1].c3 or self.blocks[-1].c2).cout
         self.mlps = []
@@ -321,23 +355,6 @@ class Engine(object):
                 raise ValueError("byol_b200: layer %s (%s %d -> %d): channel / feature counts on the tensor-core path "
                                  "must be multiples of 8 (only the image channels and the number of classes are free)"
                                  % (u.name, u.kind, u.cin, u.cout))
-        self.module_key = self._module_key()
-        self.bn_modules = [u.bn for u in self.units if u.bn is not None]
-        self.bn_channels = sum(u.cout for u in self.units if u.bn is not None)
-        self.sync = any(isinstance(b, nn.SyncBatchNorm) for b in self.bn_modules)
-        self._side_stream = torch.cuda.Stream(device=self.device) if self.overlap_wgrad else None
-        # the same two streams serve the forward lane pairs and the backward views: every extra stream is an extra
-        # caching-allocator pool, and pools do not share their cached blocks
-        self._fwd_streams = [torch.cuda.Stream(device=self.device) for _ in range(2)]
-        self._bwd_streams = self._fwd_streams
-        self.w_online = _Weights(self.units, self.device, True)
-        self.w_target = _Weights(self.units, self.device, False)
-        self.graphs = {}           # captured steps point into the old buffers
-        self.s_online = self.s_target = None
-        if self.T:
-            self.s_online = _SplitWeights(self.units, self.device, self.T, want_dgrad=self.bwd32)
-            self.s_target = _SplitWeights(self.units, self.device, self.T)
-        self.ready = True
 
     def _module_key(self):
         """Identity of every sub-module: module surgery after the first forward (e.g. convert_sync_batchnorm, which
@@ -364,11 +381,110 @@ class Engine(object):
                                   out=wset.w_stem4)
 
     # ------------------------------------------------------------------------------------------
+    # activation recomputation: a memory model of one bf16 training step from the layer shapes, and the blocks whose
+    # online lanes keep only their input, BN coefficients and output mask (the backward pass rebuilds the rest)
+    # ------------------------------------------------------------------------------------------
+    # The measured bf16 steps reserved 1.23-1.29x their peak allocated bytes (profiles/): under CUDA graphs a stream
+    # does not reuse what another stream freed.  MARGIN covers what the model leaves out: LARS momentum, loss,
+    # classifier, a training loop's prefetched input batches.
+    RESERVE_FACTOR = 1.3
+    MARGIN = 3 << 30
+
+    def memory_model(self, n, h, w):
+        """Bytes of one bf16 training step with n images per view at h x w.  Per block: "stored" / "kept" = what one
+        online lane saves for it without / with recompute (the block output and its mask are kept either way),
+        "dy" = the backward gradients one view holds until the weight-gradient join, "work" = one view's other backward
+        transients of the block (a recomputed block adds stored - kept), "flops" = its recompute.  "first_input" is the first block's input
+        (saved by each online lane), "fixed" the step's other activations (stem, MLPs, input layouts)."""
+        cs = ops.conv_out_size
+
+        def conv(u, hi, wi):
+            ho, wo = cs(hi, u.k, u.stride, u.pad), cs(wi, u.k, u.stride, u.pad)
+            e = n * ho * wo * u.cout
+            return ho, wo, e, 2 * e * (u.cin // u.groups) * u.k * u.k
+
+        st = self.stem
+        h0, w0, e0, _ = conv(st, h, w)
+        H, W = cs(h0, self.pool_k, self.pool_s, self.pool_p), cs(w0, self.pool_k, self.pool_s, self.pool_p)
+        first = 2 * n * H * W * st.cout
+        blocks = []
+        for b in self.blocks:
+            h1, w1, e1, f1 = conv(b.c1, H, W)
+            h2, w2, e2, f2 = conv(b.c2, h1, w1)
+            e3 = f3 = ea2 = 0
+            hl, wl, eo = h2, w2, e2
+            if b.kind == "bottleneck":
+                ea2 = e2
+                hl, wl, eo, f3 = conv(b.c3, h2, w2)
+                e3 = eo
+            ed = fd = exs = 0
+            if b.down is not None:
+                _, _, ed, fd = conv(b.down, H, W)
+                if self._down_as_gemm(b.down, H, W):
+                    exs = n * (H // 2) * (W // 2) * b.down.cin
+            kept = 2 * eo + eo // 8
+            stored = kept + 2 * (e1 + e1 + e2 + ea2 + e3 + ed + exs)       # y1 a1 y2 a2 y3 yd xsub
+            dy = 2 * (e1 + e2 + e3 + ed)
+            blocks.append({"stored": stored, "kept": kept, "dy": dy, "flops": f1 + f2 + f3 + fd,
+                           "work": dy + 2 * (eo + n * H * W * b.c1.cin)})
+            H, W = hl, wl
+        mlp = sum(2 * n * (l1.cin + 2 * l1.cout) for l1, _ in self.mlps)   # x, h, a
+        fixed = 2 * (2 * e0 + first // 2 + mlp) + 2 * (2 * n * h * w * 8)   # 2 lanes: y0, pool index, MLPs; 2 images
+        return {"blocks": blocks, "first_input": first, "fixed": fixed}
+
+    @staticmethod
+    def lane_bytes(mm, plan):
+        """Activation bytes one online lane saves in its block dicts under `plan`."""
+        return mm["first_input"] + sum(blk["kept" if i in plan else "stored"] for i, blk in enumerate(mm["blocks"]))
+
+    def step_need(self, mm, plan):
+        """Device bytes one training step needs under `plan`: the peak of the forward (two online lanes' saved set,
+        the target pair's largest block) and of the backward (the saved set, the gradients of the stored blocks held
+        for the side-stream weight gradients, one block's transients), scaled by RESERVE_FACTOR, plus MARGIN."""
+        blocks = mm["blocks"]
+        saved = 2 * self.lane_bytes(mm, plan)
+        fwd = saved + 2 * max(blk["stored"] for blk in blocks)
+        bwd = saved + sum(blk["dy"] for i, blk in enumerate(blocks) if i not in plan) + \
+            max(blk["work"] + (blk["stored"] - blk["kept"] if i in plan else 0) for i, blk in enumerate(blocks))
+        return int(self.RESERVE_FACTOR * (max(fwd, bwd) + mm["fixed"])) + self.MARGIN
+
+    def plan_blocks(self, mm, budget):
+        """The fewest blocks to recompute so that the step needs at most `budget` bytes, taken in order of saved
+        bytes per recomputed FLOP (ties: the earlier block); all blocks if even that does not fit; empty if the
+        stored step fits."""
+        blocks = mm["blocks"]
+        order = sorted(range(len(blocks)),
+                       key=lambda i: (-(blocks[i]["stored"] - blocks[i]["kept"]) / blocks[i]["flops"], i))
+        plan = []
+        for i in order:
+            if self.step_need(mm, plan) <= budget:
+                break
+            plan.append(i)
+        return frozenset(plan)
+
+    def recompute_plan(self, n, h, w):
+        """Blocks whose online lanes recompute their activations in the backward pass, for n images per view at h x w:
+        empty when the stored step fits in what the device can give (its free memory plus the allocator's unused
+        cache, read once per geometry: the GPU may be shared).  Only the bf16 path without BYOL_B200_FUSE3
+        recomputes."""
+        if self.T or self.fuse3:
+            return frozenset()
+        key = (n, h, w, self.world(), self._mem_budget)
+        plan = self._plans.get(key)
+        if plan is None:
+            budget = self._mem_budget
+            if budget is None:
+                free, _ = torch.cuda.mem_get_info(self.device)
+                budget = free + torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device)
+            plan = self._plans[key] = self.plan_blocks(self.memory_model(n, h, w), budget)
+        return plan
+
+    # ------------------------------------------------------------------------------------------
     # forward building blocks (lists are per lane)
     # ------------------------------------------------------------------------------------------
     @staticmethod
-    def _down_as_gemm(u, x):
-        return u.k == 1 and u.stride == 2 and u.pad == 0 and x.shape[1] % 2 == 0 and x.shape[2] % 2 == 0
+    def _down_as_gemm(u, h, w):
+        return u.k == 1 and u.stride == 2 and u.pad == 0 and h % 2 == 0 and w % 2 == 0
 
     def _conv_bn(self, u, xs, lanes, train, stem4=None, unit_stride=None, stats_only=False):
         """raw conv/linear outputs + BN coefficients [scale, shift, mean, invstd] per lane.
@@ -391,7 +507,7 @@ class Engine(object):
             elif u.kind == "linear":
                 y = ops.linear_fprop(x, wset.wf[u.idx], bias=bias, stats=st)
             else:
-                y = ops.conv_fprop(x, wset.wf[u.idx], u.k, u.k, unit_stride or u.stride, u.pad, stats=st)
+                y = self._conv(u, x, wset, unit_stride, stats=st)
             ys.append(y)
         coeffs = self._cpool.take(L * 4 * C).view(L, 4, C)
         bn = u.bn
@@ -418,6 +534,12 @@ class Engine(object):
         return ys, coeffs
 
     @staticmethod
+    def _conv(u, x, wset, unit_stride=None, stats=None):
+        """Raw conv output of a block conv.  The fused statistics do not change the stored y (the epilogue sums the
+        bf16 values it stores), so _rebuild calls this without them and gets the forward's bits."""
+        return ops.conv_fprop(x, wset.wf[u.idx], u.k, u.k, unit_stride or u.stride, u.pad, stats=stats)
+
+    @staticmethod
     def _apply(y, c, relu, resid=None, rc=None, mask=None):
         C = y.shape[-1]
         out = torch.empty_like(y)
@@ -437,7 +559,7 @@ class Engine(object):
             return False
         if b.down is not None:
             d = b.down
-            if d.k != 1 or d.pad != 0 or not (d.stride == 1 or self._down_as_gemm(d, x)):
+            if d.k != 1 or d.pad != 0 or not (d.stride == 1 or self._down_as_gemm(d, x.shape[1], x.shape[2])):
                 return False
         return True
 
@@ -496,15 +618,21 @@ class Engine(object):
         xsub = None
         if b.down is not None:
             # 1x1 / stride-2 downsample: compact the pixels it reads, then it is a plain TMA-fed GEMM (fprop + wgrad)
-            if self._down_as_gemm(b.down, xs[0]):
+            if self._down_as_gemm(b.down, xs[0].shape[1], xs[0].shape[2]):
                 xsub = [ops.subsample2(x) for x in xs]
             yd, cd = self._conv_bn(b.down, xsub if xsub is not None else xs, lanes, train, unit_stride=1 if xsub else None)
             outs = [self._apply(ylast[i], clast[i], True, resid=yd[i], rc=cd[i], mask=masks[i]) for i in range(L)]
         else:
             yd, cd = None, None
             outs = [self._apply(ylast[i], clast[i], True, resid=xs[i], mask=masks[i]) for i in range(L)]
+        recompute = b.idx in self._recompute_now
         for i, (_, _, saved) in enumerate(lanes):
-            if saved is not None:
+            if saved is not None and recompute:
+                # y1 .. yd are freed on return; _block_bwd rebuilds them from x and these coefficients (_rebuild)
+                saved["blocks"].append({
+                    "recompute": True, "mask": masks[i], "x": xs[i], "c1": c1[i], "c2": c2[i],
+                    "c3": c3[i] if c3 is not None else None, "cd": cd[i] if cd is not None else None, "out": outs[i]})
+            elif saved is not None:
                 saved["blocks"].append({
                     "mask": masks[i], "xsub": xsub[i] if xsub is not None else None,
                     "x": xs[i], "y1": y1[i], "c1": c1[i], "a1": a1[i], "y2": y2[i], "c2": c2[i],
@@ -606,6 +734,9 @@ class Engine(object):
             return res, reps_b
         if rep_bf16_out is None:
             rep_bf16_out = [None] * L
+        if train and any(lane[2] is not None for lane in lanes):
+            img = x8[0][0] if x8[0][0] is not None else x8[0][1]
+            self._recompute_now = self.recompute_plan(img.shape[0], x8[0][2], x8[0][3])
         # under SyncBatchNorm over NCCL the per-layer all-reduces serialise the lane pairs anyway: run all four lanes
         # lock-step on one stream there, which halves the number of (latency-bound) NCCL calls.  The peer-memory
         # exchange (comm.PeerExchange) has one channel per stream, so the two-stream schedule stays.
@@ -634,6 +765,7 @@ class Engine(object):
                 main.wait_event(e2)
         self._fin_events = None
         self._group_order = 0
+        self._recompute_now = frozenset()
         if train:
             torch._foreach_add_([b.num_batches_tracked for b in self.bn_modules], L)
         return results, reps_b_all
@@ -978,9 +1110,35 @@ class Engine(object):
         self._wgrad(b.c1, xs, dy1)
         return self._dgrad(b.c1, dy1, xshapes, resids=resid, resid_masks=resid_masks, resid_up=resid_up)
 
+    def _rebuild(self, b, s):
+        """The saved dict of a block the forward recomputes: y1, a1, y2, a2, y3, xsub, yd again from its input and the
+        forward's scale / shift, by the forward's kernels with the forward's arguments, on the current stream.  No
+        statistics, running-statistic update or SyncBatchNorm exchange: the bits equal the forward's."""
+        w, x = self.w_online, s["x"]
+        r = {k: v for k, v in s.items() if k != "recompute"}
+        r["y1"] = self._conv(b.c1, x, w)
+        r["a1"] = self._apply(r["y1"], s["c1"], True)
+        r["y2"] = self._conv(b.c2, r["a1"], w)
+        r["a2"] = r["y3"] = r["xsub"] = r["yd"] = None
+        if b.kind == "bottleneck":
+            r["a2"] = self._apply(r["y2"], s["c2"], True)
+            r["y3"] = self._conv(b.c3, r["a2"], w)
+        if b.down is not None:
+            if self._down_as_gemm(b.down, x.shape[1], x.shape[2]):
+                r["xsub"] = ops.subsample2(x)
+                r["yd"] = self._conv(b.down, r["xsub"], w, unit_stride=1)
+            else:
+                r["yd"] = self._conv(b.down, x, w)
+        return r
+
     def _block_bwd(self, b, S, gs):
         if S[0].get("fused3"):
             return self._block_bwd_fused3(b, S, gs)
+        if S[0].get("recompute"):
+            out = self._block_bwd(b, [self._rebuild(b, s) for s in S], gs)
+            # the weight gradients read the rebuilt tensors on the side stream: join, so that they are freed here
+            self._join_side_stream()
+            return out
         L = len(gs)
         outs = [s["out"] for s in S]
         xs = [s["x"] for s in S]
@@ -1258,7 +1416,8 @@ class Engine(object):
     # ------------------------------------------------------------------------------------------
     def graph_key(self, a1):
         return (tuple(a1.shape), self.world(), bool(self.sync), self.theta.data_ptr(), self.multi_stream,
-                self.overlap_wgrad, self.T, self.bwd32, self.fuse3, self.fuse3_max_planes, self.fused_mlp)
+                self.overlap_wgrad, self.T, self.bwd32, self.fuse3, self.fuse3_max_planes, self.fused_mlp,
+                self.recompute_plan(a1.shape[0], a1.shape[2], a1.shape[3]))
 
     def prep_step(self, mean, training):
         """All weight layouts one forward (+ backward) needs, from the fp32 masters."""
