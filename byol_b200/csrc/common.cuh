@@ -73,16 +73,40 @@ __device__ __forceinline__ void fix_add_words(Fix128* acc, unsigned long long lo
   atomicAdd(&acc->lo, lo);   // results unused: both compile to reductions
   atomicAdd(reinterpret_cast<unsigned long long*>(&acc->hi), (unsigned long long)hi);
 }
-__device__ __forceinline__ void fix_add(Fix128* acc, double v) {
+// Sends the part of v the fixed-point words can not take to acc's fp64 side sum; false when nothing is left for them.
+__device__ __forceinline__ bool fix_take_spill(Fix128* acc, double& v) {
   if (!(fabs(v) < kFixSplit)) {   // NaN, Inf, or a part too large for the fixed-point words
     const double big = isfinite(v) ? trunc(v * 0x1p-20) * 0x1p20 : v;
     atomicAdd(&acc->spill, big);
-    if (!isfinite(v)) return;
+    if (!isfinite(v)) return false;
     v -= big;                      // exact: the bits of v below 2^20, |v| < 2^20
   }
+  return true;
+}
+// the two fixed-point words of v, |v| < kFixSplit
+__device__ __forceinline__ void fix_words(double v, unsigned long long& lo, long long& hi) {
   const double x = v * 0x1p50;                 // exact (power-of-two scaling)
-  const double hi = floor(x * 0x1p-32);
-  fix_add_words(acc, __double2ull_rn(x - hi * 0x1p32), (long long)hi);   // lo in [0, 2^32]
+  const double h = floor(x * 0x1p-32);
+  lo = __double2ull_rn(x - h * 0x1p32);        // in [0, 2^32]
+  hi = (long long)h;
+}
+__device__ __forceinline__ void fix_add(Fix128* acc, double v) {
+  if (!fix_take_spill(acc, v)) return;
+  unsigned long long lo;
+  long long hi;
+  fix_words(v, lo, hi);
+  fix_add_words(acc, lo, hi);
+}
+// Same, but the fixed-point words go to a block-local pair words[0] (lo), words[1] (hi) in shared memory, which the
+// block adds to acc's words once (fix_add_words).  Integer sums wrap mod 2^64 in either order, so acc ends with the
+// same words as if every addend had gone to it directly.
+__device__ __forceinline__ void fix_add_local(Fix128* acc, unsigned long long* words, double v) {
+  if (!fix_take_spill(acc, v)) return;
+  unsigned long long lo;
+  long long hi;
+  fix_words(v, lo, hi);
+  atomicAdd(&words[0], lo);
+  atomicAdd(&words[1], (unsigned long long)hi);
 }
 __device__ __forceinline__ void fix_add_raw(Fix128* acc, const Fix128& v) {
   fix_add_words(acc, v.lo, v.hi);
@@ -329,6 +353,36 @@ __device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t chunk) {
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
+}
+
+// four 8x8 bf16 matrices -> shared memory; lane l gives the address of row l & 7 of matrix l >> 3, and holds row
+// l / 4, columns 2 * (l % 4) and +1 of every matrix (the accumulator fragment layout of one warp's 8-row group)
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
+
+// Accumulator fragment of this warpgroup (64 tile rows) -> bf16 (pack_bf16x2 rounding) in the epilogue's output
+// staging layout: per 32-row quarter and 32-column chunk one [32 rows][32 cols] block of 2048 bytes with the 64-byte
+// TMA swizzle (16-byte chunk j of row r at j ^ ((r >> 1) & 3)), blocks ordered [quarter][chunk] from `base` (the
+// warpgroup's first quarter, 512-byte aligned).  Warp w holds rows 16w .. 16w+15; stmatrix p writes its rows 0-7 and
+// 8-15 of the 8-column groups 2p and 2p+1.  The 8 rows of one matrix land in 8 different 16-byte bank groups.
+template <int N>
+__device__ __forceinline__ void acc_store_bf16_sw64(uint32_t base, const float (&d)[N / 2]) {
+  const int t = threadIdx.x & 127;
+  const int warp = t >> 5, lane = t & 31;
+  const uint32_t r = (uint32_t)(16 * (warp & 1) + 8 * ((lane >> 3) & 1) + (lane & 7));   // row inside the quarter
+  const uint32_t rbase = base + (uint32_t)(warp >> 1) * (N / 32) * 2048u + r * 64u;
+  const uint32_t sw = (r >> 1) & 3u;
+  const uint32_t gh = (uint32_t)lane >> 4;   // this lane addresses column group 2p + gh
+#pragma unroll
+  for (int p = 0; p < N / 16; ++p) {
+    const uint32_t g = 2u * (uint32_t)p + gh;
+    stmatrix_x4(rbase + (g >> 2) * 2048u + (((g & 3u) ^ sw) << 4), pack_bf16x2(d[8 * p], d[8 * p + 1]),
+                pack_bf16x2(d[8 * p + 2], d[8 * p + 3]), pack_bf16x2(d[8 * p + 4], d[8 * p + 5]),
+                pack_bf16x2(d[8 * p + 6], d[8 * p + 7]));
+  }
 }
 
 // ----------------------------------------------------------------------------

@@ -11,7 +11,8 @@
 //
 // One CTA computes a 128 x BN tile.  smem operand tiles use the 128-byte swizzle; two MMA warpgroups (wgmma) own
 // 64 tile rows each and keep their accumulators in registers; a finished tile is handed to the epilogue warps
-// (one tile row per lane) through an fp32 tile in shared memory.
+// (one tile row per lane) through an fp32 tile in shared memory, or, when the epilogue only stores bf16 values and
+// their statistics, as bf16 store blocks (SmemLayout, H16).
 #include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -48,6 +49,7 @@ struct ConvGemmParams {
   int out_fp32;
   int relu;
   int small_src;   // 1: the gathered tensor has < 2^31 elements (32-bit element offsets are safe)
+  int local_stats; // H16 with statistics: the CTA sums its fixed-point words in shared memory (SmemLayout)
   // stride-2 dgrad by output parity ("parity mode"): the M dimension enumerates the pixels of dX class by class
   // (class = (ih & 1, iw & 1)); a tile belongs to ONE class, for which only the taps with the parity of
   // (coordinate + pad) contribute, so every role skips the other taps entirely.
@@ -95,7 +97,16 @@ __device__ __forceinline__ TileInfo tile_info(const ConvGemmParams& p, int tile,
 // epilogue warps: warps w and w + 4 share the row quarter w & 3 of the tile and split its columns.
 // Output staging: [32 rows][32 cols] chunks with the 64-byte swizzle, NBUF staging buffers per warp.  (A variant with
 // 128-byte staging rows and a 2-stage operand ring was measured slower for every K >= 128 and removed.)
-template <int BN, int STAGES, bool A_TMA>
+// H16 (bf16 hand-off): when the epilogue only stores the bf16 value and sums its statistics (no bias, residual, ReLU
+// or fp32 output), the MMA warpgroups round the accumulators to bf16 themselves and write them straight into the
+// staging blocks, and the epilogue warps only issue the TMA stores and read the statistics.  Two such tiles
+// ([quarter][chunk] blocks, 32 KB at BN = 128) replace the fp32 tile and the per-warp staging, so the MMA warpgroups
+// can hand off tile i+1 while tile i is being stored.
+// With statistics, a CTA whose tiles alternate between column tiles (Ndim of 1024 / 2048: 8 / 16 column tiles, 132
+// CTAs) flushes its partial sums after every tile; with global fixed-point atomics those flushes cost more than the
+// GEMM.  So the H16 kernel adds its flushes to fixed-point words of its own (local_stats: [2 * Ndim][lo, hi], 32 * Ndim
+// bytes of dynamic shared memory from NEEDED on) and adds them to the global accumulators once, when it ends.
+template <int BN, int STAGES, bool A_TMA, bool H16 = false>
 struct SmemLayout {
   static constexpr int EW = A_TMA ? 8 : 4;                // epilogue warps
   static constexpr int CPW = (BN / 32) / (EW / 4);        // 32-column chunks per epilogue warp
@@ -110,7 +121,9 @@ struct SmemLayout {
   // finished accumulator tile [BM][ACC_LD] fp32 (MMA warpgroups -> epilogue warps)
   static constexpr int ACC_LD = acc_ld(BN);
   static constexpr int ACC_OFF = STAGE_OUT_OFF + EW * STAGE_PER_WARP;
-  static constexpr int BAR_OFF = ACC_OFF + BM * ACC_LD * 4;
+  // H16: two bf16 output tiles from STAGE_OUT_OFF instead of the staging buffers and the fp32 tile
+  static constexpr int OUT_TILE_BYTES = BM * BN * 2;
+  static constexpr int BAR_OFF = H16 ? STAGE_OUT_OFF + 2 * OUT_TILE_BYTES : ACC_OFF + BM * ACC_LD * 4;
   static constexpr int NEEDED = BAR_OFF + 256;
   static constexpr int TOTAL = NEEDED + 768;   // slack for the run-time 1024-byte alignment of the base
   static_assert(TOTAL <= 232448, "one CTA per SM: <= 227 KB of dynamic shared memory");
@@ -128,12 +141,16 @@ struct SmemLayout {
 // ---------------------------------------------------------------------------------------------
 static constexpr int IG_THREADS = 17 * 32;
 
-template <int BN, int STAGES, bool A_TMA, bool GROUPED = false>
+// named barrier 1 over the epilogue warps (threads 0 .. n-1) only; barrier 0 is __syncthreads
+__device__ __forceinline__ void epilogue_bar_sync(int n) { asm volatile("bar.sync 1, %0;" ::"r"(n) : "memory"); }
+
+template <int BN, int STAGES, bool A_TMA, bool GROUPED = false, bool H16 = false>
 __global__ void __launch_bounds__(IG_THREADS, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_constant__ CUtensorMap tmapB,
                   const __grid_constant__ CUtensorMap tmapC, const ConvGemmParams p, const int num_tiles) {
   static_assert(!GROUPED || (BN == 64 && !A_TMA), "grouped mode: 64-column tiles, gathered A operand");
-  using L = SmemLayout<BN, STAGES, A_TMA>;
+  static_assert(!H16 || A_TMA, "bf16 hand-off: plain GEMM only (no parity mode)");
+  using L = SmemLayout<BN, STAGES, A_TMA, H16>;
   constexpr int EW = L::EW;
   constexpr int CPW = L::CPW;
   constexpr int MMA_WARP = 8;
@@ -147,6 +164,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* tfull_bar = empty_bar + STAGES;   // accumulator tile ready for the epilogue
   uint64_t* tempty_bar = tfull_bar + 1;       // accumulator tile drained
+  uint64_t* ofull_bar = tempty_bar + 1;       // H16: bf16 tile b staged (b = 0, 1)
+  uint64_t* oempty_bar = ofull_bar + 2;       // H16: bf16 tile b stored and read
   uint8_t* stage_out = smem + L::STAGE_OUT_OFF;   // 1024-byte aligned
   float* accbuf = reinterpret_cast<float*>(smem + L::ACC_OFF);
 
@@ -161,6 +180,10 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     }
     mbar_init(tfull_bar, 256u);       // every MMA thread, after storing its fragment
     mbar_init(tempty_bar, (uint32_t)EW);   // one arrival per epilogue warp
+    for (int b = 0; b < 2; ++b) {
+      mbar_init(&ofull_bar[b], 256u);
+      mbar_init(&oempty_bar[b], (uint32_t)EW);
+    }
     fence_mbar_init();
     tma_prefetch_desc(&tmapB);
     if (A_TMA) tma_prefetch_desc(&tmapA);
@@ -185,6 +208,12 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     for (int i = 0; i < NACC; ++i) { cs1[i] = 0ull; cs2[i] = 0ull; }
     int local = 0;
     int stat_n0 = -1;   // column offset the register accumulators currently belong to
+    const bool local_stats = H16 && do_stats && p.local_stats;
+    unsigned long long* lstats = reinterpret_cast<unsigned long long*>(smem + L::NEEDED);
+    if (local_stats) {
+      for (int i = threadIdx.x; i < 4 * p.Ndim; i += EW * 32) lstats[i] = 0ull;
+      epilogue_bar_sync(EW * 32);
+    }
     auto flush_stats = [&]() {
 #pragma unroll
       for (int i = 0; i < NACC; ++i) {
@@ -196,7 +225,12 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
         b.y += __shfl_xor_sync(0xffffffffu, b.y, 16);
         const int col = stat_n0 + col_w0 + i * 32 + 2 * (lane & 15);
         const bool owner = lane < 16;
-        if (owner && col < p.Ndim) {   // Ndim is a multiple of 8: col + 1 is valid too
+        if (owner && col < p.Ndim && local_stats) {   // Ndim is a multiple of 8: col + 1 is valid too
+          fix_add_local(p.fx + col, lstats + 2 * col, a.x);
+          fix_add_local(p.fx + col + 1, lstats + 2 * (col + 1), a.y);
+          fix_add_local(p.fx + p.Ndim + col, lstats + 2 * (p.Ndim + col), b.x);
+          fix_add_local(p.fx + p.Ndim + col + 1, lstats + 2 * (p.Ndim + col + 1), b.y);
+        } else if (owner && col < p.Ndim) {
           fix_add(p.fx + col, a.x);
           fix_add(p.fx + col + 1, a.y);
           fix_add(p.fx + p.Ndim + col, b.x);
@@ -212,6 +246,33 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       if (do_stats && stat_n0 != n0) {
         if (stat_n0 >= 0) flush_stats();
         stat_n0 = n0;
+      }
+      if constexpr (H16) {
+        // the MMA warpgroups staged this warp's blocks (and fenced them for the TMA engine): store, then sum
+        // the statistics from the same bytes while the TMA engine reads them
+        const int buf = local & 1;
+        mbar_wait(&ofull_bar[buf], (uint32_t)((local >> 1) & 1));
+        const int mrow0 = m0 + quarter * 32;
+        int rows_valid = p.M - mrow0;
+        rows_valid = rows_valid < 0 ? 0 : (rows_valid > 32 ? 32 : rows_valid);
+        const uint32_t qbase = smem_u32(stage_out + buf * L::OUT_TILE_BYTES) + (uint32_t)quarter * (BN / 32) * 2048u;
+#pragma unroll
+        for (int cl = 0; cl < CPW; ++cl) {
+          const int c0 = col_w0 + cl * 32;
+          const int nbase = n0 + c0;
+          if (nbase >= p.Ndim) continue;  // warp-uniform
+          const uint32_t blk = qbase + (uint32_t)(c0 / 32) * 2048u;
+          if (lane == 0) {
+            tma_store_2d(&tmapC, blk, nbase, mrow0);   // rows >= M and columns >= Ndim are clipped by TMA
+            tma_store_commit();
+          }
+          if (do_stats) stats_narrow(blk, lane, rows_valid, cs1[cl], cs2[cl]);
+        }
+        // the TMA engine has read the blocks and every lane is past its statistics: hand the buffer back
+        if (lane == 0) tma_store_wait_read();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&oempty_bar[buf]);
+        continue;
       }
       mbar_wait(tfull_bar, (uint32_t)(local & 1));
       const int mrow0 = m0 + quarter * 32;
@@ -350,6 +411,13 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       }
     }
     if (do_stats && stat_n0 >= 0) flush_stats();
+    if (local_stats) {   // every epilogue warp has flushed: the CTA's words -> the global accumulators, once
+      epilogue_bar_sync(EW * 32);
+      for (int i = threadIdx.x; i < 2 * p.Ndim; i += EW * 32) {
+        const unsigned long long lo = lstats[2 * i], hi = lstats[2 * i + 1];
+        if ((lo | hi) != 0ull) fix_add_words(p.fx + i, lo, (long long)hi);
+      }
+    }
     if (lane == 0) tma_store_wait_all();   // global writes complete before the kernel exits
   } else if (!A_TMA && warp >= EW && warp < EW + 4) {
     // ======================= A gather producers ==========================================
@@ -596,9 +664,18 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
       wg_wait<0>();
       wg_fence_acc(d);
       if (leader && prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
-      mbar_wait(tempty_bar, (uint32_t)((local & 1) ^ 1));
-      acc_store_smem<BN>(accbuf, L::ACC_LD, wg * 64, 0, d);
-      mbar_arrive(tfull_bar);
+      if constexpr (H16) {
+        const int buf = local & 1;
+        mbar_wait(&oempty_bar[buf], (uint32_t)(((local >> 1) & 1) ^ 1));
+        // this warpgroup's two row quarters: blocks 2 * wg * (BN / 32) ..
+        acc_store_bf16_sw64<BN>(smem_u32(stage_out + buf * L::OUT_TILE_BYTES) + (uint32_t)wg * 2 * (BN / 32) * 2048u, d);
+        fence_proxy_async_smem();   // the epilogue's TMA stores (async proxy) read these writes
+        mbar_arrive(&ofull_bar[buf]);
+      } else {
+        mbar_wait(tempty_bar, (uint32_t)((local & 1) ^ 1));
+        acc_store_smem<BN>(accbuf, L::ACC_LD, wg * 64, 0, d);
+        mbar_arrive(tfull_bar);
+      }
     }
   } else if (warp == TMA_WARP) {
     // ======================= TMA producer =================================================
@@ -905,16 +982,21 @@ bool patch_wgrad_applicable(int H, int W, int C, int Cin_real, int Cout, int KH,
 int patch_wgrad_launch(const void* x, const void* dy, float* dw, int Nimg, int H, int W, int C, int Cout, int sms,
                        cudaStream_t stream, int gs = 0);
 
-template <int BN, int STAGES, bool A_TMA, bool GROUPED = false>
+template <int BN, int STAGES, bool A_TMA, bool GROUPED = false, bool H16 = false>
 static int launch_igemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
                         const ConvGemmParams& p, int tiles_m, cudaStream_t stream) {
-  using L = SmemLayout<BN, STAGES, A_TMA>;
-  auto kern = conv_igemm_kernel<BN, STAGES, A_TMA, GROUPED>;
-  if (smem_opt_in((const void*)kern, L::TOTAL, "conv_igemm_kernel") != 0) return -2;
+  using L = SmemLayout<BN, STAGES, A_TMA, H16>;
+  auto kern = conv_igemm_kernel<BN, STAGES, A_TMA, GROUPED, H16>;
+  // block-local statistic words when they fit next to the tiles (Ndim <= 2112 at BN = 128); else global atomics
+  ConvGemmParams q = p;
+  const int64_t local_bytes = 32 * (int64_t)p.Ndim;
+  q.local_stats = (H16 && p.col_sum != nullptr && L::TOTAL + local_bytes <= 232448) ? 1 : 0;
+  const int smem = L::TOTAL + (q.local_stats ? (int)local_bytes : 0);
+  if (smem_opt_in((const void*)kern, smem, "conv_igemm_kernel") != 0) return -2;
   const int num_tiles = tiles_m * p.tiles_n;
   int grid = device_sm_count();        // persistent: one CTA per SM (shared memory sized for it)
   if (grid > num_tiles) grid = num_tiles;
-  kern<<<grid, IG_THREADS, L::TOTAL, stream>>>(ta, tb, tc, p, num_tiles);
+  kern<<<grid, IG_THREADS, smem, stream>>>(ta, tb, tc, q, num_tiles);
   return check_launch("conv_igemm_kernel");
 }
 
@@ -1014,6 +1096,9 @@ static int conv_igemm_impl(const void* src, const void* wt, void* dst, const voi
     tiles_m = p.ncls * (p.Mc / BM);
   }
   const bool a_tma = !force_gather && KH == 1 && KW == 1 && stride == 1 && pad == 0;   // never true in parity mode
+  // bf16 hand-off (SmemLayout): the epilogue only stores the rounded accumulator and sums its statistics
+  const bool h16 = a_tma && !out_fp32 && bias == nullptr && resid == nullptr && resid_mask == nullptr &&
+                   resid_f32 == nullptr && !relu;
 
   CUtensorMap ta, tb, tc;
   memset(&ta, 0, sizeof(ta));
@@ -1036,11 +1121,13 @@ static int conv_igemm_impl(const void* src, const void* wt, void* dst, const voi
   if (grouped) {
     rc = launch_igemm<64, 4, false, true>(ta, tb, tc, p, tiles_m, stream);
   } else if (BN == 128) {
-    rc = a_tma ? launch_igemm<128, 3, true>(ta, tb, tc, p, tiles_m, stream)
-               : launch_igemm<128, 3, false>(ta, tb, tc, p, tiles_m, stream);
+    rc = h16     ? launch_igemm<128, 3, true, false, true>(ta, tb, tc, p, tiles_m, stream)
+         : a_tma ? launch_igemm<128, 3, true>(ta, tb, tc, p, tiles_m, stream)
+                 : launch_igemm<128, 3, false>(ta, tb, tc, p, tiles_m, stream);
   } else {
-    rc = a_tma ? launch_igemm<64, 3, true>(ta, tb, tc, p, tiles_m, stream)
-               : launch_igemm<64, 4, false>(ta, tb, tc, p, tiles_m, stream);
+    rc = h16     ? launch_igemm<64, 3, true, false, true>(ta, tb, tc, p, tiles_m, stream)
+         : a_tma ? launch_igemm<64, 3, true>(ta, tb, tc, p, tiles_m, stream)
+                 : launch_igemm<64, 4, false>(ta, tb, tc, p, tiles_m, stream);
   }
   if (rc != 0 || col_sum == nullptr) return rc;
   return fix_flush_stats(p.fx, col_sum, col_sqsum, Ndim, stream);
