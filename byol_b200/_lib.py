@@ -113,6 +113,9 @@ _SIGNATURES = {
     "byol_augment_params": [c_void_p, c_int, c_int, c_int, ctypes.c_uint64, ctypes.c_uint64, c_float, c_float, c_float,
                             c_float, c_float, c_void_p],
     "byol_augment_apply": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    "byol_augment_params_ragged": [c_void_p, c_void_p, c_int, c_int, c_int, ctypes.c_uint64, ctypes.c_uint64, c_float,
+                                   c_float, c_float, c_float, c_float, c_void_p],
+    "byol_augment_apply_ragged": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
     "byol_xchg_layout": [c_void_p, c_void_p, c_void_p],
     "byol_xchg_sum": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p],
     "byol_abi_version": [],

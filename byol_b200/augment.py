@@ -5,10 +5,11 @@ in HBM: ``RandomResizedCrop(R)``, ``RandomHorizontalFlip(0.5)``, ``RandomApply([
 
     aug = TwoViewAugment(image_size=224, seed=0)
     aug1, aug2 = aug(images)            # images: fp32 CUDA [N, 3, H, W] in [0, 1] -> two fp32 [N, 3, 224, 224]
+    aug1, aug2 = aug([u8_0, u8_1])      # or a list of CUDA uint8 [3, H_i, W_i] images of any sizes (read as v / 255)
 
 Every call draws fresh parameters from a counter-based RNG (seed, call counter, sample, view), so a run is
-reproducible and the two views of a sample are independent.  ``apply(images, params)`` runs the pipeline on explicit
-parameter records (tests/test_gpu_augment.py checks every stage against torchvision on identical parameters).
+reproducible and the two views of a sample are independent.  ``apply(images, params)`` and
+``apply_ragged(images, params)`` run the pipeline on explicit parameter records (tests/test_gpu_augment.py checks every stage against torchvision on identical parameters).
 """
 import torch
 
@@ -51,6 +52,77 @@ class TwoViewAugment(object):
                                      ops._stream()), "byol_augment_apply", kernels=4 if self.ksize else 2)
         return out[0], out[1]
 
+    def sample_params_ragged(self, sizes, device, n0=0, total=None, step=None):
+        """Records for images of their own sizes ``sizes`` (a list of ``(H, W)``): samples ``[n0, n0 + len(sizes))`` of
+        a ``total``-image batch (default: just these).  ``step`` keys the draw (default: the call counter, which then
+        advances), so the chunks of one batch, sampled with one ``step``, get the records of a single call; equal
+        sizes with ``n0 = 0`` reproduce ``sample_params``."""
+        hw = _sizes_table(sizes, device)
+        n = hw.shape[0]
+        total = n if total is None else int(total)
+        if n0 < 0 or n0 + n > total:
+            raise ValueError("TwoViewAugment: samples [%d, %d) are not part of a %d-image batch" % (n0, n0 + n, total))
+        if step is None:
+            step = self.calls
+            self.calls += 1
+        params = torch.empty((2, n, RECORD), dtype=torch.float32, device=device)
+        check(lib.byol_augment_params_ragged(params.data_ptr(), hw.data_ptr(), n, int(n0), total, self.seed, int(step),
+                                             self.strength, self.p[0], self.p[1], self.p[2], self.p[3], ops._stream()),
+              "byol_augment_params_ragged")
+        return params
+
+    def resize_params(self, sizes, device):
+        """Records that take the whole image, with no flip, jitter, grayscale or blur: ``Resize((R, R))``, antialiased,
+        as the reference's test transform (main.py:398), through the same kernels as the training views."""
+        params = torch.zeros((2, len(sizes), RECORD), dtype=torch.float32)
+        params[:, :, 2:4] = torch.tensor([[float(h), float(w)] for h, w in sizes], dtype=torch.float32)
+        params[:, :, 6:10] = torch.arange(4, dtype=torch.float32)
+        return params.to(device)
+
+    def apply_ragged(self, images, params):
+        """``images``: a list of CUDA uint8 ``[3, H_i, W_i]`` tensors (values read as v / 255) -> two fp32
+        ``[N, 3, R, R]`` views, computed exactly as ``apply`` computes them on ``[u8.float() / 255]``."""
+        device = _check_ragged(images)
+        n = len(images)
+        if tuple(params.shape) != (2, n, RECORD) or params.dtype != torch.float32 or not params.is_contiguous() \
+                or params.device != device:
+            raise ValueError("TwoViewAugment: params must be a contiguous fp32 [2, N, %d] tensor on %s" % (RECORD, device))
+        hw = _sizes_table([tuple(t.shape[1:]) for t in images], device)
+        ptrs = torch.tensor([t.data_ptr() for t in images], dtype=torch.int64).to(device)
+        out = torch.empty((2, n, 3, self.R, self.R), dtype=torch.float32, device=device)
+        tmp = torch.empty_like(out) if self.ksize else None
+        check(lib.byol_augment_apply_ragged(ptrs.data_ptr(), hw.data_ptr(), params.data_ptr(), out.data_ptr(),
+                                            0 if tmp is None else tmp.data_ptr(), n, self.R, self.ksize, ops._stream()),
+              "byol_augment_apply_ragged", kernels=4 if self.ksize else 2)
+        return out[0], out[1]
+
     def __call__(self, images):
+        if isinstance(images, (list, tuple)):
+            device = _check_ragged(images)
+            return self.apply_ragged(images, self.sample_params_ragged([tuple(t.shape[1:]) for t in images], device))
         n, _, hs, ws = images.shape
         return self.apply(images, self.sample_params(n, hs, ws, images.device))
+
+
+def _check_ragged(images):
+    """A non-empty list of contiguous CUDA uint8 [3, H, W] tensors on one device; returns that device."""
+    if not isinstance(images, (list, tuple)) or len(images) == 0:
+        raise ValueError("TwoViewAugment: expected a non-empty list of CUDA uint8 [3, H, W] tensors")
+    device = images[0].device if isinstance(images[0], torch.Tensor) else None
+    for t in images:
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.uint8 or t.dim() != 3 \
+                or t.shape[0] != 3 or t.shape[1] < 1 or t.shape[2] < 1:
+            raise ValueError("TwoViewAugment: every image must be a CUDA uint8 [3, H, W] tensor (no CPU path)")
+        if not t.is_contiguous():
+            raise ValueError("TwoViewAugment: every image must be contiguous")
+        if t.device != device:
+            raise ValueError("TwoViewAugment: all images must be on one device")
+    return device
+
+
+def _sizes_table(sizes, device):
+    """``[(H, W), ...]`` -> device int32 [n, 2]"""
+    hw = torch.tensor([[int(h), int(w)] for h, w in sizes], dtype=torch.int32).reshape(-1, 2)
+    if hw.shape[0] == 0 or int(hw.min()) < 1:
+        raise ValueError("TwoViewAugment: sizes must be a non-empty list of (H, W) with H, W >= 1")
+    return hw.to(device)

@@ -2,8 +2,9 @@
 // /root/reference/main.py:386-397
 //     RandomResizedCrop(R) -> RandomHorizontalFlip(0.5) -> RandomApply(ColorJitter(0.8s, 0.8s, 0.8s, 0.2s), 0.8)
 //     -> RandomGrayscale(0.2) -> GaussianBlur(kernel 0.1 R, p 0.5)
-// for a batch of decoded images already resident in HBM (fp32 NCHW in [0, 1]), so that real data can feed the step at
-// > 20 k images/s/GPU without host-side PIL work.  Three kinds of kernels:
+// for a batch of decoded images already resident in HBM, so that real data can feed the step without host-side PIL
+// work.  Two kinds of input: one fp32 NCHW batch in [0, 1] of equal-sized images, or a table of uint8 CHW images of
+// any sizes, as a GPU JPEG decoder returns them (read as v / 255; the arithmetic after that is the same).  Three kinds of kernels:
 //   augment_params_kernel : per (sample, view) the random parameters (Philox counter RNG keyed by seed / step / sample)
 //   augment_gray_mean_kernel + augment_apply_kernel : crop + bilinear resize + flip + colour ops in the sampled order
 //       (adjust_contrast blends with the MEAN grey level of the image as it stands before that op, hence the small
@@ -48,12 +49,9 @@ struct Rng {
   }
 };
 
-__global__ void augment_params_kernel(float* __restrict__ params, int N, int Hs, int Ws, uint64_t seed, uint64_t step,
-                                      float strength, float p_flip, float p_jitter, float p_gray, float p_blur) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;      // (sample, view)
-  if (i >= 2 * N) return;
-  Rng rng(seed, step * (uint64_t)(2 * N) + (uint64_t)i);
-  float* q = params + (int64_t)i * AP;
+// one (sample, view) record for an Hs x Ws source image, drawn from `rng`
+__device__ __forceinline__ void sample_record(float* q, Rng& rng, int Hs, int Ws, float strength, float p_flip,
+                                              float p_jitter, float p_gray, float p_blur) {
   // RandomResizedCrop.get_params: scale (0.08, 1), ratio (3/4, 4/3), 10 attempts, then a centre crop
   const float area = (float)Hs * (float)Ws;
   const float lr0 = logf(3.f / 4.f), lr1 = logf(4.f / 3.f);
@@ -100,6 +98,28 @@ __global__ void augment_params_kernel(float* __restrict__ params, int N, int Hs,
   q[15] = rng.uniform() < p_blur ? sigma : 0.f;
 }
 
+__global__ void augment_params_kernel(float* __restrict__ params, int N, int Hs, int Ws, uint64_t seed, uint64_t step,
+                                      float strength, float p_flip, float p_jitter, float p_gray, float p_blur) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;      // (sample, view)
+  if (i >= 2 * N) return;
+  Rng rng(seed, step * (uint64_t)(2 * N) + (uint64_t)i);
+  sample_record(params + (int64_t)i * AP, rng, Hs, Ws, strength, p_flip, p_jitter, p_gray, p_blur);
+}
+
+// records for samples [n0, n0 + n) of a batch of N images of their own sizes (hw: int32 [n, 2], rows H, W).  The
+// stream of (view, sample) is the one augment_params_kernel gives it for an N-image batch, so a batch sampled in
+// chunks gets the same records as one call, and equal sizes with n0 = 0, n = N reproduce augment_params_kernel.
+// params: [2, n, AP], view-major over the chunk.
+__global__ void augment_params_ragged_kernel(float* __restrict__ params, const int* __restrict__ hw, int n, int n0,
+                                             int N, uint64_t seed, uint64_t step, float strength, float p_flip,
+                                             float p_jitter, float p_gray, float p_blur) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;      // view * n + j
+  if (i >= 2 * n) return;
+  const int view = i / n, j = i % n;
+  Rng rng(seed, step * (uint64_t)(2 * N) + (uint64_t)view * (uint64_t)N + (uint64_t)(n0 + j));
+  sample_record(params + (int64_t)i * AP, rng, hw[2 * j], hw[2 * j + 1], strength, p_flip, p_jitter, p_gray, p_blur);
+}
+
 __device__ __forceinline__ float clamp01(float v) { return fminf(fmaxf(v, 0.f), 1.f); }
 __device__ __forceinline__ float gray_of(float r, float g, float b) { return 0.2989f * r + 0.587f * g + 0.114f * b; }
 
@@ -126,7 +146,12 @@ __device__ __forceinline__ float tap_w(const AxisTaps& t, int j) {
   const float x = fabsf(((float)(j + t.lo) - t.center + 0.5f) * t.invscale);
   return (x < 1.f ? 1.f - x : 0.f) / t.total;
 }
-__device__ __forceinline__ void sample_crop(const float* __restrict__ src, int Hs, int Ws, const float* q, int R, int y,
+// a source value in [0, 1]: fp32 images are read as they are, uint8 ones as v / 255
+__device__ __forceinline__ float load_px(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float load_px(const uint8_t* p) { return (float)__ldg(p) / 255.f; }
+
+template <typename T>
+__device__ __forceinline__ void sample_crop(const T* __restrict__ src, int Hs, int Ws, const float* q, int R, int y,
                                             int x, float& r, float& g, float& b) {
   const int top = (int)q[0], left = (int)q[1], ch = (int)q[2], cw = (int)q[3];
   const int xx = q[4] != 0.f ? (R - 1 - x) : x;
@@ -135,12 +160,12 @@ __device__ __forceinline__ void sample_crop(const float* __restrict__ src, int H
   float v[3] = {0.f, 0.f, 0.f};
   for (int jy = 0; jy < ty.n; ++jy) {
     const float wy = tap_w(ty, jy);
-    const float* row = src + (int64_t)(top + ty.lo + jy) * Ws + left + tx.lo;
+    const T* row = src + (int64_t)(top + ty.lo + jy) * Ws + left + tx.lo;
     float h[3] = {0.f, 0.f, 0.f};
     for (int jx = 0; jx < tx.n; ++jx) {
       const float wx = tap_w(tx, jx);
 #pragma unroll
-      for (int c = 0; c < 3; ++c) h[c] += wx * __ldg(row + jx + c * plane);
+      for (int c = 0; c < 3; ++c) h[c] += wx * load_px(row + jx + c * plane);
     }
 #pragma unroll
     for (int c = 0; c < 3; ++c) v[c] += wy * h[c];
@@ -201,18 +226,36 @@ __device__ __forceinline__ void colour_ops(const float* q, float& r, float& g, f
   }
 }
 
+// where sample n's image is and how large: one fp32 [N, 3, Hs, Ws] batch, or a table of per-image uint8 [3, H, W]
+// tensors with their sizes (hw: int32 [N, 2])
+struct DenseSrc {
+  using T = float;
+  const float* p;
+  int Hs, Ws;
+  __device__ const float* image(int n, int& h, int& w) const { h = Hs; w = Ws; return p + (int64_t)n * 3 * Hs * Ws; }
+};
+struct RaggedSrc {
+  using T = uint8_t;
+  const uint8_t* const* p;
+  const int* hw;
+  __device__ const uint8_t* image(int n, int& h, int& w) const { h = hw[2 * n]; w = hw[2 * n + 1]; return p[n]; }
+};
+
 // mean grey level per (sample, view) of the image as it stands right before adjust_contrast (sum in fp32 per block,
 // blocks combined in fixed point); skipped (mean unused) when the jitter is off
-__global__ void augment_gray_mean_kernel(const float* __restrict__ src, const float* __restrict__ params,
-                                         Fix128* __restrict__ gray_sum, int N, int Hs, int Ws, int R) {
+template <typename Src>
+__global__ void augment_gray_mean_kernel(Src src, const float* __restrict__ params, Fix128* __restrict__ gray_sum,
+                                         int N, int R) {
   const int sv = blockIdx.y;                      // sample * 2 + view... laid out view-major: sv = view * N + n
   const int n = sv % N;
   const float* q = params + (int64_t)sv * AP;
   if (q[5] == 0.f) return;
+  int Hs, Ws;
+  const typename Src::T* img = src.image(n, Hs, Ws);
   float acc = 0.f;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < R * R; i += gridDim.x * blockDim.x) {
     float r, g, b;
-    sample_crop(src + (int64_t)n * 3 * Hs * Ws, Hs, Ws, q, R, i / R, i % R, r, g, b);
+    sample_crop(img, Hs, Ws, q, R, i / R, i % R, r, g, b);
     colour_ops(q, r, g, b, 1, 0.f);
     acc += gray_of(r, g, b);
   }
@@ -229,17 +272,19 @@ __global__ void augment_gray_mean_kernel(const float* __restrict__ src, const fl
 }
 
 // out[view][n, c, y, x] (fp32 NCHW): crop / resize / flip, colour jitter, grayscale
-__global__ void augment_apply_kernel(const float* __restrict__ src, const float* __restrict__ params,
-                                     const Fix128* __restrict__ gray_sum, float* __restrict__ out, int N, int Hs, int Ws,
-                                     int R) {
+template <typename Src>
+__global__ void augment_apply_kernel(Src src, const float* __restrict__ params, const Fix128* __restrict__ gray_sum,
+                                     float* __restrict__ out, int N, int R) {
   const int sv = blockIdx.y;
   const int n = sv % N;
   const float* q = params + (int64_t)sv * AP;
   const float mean_gray = (float)(fix_value(gray_sum[sv]) / (double)(R * R));
   float* o = out + (int64_t)sv * 3 * R * R;
+  int Hs, Ws;
+  const typename Src::T* img = src.image(n, Hs, Ws);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < R * R; i += gridDim.x * blockDim.x) {
     float r, g, b;
-    sample_crop(src + (int64_t)n * 3 * Hs * Ws, Hs, Ws, q, R, i / R, i % R, r, g, b);
+    sample_crop(img, Hs, Ws, q, R, i / R, i % R, r, g, b);
     colour_ops(q, r, g, b, 4, mean_gray);
     if (q[14] != 0.f) { const float gr = gray_of(r, g, b); r = gr; g = gr; b = gr; }
     o[i] = r; o[R * R + i] = g; o[2 * R * R + i] = b;
@@ -289,22 +334,20 @@ extern "C" int byol_augment_params(float* params, int N, int Hs, int Ws, uint64_
   return check_launch("augment_params_kernel");
 }
 
-// src: fp32 NCHW [N, 3, Hs, Ws] in [0, 1]; out: fp32 [2, N, 3, R, R] (view 1 | view 2); tmp: same size as out (blur);
-// gray_sum: part of the ABI, no longer used (the per-view sums live in the stream's fix_scratch); ksize: odd Gaussian kernel size (0 = no blur stage).
-extern "C" int byol_augment_apply(const float* src, const float* params, float* out, float* tmp, double* gray_sum,
-                                  int N, int Hs, int Ws, int R, int ksize, cudaStream_t stream) {
-  BYOL_CHECK_ARG(src && params && out && gray_sum && N > 0 && R > 0, "byol_augment_apply: bad args");
-  BYOL_CHECK_ARG(ksize == 0 || (ksize % 2 == 1 && ksize < 2 * R - 1 && tmp != nullptr), "byol_augment_apply: bad ksize %d", ksize);
+// the gray-mean, apply and blur passes over any source (DenseSrc / RaggedSrc)
+template <typename Src>
+static int augment_apply_launch(Src src, const float* params, float* out, float* tmp, int N, int R, int ksize,
+                                cudaStream_t stream, const char* what) {
   Fix128* gsum = fix_scratch(stream, 2 * (int64_t)N);
   if (gsum == nullptr) return -2;
   int bx = (R * R + 255) / 256;
   if (bx > 64) bx = 64;
   dim3 grid((unsigned)bx, (unsigned)(2 * N));
-  augment_gray_mean_kernel<<<grid, 256, 0, stream>>>(src, params, gsum, N, Hs, Ws, R);
-  augment_apply_kernel<<<grid, 256, 0, stream>>>(src, params, gsum, out, N, Hs, Ws, R);
+  augment_gray_mean_kernel<<<grid, 256, 0, stream>>>(src, params, gsum, N, R);
+  augment_apply_kernel<<<grid, 256, 0, stream>>>(src, params, gsum, out, N, R);
   // every block of augment_apply_kernel read the sums: leave the scratch zeroed (fix_scratch)
   if (cudaMemsetAsync(gsum, 0, 2 * (size_t)N * sizeof(Fix128), stream) != cudaSuccess) {
-    set_last_error("byol_augment_apply: memset failed");
+    set_last_error("%s: memset failed", what);
     return -2;
   }
   if (ksize > 0) {
@@ -312,4 +355,37 @@ extern "C" int byol_augment_apply(const float* src, const float* params, float* 
     augment_blur_kernel<<<grid, 256, 0, stream>>>(tmp, out, params, R, ksize, 0);
   }
   return fix_done(stream, check_launch("augment kernels"));
+}
+
+// src: fp32 NCHW [N, 3, Hs, Ws] in [0, 1]; out: fp32 [2, N, 3, R, R] (view 1 | view 2); tmp: same size as out (blur);
+// gray_sum: part of the ABI, no longer used (the per-view sums live in the stream's fix_scratch); ksize: odd Gaussian kernel size (0 = no blur stage).
+extern "C" int byol_augment_apply(const float* src, const float* params, float* out, float* tmp, double* gray_sum,
+                                  int N, int Hs, int Ws, int R, int ksize, cudaStream_t stream) {
+  BYOL_CHECK_ARG(src && params && out && gray_sum && N > 0 && R > 0, "byol_augment_apply: bad args");
+  BYOL_CHECK_ARG(ksize == 0 || (ksize % 2 == 1 && ksize < 2 * R - 1 && tmp != nullptr), "byol_augment_apply: bad ksize %d", ksize);
+  return augment_apply_launch(DenseSrc{src, Hs, Ws}, params, out, tmp, N, R, ksize, stream, "byol_augment_apply");
+}
+
+// Mixed-size batches.  hw: device int32 [n, 2] (H, W of each image); params: [2, n, 16] records for samples
+// [n0, n0 + n) of an N-image batch (see augment_params_ragged_kernel).
+extern "C" int byol_augment_params_ragged(float* params, const int* hw, int n, int n0, int N, uint64_t seed,
+                                          uint64_t step, float strength, float p_flip, float p_jitter, float p_gray,
+                                          float p_blur, cudaStream_t stream) {
+  BYOL_CHECK_ARG(params && hw, "byol_augment_params_ragged: null pointer");
+  BYOL_CHECK_ARG(n > 0 && n0 >= 0 && N > 0 && n0 <= N - n, "byol_augment_params_ragged: bad chunk n %d n0 %d N %d",
+                 n, n0, N);
+  augment_params_ragged_kernel<<<(2 * n + 127) / 128, 128, 0, stream>>>(params, hw, n, n0, N, seed, step, strength,
+                                                                       p_flip, p_jitter, p_gray, p_blur);
+  return check_launch("augment_params_ragged_kernel");
+}
+
+// srcs: device table of N pointers to uint8 CHW [3, H_i, W_i] images (values v read as v / 255); hw: device int32
+// [N, 2]; the rest as byol_augment_apply.
+extern "C" int byol_augment_apply_ragged(const uint8_t* const* srcs, const int* hw, const float* params, float* out,
+                                         float* tmp, int N, int R, int ksize, cudaStream_t stream) {
+  BYOL_CHECK_ARG(srcs && hw && params && out, "byol_augment_apply_ragged: null pointer");
+  BYOL_CHECK_ARG(N > 0 && 2 * (int64_t)N <= 65535 && R > 0, "byol_augment_apply_ragged: bad N %d or R %d", N, R);
+  BYOL_CHECK_ARG(ksize == 0 || (ksize % 2 == 1 && ksize < 2 * R - 1 && tmp != nullptr),
+                 "byol_augment_apply_ragged: bad ksize %d", ksize);
+  return augment_apply_launch(RaggedSrc{srcs, hw}, params, out, tmp, N, R, ksize, stream, "byol_augment_apply_ragged");
 }

@@ -265,6 +265,16 @@ int byol_augment_params(float* params, int N, int Hs, int Ws, uint64_t seed, uin
                         float p_flip, float p_jitter, float p_gray, float p_blur, byol_stream_t stream);
 int byol_augment_apply(const float* src, const float* params, float* out /* [2, N, 3, R, R] */, float* tmp,
                        double* gray_sum /* [2N] */, int N, int Hs, int Ws, int R, int ksize, byol_stream_t stream);
+/* mixed-size batches: hw is a device int32 [n, 2] table of image heights and widths.  The sampler draws the records of
+ * samples [n0, n0 + n) of an N-image batch (chunks of one batch give the records of one call; equal sizes with n0 = 0,
+ * n = N give byol_augment_params' records).  The apply reads a device table of N uint8 CHW [3, H_i, W_i] images as
+ * v / 255 and otherwise computes exactly what byol_augment_apply does. */
+int byol_augment_params_ragged(float* params /* [2, n, 16] */, const int* hw, int n, int n0, int N, uint64_t seed,
+                               uint64_t step, float strength, float p_flip, float p_jitter, float p_gray, float p_blur,
+                               byol_stream_t stream);
+int byol_augment_apply_ragged(const uint8_t* const* srcs, const int* hw, const float* params,
+                              float* out /* [2, N, 3, R, R] */, float* tmp, int N, int R, int ksize,
+                              byol_stream_t stream);
 
 #ifdef __cplusplus
 }
