@@ -1077,19 +1077,24 @@ static int conv_igemm_impl(const void* src, const void* wt, void* dst, const voi
   const int BN = (Ndim > 64 && !grouped) ? 128 : 64;
   p.tiles_n = (Ndim + BN - 1) / BN;
   int tiles_m = (p.M + BM - 1) / BM;
+  // the dX parity classes with at least one tap (a 1x1 / stride-2 / pad-0 dgrad has only class (0, 0))
+  int ncls = 0, cls_list[4];
+  for (int cls = 0; cls < 4; ++cls) {
+    const int ph = cls >> 1, pw = cls & 1;
+    const int nkh = (KH - ((ph + pad) & 1) + 1) >> 1, nkw = (KW - ((pw + pad) & 1) + 1) >> 1;
+    if (nkh > 0 && nkw > 0) cls_list[ncls++] = cls;
+  }
+  // Parity mode launches tiles for the classes with taps only, so the residual of a pixel without taps would never
+  // be added: with a residual, a layer with tap-less classes takes the gathered path, which visits every dX pixel.
   if (mode == 1 && stride == 2 && Ho % 2 == 0 && Wo % 2 == 0 && C % BK == 0 && p.small_src && KH <= 3 && KW <= 3 &&
-      ((int64_t)Nimg * (Ho / 2) * (Wo / 2)) % BM == 0 && !out_fp32) {
+      ((int64_t)Nimg * (Ho / 2) * (Wo / 2)) % BM == 0 && !out_fp32 && (resid == nullptr || ncls == 4)) {
     p.parity = 1;
     p.Hh = Ho / 2;
     p.Wh = Wo / 2;
     p.Mc = Nimg * p.Hh * p.Wh;
-    p.ncls = 0;
-    for (int cls = 0; cls < 4; ++cls) {
-      const int ph = cls >> 1, pw = cls & 1;
-      const int nkh = (KH - ((ph + pad) & 1) + 1) >> 1, nkw = (KW - ((pw + pad) & 1) + 1) >> 1;
-      if (nkh > 0 && nkw > 0) p.cls_list[p.ncls++] = cls;
-    }
-    if (p.ncls < 4) {   // pixels of classes without any tap receive zero gradient
+    p.ncls = ncls;
+    for (int i = 0; i < ncls; ++i) p.cls_list[i] = cls_list[i];
+    if (p.ncls < 4) {   // pixels of classes without any tap receive zero gradient (no residual here)
       cudaError_t e = cudaMemsetAsync(dst, 0, (size_t)p.M * ldc * sizeof(bf16), stream);
       if (e != cudaSuccess) { set_last_error("byol_conv_igemm: memset failed: %s", cudaGetErrorString(e)); return -2; }
     }
