@@ -118,6 +118,10 @@ _SIGNATURES = {
     "byol_augment_apply_ragged": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
     "byol_xchg_layout": [c_void_p, c_void_p, c_void_p],
     "byol_xchg_sum": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p],
+    # k-NN evaluation, csrc/knn.cu
+    "byol_l2_normalize_rows": [c_void_p, c_void_p, c_int64, c_int, c_int64, c_void_p],
+    "byol_knn_topk": [c_void_p, c_int, c_int, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
+    "byol_knn_vote": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p],
     "byol_abi_version": [],
     "byol_device_sm_count": [],
 }

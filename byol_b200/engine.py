@@ -183,6 +183,9 @@ class Engine(object):
         self.bwd32 = False
         self.cls_planes = None
         self.s_online = self.s_target = None
+        # weight layouts of representations(): apart from the training step's, so that a call between a captured
+        # forward and its backward leaves every buffer the graphs read untouched (allocated on first use)
+        self.w_eval = self.s_eval = None
         # block-output BatchNorm fused into the expanding 1x1 GEMMs (see _fuse3).  OFF by default: the statistics pass
         # re-runs the GEMM, so the fused form moves more work than the unfused conv + BN-apply kernels
         # (tools/time_fused.py times both).  It saves 7-14 GB of activations per 512 images; BYOL_B200_FUSE3=1
@@ -301,6 +304,7 @@ class Engine(object):
         self.graphs = {}           # captured steps point into the old buffers
         self._plans = {}
         self.s_online = self.s_target = None
+        self.w_eval = self.s_eval = None
         if self.T:
             self.s_online = _SplitWeights(self.units, self.device, self.T, want_dgrad=self.bwd32)
             self.s_target = _SplitWeights(self.units, self.device, self.T)
@@ -715,9 +719,10 @@ class Engine(object):
             res.append(conv[id(a)])
         return res
 
-    def forward_lanes(self, augs, lanes, train, rep_bf16_out=None, x8=None):
+    def forward_lanes(self, augs, lanes, train, rep_bf16_out=None, x8=None, reps_only=False):
         """augs: fp32 NCHW inputs per lane; lanes: (flat params, weight set, saved dict or None) per lane.
-        Returns per lane (representation fp32, projection fp32, prediction fp32).
+        Returns per lane (representation fp32, projection fp32, prediction fp32); with reps_only (encoder-only
+        evaluation, see representations) the forward stops after the average pool and returns (representation,).
 
         With four lanes (online x2, target x2) the two pairs run on two CUDA streams forked from / joined into the
         caller's stream: the HBM-bound BatchNorm kernels of one pair overlap the tensor-core convolutions of the
@@ -728,7 +733,7 @@ class Engine(object):
         if x8 is None:
             x8 = self.convert_inputs(augs)
         if self.T:
-            res, reps_b = self._forward_split(x8, lanes, train, rep_bf16_out or [None] * L)
+            res, reps_b = self._forward_split(x8, lanes, train, rep_bf16_out or [None] * L, reps_only)
             if train:
                 torch._foreach_add_([b.num_batches_tracked for b in self.bn_modules], L)
             return res, reps_b
@@ -755,7 +760,7 @@ class Engine(object):
             self._group_order = order
             with torch.cuda.stream(stream):
                 res, rb = self._forward_group([x8[i] for i in idxs], [lanes[i] for i in idxs], train,
-                                              [rep_bf16_out[i] for i in idxs])
+                                              [rep_bf16_out[i] for i in idxs], reps_only)
             for j, i in enumerate(idxs):
                 results[i], reps_b_all[i] = res[j], rb[j]
         if two:
@@ -770,7 +775,7 @@ class Engine(object):
             torch._foreach_add_([b.num_batches_tracked for b in self.bn_modules], L)
         return results, reps_b_all
 
-    def _forward_group(self, x8, lanes, train, rep_bf16_out):
+    def _forward_group(self, x8, lanes, train, rep_bf16_out, reps_only=False):
         L = len(lanes)
         st = self.stem
         self._zpool = _Pool(L * 2 * self.bn_channels, self.device, zero=True) if train else None
@@ -803,6 +808,8 @@ class Engine(object):
             reps_b.append(yb)
             if lanes[i][2] is not None:
                 lanes[i][2]["final_shape"] = (n, h, w, c)
+        if reps_only:
+            return [(r,) for r in reps_f], reps_b
         # Under SyncBatchNorm the fused MLP kernels are cooperative (most of the GPU each) AND wait for their peer
         # ranks: two of them from different streams must never be schedulable in different orders on different ranks
         # (rank X resident with stream A's kernel, rank Y with stream B's -> circular wait).  So the second lane pair
@@ -823,12 +830,19 @@ class Engine(object):
     # Lanes run lock-step on the caller's stream.  For the online lanes the bf16 tensors the (bf16) backward pass
     # needs are written alongside, under the same keys as the fast path.
     # ------------------------------------------------------------------------------------------
+    def _split_set(self, lane):
+        """The plane layouts a lane runs on: its own weight set when it carries _SplitWeights (representations),
+        else the online or target set by its parameter vector."""
+        if isinstance(lane[1], _SplitWeights):
+            return lane[1]
+        return self.s_online if lane[0] is self.theta else self.s_target
+
     def _conv_bn_split(self, u, xs, lanes, train, is_linear=False):
         L, C, T = len(lanes), u.cout, self.T
         stats = torch.zeros(L * 2 * C, dtype=torch.float64, device=self.device) if train else None
         ys = []
         for i, (flat, _, _) in enumerate(lanes):
-            wset = self.s_online if flat is self.theta else self.s_target
+            wset = self._split_set(lanes[i])
             bias = flat[u.b_off:u.b_off + C] if u.b_off >= 0 else None
             if u.kind == "linear":
                 y = ops.linear_fprop(xs[i], wset.w[u.idx], bias=bias, out_fp32=True)
@@ -916,7 +930,7 @@ class Engine(object):
         h, c = self._conv_bn_split(l1, [x[0] for x in X], lanes, train)
         outs = []
         for i, (flat, _, saved) in enumerate(lanes):
-            wset = self.s_online if flat is self.theta else self.s_target
+            wset = self._split_set(lanes[i])
             _, ap, ab, _ = ops.bn_apply_f32(h[i], c[i][0], c[i][1], True, self.T, want_planes=True,
                                             want_copy=saved is not None and not self.bwd32)
             outs.append(ops.linear_fprop(ap, wset.w[l2.idx], bias=flat[l2.b_off:l2.b_off + l2.cout], out_fp32=True))
@@ -926,7 +940,7 @@ class Engine(object):
                 saved[key] = {"x": X[i][1], "h": ops.cast_bf16(h[i]), "c": c[i], "a": ab}
         return outs
 
-    def _forward_split(self, x8, lanes, train, rep_bf16_out):
+    def _forward_split(self, x8, lanes, train, rep_bf16_out, reps_only=False):
         L, T = len(lanes), self.T
         st = self.stem
         keep = [lanes[i][2] is not None for i in range(L)]
@@ -950,6 +964,8 @@ class Engine(object):
         for b in self.blocks:
             X = self._block_fwd_split(b, X, lanes, train)
         reps_f, reps_b, M = [], [], []
+        if reps_only:
+            return [(ops.avgpool_f32(X[i][0]),) for i in range(L)], [None] * L
         for i in range(L):
             n, h, w, c = X[i][0].shape
             rep = ops.avgpool_f32(X[i][0])
@@ -1427,6 +1443,26 @@ class Engine(object):
             self.s_target.prepare(self.units, mean)
         else:
             self.prep_weights(mean, self.w_target, want_dgrad=False)
+
+    def representations(self, images, flat):
+        """Encoder-only eval-mode forward of fp32 NCHW `images` at the parameter vector `flat` (theta or the EMA mean):
+        the average-pooled encoder output, fp32 [B, rep_dim].  One lane on the caller's stream with eval BatchNorm
+        (running statistics); nothing is saved or updated.  It runs the kernels of the eval forward's representation
+        lanes on the same inputs, so the result has their bits.  Its weight layouts live in their own buffers
+        (w_eval / s_eval, encoder layers only): the captured training step's buffers are neither read nor written."""
+        enc = self.units[:self.mlps[0][0].idx]      # walk_layers lists the encoder's units first
+        if self.T:
+            if self.s_eval is None:
+                self.s_eval = _SplitWeights(enc, self.device, self.T)
+            self.s_eval.prepare(enc, flat)
+            wset = self.s_eval
+        else:
+            if self.w_eval is None:
+                self.w_eval = _Weights(enc, self.device, False)
+            self.prep_weights(flat, self.w_eval, want_dgrad=False)
+            wset = self.w_eval
+        res, _ = self.forward_lanes([images], [(flat, wset, None)], False, reps_only=True)
+        return res[0][0]
 
     def graphed_step(self, model, a1, a2):
         """Returns the captured step for this input geometry, or None while it is still warming up / if graphs are

@@ -253,6 +253,31 @@ class BYOL(nn.Module):
         nn.utils.parameters_to_vector at main.py:212,223,255) — here a persistent buffer, not a copy."""
         return self._ensure_ready(1).theta if self._rep_cat is None else self._engine.theta
 
+    def representations(self, images, network="online"):
+        """Frozen-encoder features for evaluation (k-NN, linear probes): fp32 [B, base_network_output_size], the
+        average-pooled encoder output of fp32 NCHW CUDA `images` (values in [0, 1], any batch size and resolution the
+        stem supports).  network="target" runs the EMA weights (``target_network.mean``).
+
+        Always eval-mode BatchNorm (running statistics), whatever ``self.training`` is; it updates nothing (no EMA step,
+        no running statistics, no ``num_batches_tracked``) and computes no gradient.  Only the encoder runs (no
+        projector, predictor or classifier), so the result equals ``model.eval(); model(x, x)["online_representation1"]``
+        (``"target_representation1"``) bit for bit, at about a quarter of its cost.  It may be called anywhere in a
+        training loop, also between a CUDA-graphed forward and its backward: it touches no buffer the training step
+        uses."""
+        if network not in ("online", "target"):
+            raise ValueError("network must be 'online' or 'target', got %r" % (network,))
+        if not isinstance(images, torch.Tensor) or not images.is_cuda:
+            raise RuntimeError("byol_b200.BYOL.representations needs CUDA tensors (no CPU path)")
+        if images.dim() != 4 or images.shape[0] < 1:
+            raise ValueError("images must be a non-empty [B, C, H, W] batch, got shape %s" % (tuple(images.shape),))
+        eng = self._engine
+        if not eng.plan_is_current():
+            eng.flatten()
+            eng.build_plan()
+        flat = self.target_network.mean if network == "target" else eng.theta
+        with torch.no_grad():
+            return eng.representations(images.detach().contiguous().float(), flat)
+
     def forward(self, augmentation1, augmentation2):
         """Returns the online and target network representations, projections and predictions (main.py:242-276)."""
         if not augmentation1.is_cuda:

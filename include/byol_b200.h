@@ -276,6 +276,23 @@ int byol_augment_apply_ragged(const uint8_t* const* srcs, const int* hw, const f
                               float* out /* [2, N, 3, R, R] */, float* tmp, int N, int R, int ksize,
                               byol_stream_t stream);
 
+/* ---- weighted k-NN evaluation of frozen features (csrc/knn.cu; the similarity chunks come from byol_conv_igemm as a
+ *      linear layer over bf16 rows).  Entries rank by similarity descending, then bank index ascending (-0 as +0, NaN
+ *      last): a total order, so the selection is exactly the first k entries of a full sort of each row. ---- */
+/* y bf16 [R, D] = x / ||x||_2 per row of fp32 x [R, D] (row pitch ldx); the norm is a fixed-order fp32 sum; a zero row
+ * stays zero */
+int byol_l2_normalize_rows(const float* x, void* y, int64_t R, int D, int64_t ldx, byol_stream_t stream);
+/* sim fp32 [Q, Nc] (row pitch ld): similarities of Q queries against bank rows n0 .. n0 + Nc - 1.  top_vals fp32 /
+ * top_idx int32 [Q, k] (1 <= k <= 256): per query the k best entries, best first, of the chunk merged with the list
+ * already there (merge = 1) or of the chunk alone (merge = 0); slots beyond the entries seen hold -inf / -1 */
+int byol_knn_topk(const float* sim, int Q, int Nc, int64_t ld, int n0, int k, int merge, float* top_vals,
+                  int* top_idx, byol_stream_t stream);
+/* pred int32 [Q, 5]: the 5 best classes by score = sum over the class's neighbours (rank order, fp64) of the fp32
+ * weight expf(s / temperature), then class index ascending; bank_labels int64 in [0, num_classes); slots beyond
+ * num_classes hold -1; pred_scores (optional) fp32 [Q, 5]: the scores of pred */
+int byol_knn_vote(const float* top_vals, const int* top_idx, const int64_t* bank_labels, int Q, int k, int num_classes,
+                  float temperature, int* pred, float* pred_scores, byol_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
