@@ -122,6 +122,11 @@ _SIGNATURES = {
     "byol_l2_normalize_rows": [c_void_p, c_void_p, c_int64, c_int, c_int64, c_void_p],
     "byol_knn_topk": [c_void_p, c_int, c_int, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "byol_knn_vote": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p],
+    # linear evaluation, csrc/linear_eval.cu
+    "byol_linprobe_ce": [c_void_p, c_int64, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                         c_void_p],
+    "byol_linprobe_sgd": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float, c_int, c_int,
+                          c_int, c_int, c_void_p],
     "byol_abi_version": [],
     "byol_device_sm_count": [],
 }

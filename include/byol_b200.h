@@ -293,6 +293,27 @@ int byol_knn_topk(const float* sim, int Q, int Nc, int64_t ld, int n0, int k, in
 int byol_knn_vote(const float* top_vals, const int* top_idx, const int64_t* bank_labels, int Q, int k, int num_classes,
                   float temperature, int* pred, float* pred_scores, byol_stream_t stream);
 
+/* ---- linear evaluation of frozen features (csrc/linear_eval.cu): H linear heads over one feature matrix, stored as
+ *      one [H * Cp, D] weight matrix (Cp = C rounded up to a multiple of 8, rows c >= C of each head are padding) and
+ *      [H, Cp] biases, so that one byol_conv_igemm computes the logits of every head. ---- */
+/* logits fp32 [B, >= H * Cp] (row pitch ld, a multiple of 4; 16-byte aligned): per row r and head h the softmax
+ * cross-entropy of columns h * Cp .. h * Cp + C - 1 against labels[r] (int64; 2 <= C; a row whose label is outside
+ * [0, C) is ignored: no loss, no hit, zero gradient).  Outputs (each
+ * optional, at least one given): dlogits bf16 [B, H * Cp] (16-byte aligned) = (softmax - onehot) / B, 0 in the padding
+ * columns; loss_sum fp32 [H] += the per-head sum of the row losses; hits int64 [H, 2] += the rows whose label has
+ * rank < 1 / rank < 5 (rank = the number of other logits not <= the label's: strictly larger ones and NaNs; a NaN label
+ * logit is a miss).  Deterministic (fixed-point / integer sums). */
+int byol_linprobe_ce(const float* logits, int64_t ld, const int64_t* labels, int B, int H, int C, int Cp,
+                     void* dlogits, float* loss_sum, long long* hits, byol_stream_t stream);
+/* One Nesterov-SGD step of every head, in torch.optim.SGD's order with each fp32 operation rounded on its own:
+ * g = dW + wd*w; buf = momentum*buf + g; d = g + momentum*buf; w = w - lr*d with lr = fp32(lr[h] * lr_scale).
+ * params / grads / momentum_buf: fp32 [H * Cp * D] weights followed by [H * Cp] biases (16-byte aligned); lr, wd: fp32
+ * [H] on the device.  Writes weight_bf16 [H * Cp, D] = bf16(w) (round to nearest even) and zeroes grads; the padding
+ * rows c >= C are not touched. */
+int byol_linprobe_sgd(float* params, float* grads, float* momentum_buf, void* weight_bf16, const float* lr,
+                      const float* wd, float lr_scale, float momentum, int H, int C, int Cp, int D,
+                      byol_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
