@@ -76,6 +76,8 @@ _SIGNATURES = {
     "byol_ema_update": [c_void_p, c_void_p, c_float, c_float, c_int64, c_void_p],
     "byol_lars_sgd_step": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                            c_void_p, c_void_p, c_int, c_void_p, c_float, c_float, c_float, c_int, c_void_p],
+    "byol_sgd_nesterov_step": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
+                               c_float, c_float, c_void_p],
     "byol_ce_topk_fwd": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                          c_void_p],
     "byol_ce_bwd": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p],

@@ -145,6 +145,16 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
+// One Nesterov-SGD element update in torch.optim.SGD(nesterov=True, dampening=0)'s order, every fp32 operation rounded
+// on its own (no FMA contraction): g = grad + wd*w; buf = mu*buf + g; d = g + mu*buf; w = w - lr*d; grad = 0.
+__device__ __forceinline__ void nesterov_update(float& w, float& buf, float& grad, float lr, float wd, float mu) {
+  const float g = __fadd_rn(grad, __fmul_rn(wd, w));
+  buf = __fadd_rn(__fmul_rn(mu, buf), g);
+  const float d = __fadd_rn(g, __fmul_rn(mu, buf));
+  w = __fsub_rn(w, __fmul_rn(lr, d));
+  grad = 0.f;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -136,21 +136,13 @@ linprobe_ce_kernel(const float* __restrict__ logits, int64_t ld, const int64_t* 
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Nesterov SGD, torch.optim.SGD(nesterov=True, dampening=0)'s order with every operation rounded on its own (no FMA
-// contraction, as ema_kernel):
+// contraction, as ema_kernel; nesterov_update, common.cuh):
 //   g = dW + wd * w;   buf = mu * buf + g;   d = g + mu * buf;   w = w - lr * d
 // The momentum starts at zero, so the first step gives buf = g, torch's first step.  One block per weight row (h, c):
 // the row's D weights as float4, then its bias by thread 0.  The same pass writes bf16(w) (round to nearest even) to
 // the GEMM copy and zeroes dW and db, so the next wgrad / column sum accumulate onto zero.  Padding rows c >= C are
 // never read or written.
 // ---------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void nesterov(float& w, float& buf, float& grad, float lr, float wd, float mu) {
-  const float g = __fadd_rn(grad, __fmul_rn(wd, w));
-  buf = __fadd_rn(__fmul_rn(mu, buf), g);
-  const float d = __fadd_rn(g, __fmul_rn(mu, buf));
-  w = __fsub_rn(w, __fmul_rn(lr, d));
-  grad = 0.f;
-}
-
 __global__ void __launch_bounds__(SGD_THREADS)
 linprobe_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict__ m, bf16* __restrict__ wb,
                     const float* __restrict__ lr, const float* __restrict__ wd, float lr_scale, float mu, int H, int C,
@@ -167,10 +159,10 @@ linprobe_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restr
     uint2* __restrict__ b4 = reinterpret_cast<uint2*>(wb + row * D);
     for (int j = threadIdx.x; j < d4; j += SGD_THREADS) {
       float4 wv = w4[j], gv = g4[j], mv = m4[j];
-      nesterov(wv.x, mv.x, gv.x, rate, decay, mu);
-      nesterov(wv.y, mv.y, gv.y, rate, decay, mu);
-      nesterov(wv.z, mv.z, gv.z, rate, decay, mu);
-      nesterov(wv.w, mv.w, gv.w, rate, decay, mu);
+      nesterov_update(wv.x, mv.x, gv.x, rate, decay, mu);
+      nesterov_update(wv.y, mv.y, gv.y, rate, decay, mu);
+      nesterov_update(wv.z, mv.z, gv.z, rate, decay, mu);
+      nesterov_update(wv.w, mv.w, gv.w, rate, decay, mu);
       w4[j] = wv;
       m4[j] = mv;
       g4[j] = gv;
@@ -178,7 +170,7 @@ linprobe_sgd_kernel(float* __restrict__ w, float* __restrict__ g, float* __restr
     }
     if (threadIdx.x == 0) {
       const int64_t bi = rows * D + row;                 // the biases [H, Cp] follow the weights
-      nesterov(w[bi], m[bi], g[bi], rate, decay, mu);
+      nesterov_update(w[bi], m[bi], g[bi], rate, decay, mu);
     }
   }
 }

@@ -6,6 +6,7 @@
 //                         separately rounded fp32 ops; bit-exact => no FMA contraction)
 //   byol_lars_*         : /root/reference/optimizers/lars.py:84-127 (apply_adaptive_lrs + wrapped SGD step,
 //                         torch.optim.SGD momentum=0.9, dampening 0, no nesterov, weight decay folded by LARS)
+//   byol_sgd_nesterov_step : Nesterov SGD over the same chunk tables (fine-tuning, byol_b200/finetune.py)
 #include "common.cuh"
 
 namespace byol {
@@ -179,6 +180,61 @@ lars_norms_kernel(const uint64_t* __restrict__ p_ptrs, const uint64_t* __restric
   }
 }
 
+// The elementwise part of a chunk update, shared by the LARS and the Nesterov-SGD kernels: `rule` updates element i
+// of the chunk (vec: the four elements 4i .. 4i + 3 as float4, when p / g / momentum share a 16-byte phase; scalar:
+// element i), one thread per element (group), block-strided.
+template <class Rule, class G>
+__device__ __forceinline__ void update_chunk(float* __restrict__ p, G* __restrict__ g, float* __restrict__ mom, int len,
+                                             const Rule& rule) {
+  int done = 0;
+  if (aligned16(p, g, mom)) {
+    const int n4 = len >> 2;
+    for (int i = threadIdx.x; i < n4; i += blockDim.x) rule.vec(p, g, mom, i);
+    done = n4 << 2;
+  }
+  for (int i = done + threadIdx.x; i < len; i += blockDim.x) rule.scalar(p, g, mom, i);
+}
+
+// LARS-scaled SGD with momentum (torch.optim.SGD, momentum without nesterov; mom may be null: no momentum)
+struct LarsRule {
+  float w, ratio, rate, momentum;
+  int first_step;
+  __device__ __forceinline__ void vec(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ mom,
+                                      int i) const {
+    float4* __restrict__ p4 = reinterpret_cast<float4*>(p);
+    const float4* __restrict__ g4 = reinterpret_cast<const float4*>(g);
+    float4* __restrict__ m4 = reinterpret_cast<float4*>(mom);
+    float4 pv = p4[i];
+    float4 gv = __ldg(g4 + i);
+    if (w > 0.f) { gv.x += w * pv.x; gv.y += w * pv.y; gv.z += w * pv.z; gv.w += w * pv.w; }
+    gv.x *= ratio; gv.y *= ratio; gv.z *= ratio; gv.w *= ratio;
+    float4 b = gv;
+    if (mom != nullptr) {
+      if (!first_step) {
+        const float4 mv = m4[i];
+        b.x = momentum * mv.x + gv.x; b.y = momentum * mv.y + gv.y;
+        b.z = momentum * mv.z + gv.z; b.w = momentum * mv.w + gv.w;
+      }
+      m4[i] = b;
+    }
+    pv.x -= rate * b.x; pv.y -= rate * b.y; pv.z -= rate * b.z; pv.w -= rate * b.w;
+    p4[i] = pv;
+  }
+  __device__ __forceinline__ void scalar(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ mom,
+                                         int i) const {
+    const float pv = p[i];
+    float gv = g[i];
+    if (w > 0.f) gv = gv + w * pv;
+    gv = gv * ratio;
+    float b = gv;
+    if (mom != nullptr) {
+      b = first_step ? gv : momentum * mom[i] + gv;
+      mom[i] = b;
+    }
+    p[i] = pv - rate * b;
+  }
+};
+
 __global__ void __launch_bounds__(256)
 lars_update_kernel(const uint64_t* __restrict__ p_ptrs, const uint64_t* __restrict__ g_ptrs,
                    const uint64_t* __restrict__ m_ptrs, const int64_t* __restrict__ chunk_start,
@@ -217,44 +273,44 @@ lars_update_kernel(const uint64_t* __restrict__ p_ptrs, const uint64_t* __restri
     if (threadIdx.x == 0) s_ratio = ratio;
   }
   __syncthreads();
-  const float ratio = s_ratio;
-  int done = 0;
-  if (aligned16(p, g, mom)) {
-    const int n4 = len >> 2;
+  update_chunk(p, g, mom, len, LarsRule{w, s_ratio, rate, momentum, first_step});
+}
+
+// Nesterov SGD (torch.optim.SGD(nesterov=True, dampening=0)) in torch's order with every fp32 operation rounded on its
+// own (nesterov_update, common.cuh); the gradient is zeroed as it is read, for the next backward pass to accumulate on.
+struct NesterovRule {
+  float rate, decay, momentum;
+  __device__ __forceinline__ void vec(float* __restrict__ p, float* __restrict__ g, float* __restrict__ mom,
+                                      int i) const {
     float4* __restrict__ p4 = reinterpret_cast<float4*>(p);
-    const float4* __restrict__ g4 = reinterpret_cast<const float4*>(g);
+    float4* __restrict__ g4 = reinterpret_cast<float4*>(g);
     float4* __restrict__ m4 = reinterpret_cast<float4*>(mom);
-    for (int i = threadIdx.x; i < n4; i += blockDim.x) {
-      float4 pv = p4[i];
-      float4 gv = __ldg(g4 + i);
-      if (w > 0.f) { gv.x += w * pv.x; gv.y += w * pv.y; gv.z += w * pv.z; gv.w += w * pv.w; }
-      gv.x *= ratio; gv.y *= ratio; gv.z *= ratio; gv.w *= ratio;
-      float4 b = gv;
-      if (mom != nullptr) {
-        if (!first_step) {
-          const float4 mv = m4[i];
-          b.x = momentum * mv.x + gv.x; b.y = momentum * mv.y + gv.y;
-          b.z = momentum * mv.z + gv.z; b.w = momentum * mv.w + gv.w;
-        }
-        m4[i] = b;
-      }
-      pv.x -= rate * b.x; pv.y -= rate * b.y; pv.z -= rate * b.z; pv.w -= rate * b.w;
-      p4[i] = pv;
-    }
-    done = n4 << 2;
+    float4 pv = p4[i], gv = g4[i], mv = m4[i];
+    nesterov_update(pv.x, mv.x, gv.x, rate, decay, momentum);
+    nesterov_update(pv.y, mv.y, gv.y, rate, decay, momentum);
+    nesterov_update(pv.z, mv.z, gv.z, rate, decay, momentum);
+    nesterov_update(pv.w, mv.w, gv.w, rate, decay, momentum);
+    p4[i] = pv;
+    m4[i] = mv;
+    g4[i] = gv;
   }
-  for (int i = done + threadIdx.x; i < len; i += blockDim.x) {
-    const float pv = p[i];
-    float gv = g[i];
-    if (w > 0.f) gv = gv + w * pv;
-    gv = gv * ratio;
-    float b = gv;
-    if (mom != nullptr) {
-      b = first_step ? gv : momentum * mom[i] + gv;
-      mom[i] = b;
-    }
-    p[i] = pv - rate * b;
+  __device__ __forceinline__ void scalar(float* __restrict__ p, float* __restrict__ g, float* __restrict__ mom,
+                                         int i) const {
+    nesterov_update(p[i], mom[i], g[i], rate, decay, momentum);
   }
+};
+
+__global__ void __launch_bounds__(256)
+sgd_nesterov_kernel(const uint64_t* __restrict__ p_ptrs, const uint64_t* __restrict__ g_ptrs,
+                    const uint64_t* __restrict__ m_ptrs, const int64_t* __restrict__ chunk_start,
+                    const int* __restrict__ chunk_len, const int* __restrict__ chunk_tensor,
+                    const float* __restrict__ wd, const float* __restrict__ lr, float lr_scale, float momentum) {
+  const int j = blockIdx.x;
+  const int t = chunk_tensor[j];
+  float* __restrict__ p = reinterpret_cast<float*>(p_ptrs[t]) + chunk_start[j];
+  float* __restrict__ g = reinterpret_cast<float*>(g_ptrs[t]) + chunk_start[j];
+  float* __restrict__ mom = reinterpret_cast<float*>(m_ptrs[t]) + chunk_start[j];
+  update_chunk(p, g, mom, chunk_len[j], NesterovRule{__fmul_rn(lr[t], lr_scale), wd[t], momentum});
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -410,6 +466,20 @@ extern "C" int byol_lars_sgd_step(const void* p_ptrs, const void* g_ptrs, const 
                                                     tensor_first_chunk, wd, lr, ignore, partial, trust_coef, eps,
                                                     momentum, first_step);
   return check_launch("lars kernels");
+}
+
+// The chunk tables of byol_lars_sgd_step (m_ptrs required); lr = fp32(lr[t] * lr_scale) per tensor.
+extern "C" int byol_sgd_nesterov_step(const void* p_ptrs, const void* g_ptrs, const void* m_ptrs,
+                                      const int64_t* chunk_start, const int* chunk_len, const int* chunk_tensor,
+                                      int num_chunks, const float* wd, const float* lr, float lr_scale, float momentum,
+                                      cudaStream_t stream) {
+  BYOL_CHECK_ARG(p_ptrs && g_ptrs && m_ptrs && chunk_start && chunk_len && chunk_tensor && wd && lr,
+                 "byol_sgd_nesterov_step: null pointer");
+  BYOL_CHECK_ARG(num_chunks > 0, "byol_sgd_nesterov_step: empty");
+  sgd_nesterov_kernel<<<num_chunks, 256, 0, stream>>>((const uint64_t*)p_ptrs, (const uint64_t*)g_ptrs,
+                                                     (const uint64_t*)m_ptrs, chunk_start, chunk_len, chunk_tensor,
+                                                     wd, lr, lr_scale, momentum);
+  return check_launch("sgd_nesterov_kernel");
 }
 
 // logits: fp32 [R, C] with row pitch ld; labels: int64 [label_rows], row r uses labels[r % label_rows].  row_lse / row_loss: R floats, row_rank: R ints,

@@ -394,12 +394,16 @@ class Engine(object):
     RESERVE_FACTOR = 1.3
     MARGIN = 3 << 30
 
-    def memory_model(self, n, h, w):
-        """Bytes of one bf16 training step with n images per view at h x w.  Per block: "stored" / "kept" = what one
+    def memory_model(self, n, h, w, lanes=2, target=True, mlps=True):
+        """Bytes of one bf16 training step with n images per view at h x w, `lanes` online lanes (one view each) that
+        save activations, the target pair's lanes if `target`, the projector and predictor if `mlps`.  The defaults
+        are the BYOL step; the fine-tune step (finetune.py) is one lane without target pair or MLPs.
+        Per block: "stored" / "kept" = what one
         online lane saves for it without / with recompute (the block output and its mask are kept either way),
         "dy" = the backward gradients one view holds until the weight-gradient join, "work" = one view's other backward
         transients of the block (a recomputed block adds stored - kept), "flops" = its recompute.  "first_input" is the first block's input
-        (saved by each online lane), "fixed" the step's other activations (stem, MLPs, input layouts)."""
+        (saved by each online lane), "fixed" the step's other activations (stem, MLPs, input layouts); "lanes" and
+        "target" describe the step to step_need."""
         cs = ops.conv_out_size
 
         def conv(u, hi, wi):
@@ -432,9 +436,9 @@ class Engine(object):
             blocks.append({"stored": stored, "kept": kept, "dy": dy, "flops": f1 + f2 + f3 + fd,
                            "work": dy + 2 * (eo + n * H * W * b.c1.cin)})
             H, W = hl, wl
-        mlp = sum(2 * n * (l1.cin + 2 * l1.cout) for l1, _ in self.mlps)   # x, h, a
-        fixed = 2 * (2 * e0 + first // 2 + mlp) + 2 * (2 * n * h * w * 8)   # 2 lanes: y0, pool index, MLPs; 2 images
-        return {"blocks": blocks, "first_input": first, "fixed": fixed}
+        mlp = sum(2 * n * (l1.cin + 2 * l1.cout) for l1, _ in self.mlps) if mlps else 0   # x, h, a
+        fixed = lanes * (2 * e0 + first // 2 + mlp + 2 * n * h * w * 8)   # per lane: y0, pool index, MLPs, its image
+        return {"blocks": blocks, "first_input": first, "fixed": fixed, "lanes": lanes, "target": target}
 
     @staticmethod
     def lane_bytes(mm, plan):
@@ -442,12 +446,13 @@ class Engine(object):
         return mm["first_input"] + sum(blk["kept" if i in plan else "stored"] for i, blk in enumerate(mm["blocks"]))
 
     def step_need(self, mm, plan):
-        """Device bytes one training step needs under `plan`: the peak of the forward (two online lanes' saved set,
-        the target pair's largest block) and of the backward (the saved set, the gradients of the stored blocks held
-        for the side-stream weight gradients, one block's transients), scaled by RESERVE_FACTOR, plus MARGIN."""
+        """Device bytes one training step needs under `plan`: the peak of the forward (the online lanes' saved set,
+        the target pair's largest block when the step has one) and of the backward (the saved set, the gradients of
+        the stored blocks held for the side-stream weight gradients, one block's transients), scaled by
+        RESERVE_FACTOR, plus MARGIN.  The step's lanes and target pair are those of `mm` (memory_model)."""
         blocks = mm["blocks"]
-        saved = 2 * self.lane_bytes(mm, plan)
-        fwd = saved + 2 * max(blk["stored"] for blk in blocks)
+        saved = mm["lanes"] * self.lane_bytes(mm, plan)
+        fwd = saved + (2 * max(blk["stored"] for blk in blocks) if mm["target"] else 0)
         bwd = saved + sum(blk["dy"] for i, blk in enumerate(blocks) if i not in plan) + \
             max(blk["work"] + (blk["stored"] - blk["kept"] if i in plan else 0) for i, blk in enumerate(blocks))
         return int(self.RESERVE_FACTOR * (max(fwd, bwd) + mm["fixed"])) + self.MARGIN
@@ -466,21 +471,22 @@ class Engine(object):
             plan.append(i)
         return frozenset(plan)
 
-    def recompute_plan(self, n, h, w):
-        """Blocks whose online lanes recompute their activations in the backward pass, for n images per view at h x w:
-        empty when the stored step fits in what the device can give (its free memory plus the allocator's unused
+    def recompute_plan(self, n, h, w, lanes=2, target=True, mlps=True):
+        """Blocks whose online lanes recompute their activations in the backward pass, for n images per view at h x w
+        in a step of `lanes` saving lanes, with or without the target pair and the MLPs (memory_model): empty when
+        the stored step fits in what the device can give (its free memory plus the allocator's unused
         cache, read once per geometry: the GPU may be shared).  Only the bf16 path without BYOL_B200_FUSE3
         recomputes."""
         if self.T or self.fuse3:
             return frozenset()
-        key = (n, h, w, self.world(), self._mem_budget)
+        key = (n, h, w, lanes, target, mlps, self.world(), self._mem_budget)
         plan = self._plans.get(key)
         if plan is None:
             budget = self._mem_budget
             if budget is None:
                 free, _ = torch.cuda.mem_get_info(self.device)
                 budget = free + torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device)
-            plan = self._plans[key] = self.plan_blocks(self.memory_model(n, h, w), budget)
+            plan = self._plans[key] = self.plan_blocks(self.memory_model(n, h, w, lanes, target, mlps), budget)
         return plan
 
     # ------------------------------------------------------------------------------------------
@@ -739,9 +745,12 @@ class Engine(object):
             return res, reps_b
         if rep_bf16_out is None:
             rep_bf16_out = [None] * L
-        if train and any(lane[2] is not None for lane in lanes):
+        saving = sum(lane[2] is not None for lane in lanes)
+        if train and saving:
             img = x8[0][0] if x8[0][0] is not None else x8[0][1]
-            self._recompute_now = self.recompute_plan(img.shape[0], x8[0][2], x8[0][3])
+            # the lanes that save nothing are the target pair
+            self._recompute_now = self.recompute_plan(img.shape[0], x8[0][2], x8[0][3], saving, L > saving,
+                                                      not reps_only)
         # under SyncBatchNorm over NCCL the per-layer all-reduces serialise the lane pairs anyway: run all four lanes
         # lock-step on one stream there, which halves the number of (latency-bound) NCCL calls.  The peer-memory
         # exchange (comm.PeerExchange) has one channel per stream, so the two-stream schedule stays.
@@ -1414,6 +1423,12 @@ class Engine(object):
         for i, s in enumerate(saved):
             n, h, w, c = s["final_shape"]
             du = d_reps[i].contiguous() if d_reps[i] is not None else None
+            if du is not None and du.dtype == BF16:
+                # the fine-tune step's bf16 classifier dgrad (finetune.py) takes the kernel's bf16 input: the kernel adds
+                # either input to 0.f, so the result has the bits of du.float() passed as the fp32 input
+                assert rep_g is None
+                gs.append(ops.avgpool_bwd(du, None, n, h, w, c))
+                continue
             gs.append(ops.avgpool_bwd(None if rep_g is None else rep_g[i], du, n, h, w, c))
         for bi in range(len(self.blocks) - 1, -1, -1):
             gs = self._block_bwd(self.blocks[bi], [s["blocks"][bi] for s in saved], gs)

@@ -15,6 +15,23 @@ __all__ = ['LARS']
 _CHUNK = 32768
 
 
+def chunk_table(lengths, dev):
+    """The work items of the multi-tensor kernels (byol_lars_sgd_step, byol_sgd_nesterov_step) over tensors of the
+    given lengths: chunk j covers elements [chunk_start[j], chunk_start[j] + chunk_len[j]) of tensor chunk_tensor[j],
+    chunks of at most 32 768 elements; tensor t's chunks are [tensor_first_chunk[t], tensor_first_chunk[t + 1])."""
+    cs, cl, ct, first = [], [], [], []
+    for t, n in enumerate(lengths):
+        first.append(len(cs))
+        for s in range(0, n, _CHUNK):
+            cs.append(s)
+            cl.append(min(_CHUNK, n - s))
+            ct.append(t)
+    first.append(len(cs))
+    i32 = lambda v: torch.tensor(v, dtype=torch.int32, device=dev)
+    return {"chunk_start": torch.tensor(cs, dtype=torch.int64, device=dev), "chunk_len": i32(cl),
+            "chunk_tensor": i32(ct), "tensor_first_chunk": i32(first)}
+
+
 class LARS(Optimizer):
     """Wraps a ``torch.optim.SGD`` (the reference wraps arbitrary optimizers; its configurations only ever use
     SGD / SGD-momentum, main.py:316,332-340).  Param groups may carry the ``'ignore'`` flag set by
@@ -74,15 +91,10 @@ class LARS(Optimizer):
         total = sum(p.numel() for p, _ in entries)
         use_mom = any(g['momentum'] != 0 for _, g in entries)
         flat_m = torch.zeros(total, dtype=torch.float32, device=dev) if use_mom else None
-        cs, cl, ct, first, m_ptrs = [], [], [], [], []
+        m_ptrs = []
         off = 0
-        for t, (p, g) in enumerate(entries):
+        for p, g in entries:
             n = p.numel()
-            first.append(len(cs))
-            for s in range(0, n, _CHUNK):
-                cs.append(s)
-                cl.append(min(_CHUNK, n - s))
-                ct.append(t)
             if use_mom:
                 view = flat_m[off:off + n].view(p.shape)
                 st = self.optim.state[p]
@@ -92,18 +104,17 @@ class LARS(Optimizer):
                 st['momentum_buffer'] = view
                 m_ptrs.append(view.data_ptr())
             off += n
-        first.append(len(cs))
         i64 = lambda v: torch.tensor(v, dtype=torch.int64, device=dev)
-        i32 = lambda v: torch.tensor(v, dtype=torch.int32, device=dev)
         T = len(entries)
-        return {
+        table = chunk_table([p.numel() for p, _ in entries], dev)
+        table.update({
             "p_ptrs": i64([p.data_ptr() for p, _ in entries]), "g_ptrs": i64([p.grad.data_ptr() for p, _ in entries]),
-            "m_ptrs": i64(m_ptrs) if use_mom else None, "chunk_start": i64(cs), "chunk_len": i32(cl),
-            "chunk_tensor": i32(ct), "tensor_first_chunk": i32(first), "wd": torch.zeros(T, device=dev),
-            "lr": torch.zeros(T, device=dev), "ignore": i32([0] * T),
-            "partial": torch.zeros(2 * len(cs), dtype=torch.float64, device=dev),
+            "m_ptrs": i64(m_ptrs) if use_mom else None, "wd": torch.zeros(T, device=dev),
+            "lr": torch.zeros(T, device=dev), "ignore": torch.zeros(T, dtype=torch.int32, device=dev),
+            "partial": torch.zeros(2 * table["chunk_start"].numel(), dtype=torch.float64, device=dev),
             "flat_m": flat_m, "hyper": None, "ptrs": None,
-        }
+        })
+        return table
 
     def step(self, closure=None):
         loss = None

@@ -532,6 +532,15 @@ def lars_sgd_step(table, trust_coef, eps, momentum, first_step):
           "byol_lars_sgd_step", kernels=2)
 
 
+def sgd_nesterov_step(table, lr_scale, momentum):
+    """One Nesterov-SGD step over the tensors of `table` (lars.chunk_table plus int64 pointer tables p_ptrs / g_ptrs /
+    m_ptrs and fp32 [tensors] wd / lr); tensor t's learning rate is fp32(lr[t] * lr_scale).  Zeroes the gradients."""
+    check(lib.byol_sgd_nesterov_step(_ptr(table["p_ptrs"]), _ptr(table["g_ptrs"]), _ptr(table["m_ptrs"]),
+                                     _ptr(table["chunk_start"]), _ptr(table["chunk_len"]), _ptr(table["chunk_tensor"]),
+                                     table["chunk_start"].numel(), _ptr(table["wd"]), _ptr(table["lr"]),
+                                     float(lr_scale), float(momentum), _stream()), "byol_sgd_nesterov_step")
+
+
 def ce_topk_fwd(logits, labels, scratch=None):
     """Softmax cross-entropy (mean) + top-1 / top-5 accuracy (%) of fp32 logits [R, C] in one launch; `labels` has R
     entries or a divisor of R (row r uses labels[r % len]: both views of a sample share its label).

@@ -176,6 +176,15 @@ int byol_lars_sgd_step(const void* p_ptrs, const void* g_ptrs, const void* m_ptr
                        const float* wd, const float* lr, const int* ignore, int num_tensors, double* partial,
                        float trust_coef, float eps, float momentum, int first_step, byol_stream_t stream);
 
+/* One Nesterov-SGD step over the chunk tables of byol_lars_sgd_step (fine-tuning, byol_b200/finetune.py), in
+ * torch.optim.SGD(nesterov=True)'s order with each fp32 operation rounded on its own: g = dW + wd*w;
+ * buf = momentum*buf + g; d = g + momentum*buf; w = w - lr*d, with lr = fp32(lr[t] * lr_scale) and wd[t] per tensor
+ * (fp32 device arrays).  m_ptrs is required; the gradients are zeroed.  Any range length and alignment (float4 accesses
+ * where p / g / momentum share a 16-byte phase). */
+int byol_sgd_nesterov_step(const void* p_ptrs, const void* g_ptrs, const void* m_ptrs, const int64_t* chunk_start,
+                           const int* chunk_len, const int* chunk_tensor, int num_chunks, const float* wd,
+                           const float* lr, float lr_scale, float momentum, byol_stream_t stream);
+
 /* ---- linear-probe objective: replaces F.cross_entropy + helpers.metrics.topk, main.py:596-598 ----
  * logits fp32 [R, C] (row pitch ld), labels int64 [label_rows] (row r uses labels[r % label_rows]: the two views
  * of a sample share its label, main.py:591); scratch: row_lse / row_loss [R] floats, row_rank [R] ints,
