@@ -219,10 +219,12 @@ __global__ void maxpool_fwd_kernel(const bf16* __restrict__ x, bf16* __restrict_
     const int ow = (int)(t % Wo); t /= Wo;
     const int oh = (int)(t % Ho);
     const int n = (int)(t / Ho);
+    // a window whose in-image values are all -inf reports its first in-image position (ATen), never a padding one
+    const int first = (p - oh * s > 0 ? p - oh * s : 0) * k + (p - ow * s > 0 ? p - ow * s : 0);
     float best[8];
     int bi[8];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) { best[e] = -INFINITY; bi[e] = 0; }
+    for (int e = 0; e < 8; ++e) { best[e] = -INFINITY; bi[e] = first; }
     for (int kh = 0; kh < k; ++kh) {
       const int ih = oh * s - p + kh;
       if (ih < 0 || ih >= H) continue;

@@ -270,7 +270,7 @@ __global__ void maxpool_f32_kernel(const float* __restrict__ x, float* __restric
     const int oh = (int)(t % Ho);
     const int n = (int)(t / Ho);
     float best = -INFINITY;
-    int bi = 0;
+    int bi = (p - oh * s > 0 ? p - oh * s : 0) * k + (p - ow * s > 0 ? p - ow * s : 0);   // all -inf: first in-image
     for (int kh = 0; kh < k; ++kh) {
       const int ih = oh * s - p + kh;
       if (ih < 0 || ih >= H) continue;

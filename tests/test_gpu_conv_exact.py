@@ -18,7 +18,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests.util import report_mismatch
+from tests.util import gen as _gen, ints as _ints, pack_bits as _pack, pow2 as _pow2, report_mismatch, \
+    unpack_bits as _unpack
 
 pytestmark = pytest.mark.gpu
 BF = torch.bfloat16
@@ -28,37 +29,10 @@ F64 = torch.float64
 # ------------------------------------------------------------------------------------------------------------------
 # operands and comparison
 # ------------------------------------------------------------------------------------------------------------------
-def _gen(dev, seed):
-    return torch.Generator(device=dev).manual_seed(seed)
-
-
-def _ints(shape, dev, g, amp, density=1.0):
-    """fp64 integers in [-amp, amp], a fraction `density` of them non-zero (exactly representable in bf16)."""
-    v = torch.randint(-amp, amp + 1, shape, generator=g, device=dev).to(F64)
-    if density < 1.0:
-        v = v * (torch.rand(shape, generator=g, device=dev) < density)
-    return v
-
-
-def _pow2(n, dev, g):
-    return torch.pow(2.0, torch.randint(-1, 2, (n,), generator=g, device=dev).to(F64))
-
-
 def _density(k, stats):
     """Density of both GEMM operands for a reduction length k: about 8 (with statistics: 4) non-zero products per
     output, so outputs stay small and the statistics' fp32 partial sums of squares stay exact."""
     return min(1.0, ((4.0 if stats else 8.0) / k) ** 0.5)
-
-
-def _pack(keep):
-    """bool [..., C] -> uint8 bits, element i of the flat index space in bit i % 8 of byte i // 8 (bn_apply's mask)."""
-    k = keep.reshape(-1, 8).to(torch.int32) * (2 ** torch.arange(8, dtype=torch.int32, device=keep.device))
-    return k.sum(1).to(torch.uint8)
-
-
-def _unpack(bits, shape):
-    b = bits.to(torch.int32).unsqueeze(1) >> torch.arange(8, device=bits.device, dtype=torch.int32)
-    return (b & 1).bool().reshape(shape)
 
 
 def _colstats(y2d):

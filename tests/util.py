@@ -2,6 +2,38 @@
 import torch
 
 
+# exact operands for the bit-for-bit kernel tests (test_gpu_conv_exact, test_gpu_elementwise_exact)
+def gen(dev, seed):
+    return torch.Generator(device=dev).manual_seed(seed)
+
+
+def ints(shape, dev, g, amp, density=1.0):
+    """fp64 integers in [-amp, amp], a fraction `density` of them non-zero (exactly representable in bf16)."""
+    v = torch.randint(-amp, amp + 1, shape, generator=g, device=dev).to(torch.float64)
+    if density < 1.0:
+        v = v * (torch.rand(shape, generator=g, device=dev) < density)
+    return v
+
+
+def pow2(n, dev, g, signed=False):
+    """fp64 [n] powers of two in {1/2, 1, 2} (signed: either sign)."""
+    v = torch.pow(2.0, torch.randint(-1, 2, (n,), generator=g, device=dev).to(torch.float64))
+    if signed:
+        v = v * (torch.randint(0, 2, (n,), generator=g, device=dev) * 2 - 1)
+    return v
+
+
+def pack_bits(keep):
+    """bool [..., C] -> uint8 bits, element i of the flat index space in bit i % 8 of byte i // 8 (bn_apply's mask)."""
+    k = keep.reshape(-1, 8).to(torch.int32) * (2 ** torch.arange(8, dtype=torch.int32, device=keep.device))
+    return k.sum(1).to(torch.uint8)
+
+
+def unpack_bits(bits, shape):
+    b = bits.to(torch.int32).unsqueeze(1) >> torch.arange(8, device=bits.device, dtype=torch.int32)
+    return (b & 1).bool().reshape(shape)
+
+
 def report_mismatch(name, got, ref, atol, rtol):
     """Return (ok, message) with enough structure to diagnose layout / swizzle / descriptor bugs remotely."""
     got = got.detach().float().cpu()
