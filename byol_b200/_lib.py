@@ -24,11 +24,6 @@ _SIGNATURES = {
                         c_int, c_int, c_int, c_int, c_int, c_int, c_int,                      # Nimg Hs Ws C Ho Wo Ndim
                         c_int, c_int, c_int, c_int, c_int, c_int, c_int,                      # KH KW stride pad mode ldw ldc
                         c_int, c_int, c_int, c_void_p],                                        # out_fp32 relu force_gather stream
-    "byol_conv_igemm_fused": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                              c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
-    "byol_bn_bwd_prep": [c_void_p, c_void_p, c_void_p, c_int, c_void_p],
-    "byol_bn_bwd_coeffs": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_void_p, c_void_p, c_void_p,
-                           c_int, c_void_p],
     "byol_stem4_supported": [c_int, c_int, c_int, c_int, c_int, c_int, c_int],
     "byol_stem4_row_pixels": [],
     "byol_nchw_to_stem4": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],

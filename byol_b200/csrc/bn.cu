@@ -488,36 +488,6 @@ __global__ void bn_bwd_apply_kernel(const bf16* __restrict__ g, const bf16* __re
   }
 }
 
-// Per-channel vectors for the BatchNorm backward of a RECOMPUTED 1x1 convolution (byol_conv_igemm_fused):
-//   prep  : out[0:C] = invstd, out[C:2C] = -mean*invstd            (xhat = y*out0 + out1 in the reduce epilogue)
-//   coeffs: dy = A*dz + B*y + Cc with A = gamma*invstd, B = -gamma*invstd^2*s2/n, Cc = gamma*invstd*(mean*invstd*s2/n - s1/n)
-//           out[0:C] = B (column scale of the recomputed y), out[C:2C] = Cc (bias), out[2C:3C] = A (scale of dz);
-//           dgamma += s2_local, dbeta += s1_local (rank-local sums, SyncBatchNorm.backward)
-__global__ void bn_bwd_prep_kernel(const float* __restrict__ mean, const float* __restrict__ invstd,
-                                   float* __restrict__ out, int C) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  out[c] = invstd[c];
-  out[C + c] = -mean[c] * invstd[c];
-}
-
-__global__ void bn_bwd_coeffs_kernel(const float* __restrict__ s12, const float* __restrict__ s12_local,
-                                     const float* __restrict__ mean, const float* __restrict__ invstd,
-                                     const float* __restrict__ gamma, float inv_count, float* __restrict__ out,
-                                     float* __restrict__ dgamma, float* __restrict__ dbeta, int C) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  const float is = invstd[c], mu = mean[c], ga = gamma[c];
-  const float m1 = s12[c] * inv_count, m2 = s12[C + c] * inv_count;
-  out[c] = -ga * is * is * m2;
-  out[C + c] = ga * is * (mu * is * m2 - m1);
-  out[2 * C + c] = ga * is;
-  if (dgamma != nullptr) {
-    atomicAdd(dgamma + c, s12_local[C + c]);
-    atomicAdd(dbeta + c, s12_local[c]);
-  }
-}
-
 // column sum of a bf16 or fp32 [M, C] matrix (bias gradients): out[c] += sum_r x[r, c]
 template <typename T>
 __global__ void col_sum_kernel(const T* __restrict__ x, Fix128* __restrict__ out, int M, int C, int ld,
@@ -705,21 +675,4 @@ extern "C" int byol_col_sum(const void* x, float* out, int M, int C, int ld, int
     col_sum_kernel<bf16><<<grid, 128, 0, stream>>>((const bf16*)x, fx, M, C, ld, rows_per_block);
   if (check_launch("col_sum_kernel") != 0) return -100;
   return fix_done(stream, fix_flush(fx, out, C, stream));
-}
-
-extern "C" int byol_bn_bwd_prep(const float* mean, const float* invstd, float* out, int C, cudaStream_t stream) {
-  BYOL_CHECK_ARG(mean && invstd && out && C > 0, "byol_bn_bwd_prep: bad args");
-  bn_bwd_prep_kernel<<<(C + 127) / 128, 128, 0, stream>>>(mean, invstd, out, C);
-  return check_launch("bn_bwd_prep_kernel");
-}
-
-// s12: global (cross-rank) sums over `count` rows; s12_local (optional, default s12): this rank's sums for dgamma/dbeta
-extern "C" int byol_bn_bwd_coeffs(const float* s12, const float* s12_local, const float* mean, const float* invstd,
-                                  const float* gamma, double count, float* out, float* dgamma, float* dbeta, int C,
-                                  cudaStream_t stream) {
-  BYOL_CHECK_ARG(s12 && mean && invstd && gamma && out && C > 0 && count > 0, "byol_bn_bwd_coeffs: bad args");
-  if (s12_local == nullptr) s12_local = s12;
-  bn_bwd_coeffs_kernel<<<(C + 127) / 128, 128, 0, stream>>>(s12, s12_local, mean, invstd, gamma, (float)(1.0 / count),
-                                                           out, dgamma, dbeta, C);
-  return check_launch("bn_bwd_coeffs_kernel");
 }

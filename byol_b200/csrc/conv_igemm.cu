@@ -964,12 +964,10 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-// gemm_fused.cu: plain GEMM with TMA-staged residual tile / per-column vectors in the epilogue
+// gemm_fused.cu: plain GEMM with a TMA-staged (masked) residual tile added in the epilogue
 bool gemm_fused_applicable(int M, int C, int Ndim, int ldw, int ldc);
 int gemm_fused_launch(const void* src, const void* wt, void* dst, const void* resid, const void* resid_mask,
-                      const float* colscale, const float* bias, const float* resid_colscale, void* mask_out,
-                      float* col_sum, float* col_sqsum, int M, int C, int Ndim, int ldw, int ldc, int relu, int no_store,
-                      int bwd_reduce, cudaStream_t stream);
+                      const float* bias, int M, int C, int Ndim, int ldw, int ldc, int relu, cudaStream_t stream);
 
 // conv_patch.cu
 bool patch_conv_applicable(int H, int W, int C, int Ndim, int KH, int KW, int stride, int pad, int out_fp32,
@@ -1040,8 +1038,7 @@ static int conv_igemm_impl(const void* src, const void* wt, void* dst, const voi
   if (!force_gather && resid_f32 == nullptr && resid != nullptr && !resid_up && KH == 1 && KW == 1 && stride == 1 &&
       pad == 0 && !out_fp32 &&
       col_sum == nullptr && gemm_fused_applicable((int)M64, C, Ndim, ldw, ldc))
-    return gemm_fused_launch(src, wt, dst, resid, resid_mask, nullptr, bias, nullptr, nullptr, nullptr, nullptr,
-                             (int)M64, C, Ndim, ldw, ldc, relu, 0, 0, stream);
+    return gemm_fused_launch(src, wt, dst, resid, resid_mask, bias, (int)M64, C, Ndim, ldw, ldc, relu, stream);
   if (!force_gather && resid_f32 == nullptr && resid_mask == nullptr && !resid_up && Hs == Ho && Ws == Wo &&
       ldw >= 9 * (grouped ? BK : C) &&
       patch_conv_applicable(Hs, Ws, C, Ndim, KH, KW, stride, pad, out_fp32, bias, (int64_t)Nimg * Hs * Ws * C))

@@ -186,12 +186,6 @@ class Engine(object):
         # weight layouts of representations(): apart from the training step's, so that a call between a captured
         # forward and its backward leaves every buffer the graphs read untouched (allocated on first use)
         self.w_eval = self.s_eval = None
-        # block-output BatchNorm fused into the expanding 1x1 GEMMs (see _fuse3).  OFF by default: the statistics pass
-        # re-runs the GEMM, so the fused form moves more work than the unfused conv + BN-apply kernels
-        # (tools/time_fused.py times both).  It saves 7-14 GB of activations per 512 images; BYOL_B200_FUSE3=1
-        # enables it.
-        self.fuse3 = os.environ.get("BYOL_B200_FUSE3", "0") == "1"
-        self.fuse3_max_planes = int(os.environ.get("BYOL_B200_FUSE3_MAX_PLANES", "128"))
         # projector / predictor forward as one cooperative kernel per lane (csrc/mlp_fused.cu); =0: four launches
         self.fused_mlp = os.environ.get("BYOL_B200_FUSED_MLP", "1") != "0"
         self._mlp_bar = None
@@ -475,9 +469,8 @@ class Engine(object):
         """Blocks whose online lanes recompute their activations in the backward pass, for n images per view at h x w
         in a step of `lanes` saving lanes, with or without the target pair and the MLPs (memory_model): empty when
         the stored step fits in what the device can give (its free memory plus the allocator's unused
-        cache, read once per geometry: the GPU may be shared).  Only the bf16 path without BYOL_B200_FUSE3
-        recomputes."""
-        if self.T or self.fuse3:
+        cache, read once per geometry: the GPU may be shared).  Only the bf16 path recomputes."""
+        if self.T:
             return frozenset()
         key = (n, h, w, lanes, target, mlps, self.world(), self._mem_budget)
         plan = self._plans.get(key)
@@ -496,22 +489,15 @@ class Engine(object):
     def _down_as_gemm(u, h, w):
         return u.k == 1 and u.stride == 2 and u.pad == 0 and h % 2 == 0 and w % 2 == 0
 
-    def _conv_bn(self, u, xs, lanes, train, stem4=None, unit_stride=None, stats_only=False):
-        """raw conv/linear outputs + BN coefficients [scale, shift, mean, invstd] per lane.
-        stats_only (1x1 / stride-1 convolutions): the GEMM runs for its column statistics only (nothing is written;
-        in eval mode nothing runs at all) — pass 1 of the fused block-output BatchNorm, see _block_fwd."""
+    def _conv_bn(self, u, xs, lanes, train, stem4=None, unit_stride=None):
+        """raw conv/linear outputs + BN coefficients [scale, shift, mean, invstd] per lane."""
         L, C = len(lanes), u.cout
         stats = self._zpool.take(L * 2 * C) if train else None
         ys = []
-        rows = xs[0].numel() // xs[0].shape[-1] if stats_only else None
         for i, (flat, wset, _) in enumerate(lanes):
             st = stats[i * 2 * C:(i + 1) * 2 * C] if train else None
             bias = flat[u.b_off:u.b_off + C] if u.b_off >= 0 else None
             x = xs[i]
-            if stats_only:
-                if train:
-                    ops.gemm_fused(x.view(-1, x.shape[-1]), wset.wf[u.idx], stats=st, no_store=True)
-                continue
             if stem4 is not None:
                 y = ops.stem_conv_fprop(stem4[0][i], wset.w_stem4, stem4[1][i][0], stem4[1][i][1], stats=st)
             elif u.kind == "linear":
@@ -522,8 +508,7 @@ class Engine(object):
         coeffs = self._cpool.take(L * 4 * C).view(L, 4, C)
         bn = u.bn
         if train:
-            if rows is None:
-                rows = ys[0].numel() // C
+            rows = ys[0].numel() // C
             count = rows
             if self.sync and self.world() > 1:
                 comm.allreduce_sum_(stats, channel=self._group_order)
@@ -558,59 +543,7 @@ class Engine(object):
                      mask_out=mask)
         return out
 
-    def _fuse3(self, b, x):
-        """Bottleneck blocks whose expanding 1x1 convolution (conv3: planes -> 4 x planes) and 1x1 downsample branch
-        are plain GEMMs: their BatchNorm + residual + ReLU runs in the GEMM epilogue ("statistics pass + recompute"),
-        so the 4 x planes wide raw outputs y3 / yd are never written or re-read.  The second GEMM pass costs tensor
-        time, so the trade pays where the block is HBM-bound: planes <= fuse3_max_planes (stages 1-2 of ResNet-50)."""
-        if not self.fuse3 or b.kind != "bottleneck" or b.c3.k != 1 or b.c3.stride != 1 or b.c3.pad != 0:
-            return False
-        if b.c3.cin > self.fuse3_max_planes:
-            return False
-        if b.down is not None:
-            d = b.down
-            if d.k != 1 or d.pad != 0 or not (d.stride == 1 or self._down_as_gemm(d, x.shape[1], x.shape[2])):
-                return False
-        return True
-
-    def _block_fwd_fused3(self, b, xs, lanes, train):
-        L = len(lanes)
-        y1, c1 = self._conv_bn(b.c1, xs, lanes, train)
-        a1 = [self._apply(y1[i], c1[i], True) for i in range(L)]
-        y2, c2 = self._conv_bn(b.c2, a1, lanes, train)
-        a2 = [self._apply(y2[i], c2[i], True) for i in range(L)]
-        C3 = b.c3.cout
-        _, c3 = self._conv_bn(b.c3, a2, lanes, train, stats_only=True)
-        n, h, w, _ = a2[0].shape
-        masks = [torch.empty(n * h * w * C3 // 8, dtype=torch.uint8, device=self.device)
-                 if lanes[i][2] is not None else None for i in range(L)]
-        xsub, cd = None, None
-        if b.down is not None:
-            d = b.down
-            xsub = [ops.subsample2(x) for x in xs] if d.stride == 2 else None
-            xin = xsub if xsub is not None else xs
-            _, cd = self._conv_bn(d, xin, lanes, train, stats_only=True)
-            # the normalised residual branch bn_d(conv_d(x)) straight from the GEMM epilogue
-            resid = [ops.gemm_fused(xin[i].view(-1, d.cin), lanes[i][1].wf[d.idx], colscale=cd[i][0], bias=cd[i][1])
-                     for i in range(L)]
-        else:
-            resid = [x.view(-1, C3) for x in xs]
-        outs = []
-        for i in range(L):
-            o = ops.gemm_fused(a2[i].view(-1, b.c3.cin), lanes[i][1].wf[b.c3.idx], colscale=c3[i][0], bias=c3[i][1],
-                               resid=resid[i], relu=True, mask_out=masks[i])
-            outs.append(o.view(n, h, w, C3))
-        for i, (_, _, saved) in enumerate(lanes):
-            if saved is not None:
-                saved["blocks"].append({
-                    "fused3": True, "mask": masks[i], "xsub": xsub[i] if xsub is not None else None,
-                    "x": xs[i], "y1": y1[i], "c1": c1[i], "a1": a1[i], "y2": y2[i], "c2": c2[i], "a2": a2[i],
-                    "y3": None, "c3": c3[i], "yd": None, "cd": cd[i] if cd is not None else None, "out": outs[i]})
-        return outs
-
     def _block_fwd(self, b, xs, lanes, train):
-        if self._fuse3(b, xs[0]):
-            return self._block_fwd_fused3(b, xs, lanes, train)
         L = len(lanes)
         y1, c1 = self._conv_bn(b.c1, xs, lanes, train)
         a1 = [self._apply(y1[i], c1[i], True) for i in range(L)]
@@ -1076,65 +1009,6 @@ class Engine(object):
                                        resid_up=resid_up))
         return outs
 
-    def _bn_bwd_recompute(self, u, gs, xs2d, cs, masks):
-        """BatchNorm backward of a block-output BN whose input y = x2d @ W^T was never stored (_block_fwd_fused3):
-        both passes recompute y on the tensor cores — (1) sum dz, sum dz*xhat in the GEMM epilogue, (2) after the
-        cross-rank exchange, dy = A*dz + B*y + Cc written straight from the epilogue.  dz = gs masked by the ReLU bits."""
-        L, C = len(gs), u.cout
-        wf = self.w_online.wf[u.idx]
-        s12 = self._bpool.take(L * 2 * C)
-        for i in range(L):
-            prep = ops.bn_bwd_prep(cs[i][2], cs[i][3])
-            ops.gemm_fused(xs2d[i], wf, colscale=prep[:C], bias=prep[C:], resid=gs[i].view(-1, C), resid_mask=masks[i],
-                           stats=s12[i * 2 * C:(i + 1) * 2 * C], bwd_reduce=True)
-        rows = xs2d[0].shape[0]
-        count, local = rows, None
-        if self.sync and self.world() > 1:
-            local = torch.empty_like(s12)
-            comm.allreduce_sum_(s12, local_out=local, channel=self._bwd_channel)
-            count = rows * self.world()
-        gamma = self.theta[u.g_off:u.g_off + C]
-        dys = []
-        for i in range(L):
-            sl = slice(i * 2 * C, (i + 1) * 2 * C)
-            abc = ops.bn_bwd_coeffs(s12[sl], cs[i], gamma, count, s12_local=None if local is None else local[sl],
-                                    dgamma=self._gview(u.g_off, C), dbeta=self._gview(u.beta_off, C))
-            dy = ops.gemm_fused(xs2d[i], wf, colscale=abc[:C], bias=abc[C:2 * C], resid=gs[i].view(-1, C),
-                                resid_mask=masks[i], resid_colscale=abc[2 * C:])
-            dys.append(dy.view(gs[i].shape))
-        return dys
-
-    def _block_bwd_fused3(self, b, S, gs):
-        L = len(gs)
-        xs = [s["x"] for s in S]
-        xshapes = [tuple(x.shape) for x in xs]
-        masks = [s["mask"] for s in S]
-        a2 = [s["a2"] for s in S]
-        dy3 = self._bn_bwd_recompute(b.c3, gs, [a.view(-1, b.c3.cin) for a in a2], [s["c3"] for s in S], masks)
-        resid_masks, resid_up = None, False
-        if b.down is not None:
-            d = b.down
-            xin = [s["xsub"] if s["xsub"] is not None else s["x"] for s in S]
-            dyd = self._bn_bwd_recompute(d, gs, [x.view(-1, d.cin) for x in xin], [s["cd"] for s in S], masks)
-            self._wgrad(d, xin, dyd, unit_stride=1)
-            if S[0]["xsub"] is not None and b.c1.k == 1 and b.c1.stride == 1:
-                resid = self._dgrad(d, dyd, [tuple(x.shape) for x in xin], unit_stride=1)
-                resid_up = True
-            elif S[0]["xsub"] is not None:
-                raise RuntimeError("fused downsample branch needs a 1x1 / stride-1 conv1")   # not a torchvision net
-            else:
-                resid = self._dgrad(d, dyd, xshapes, unit_stride=1)
-        else:
-            resid, resid_masks = gs, masks          # masked residual gradient added by the conv1 dgrad epilogue
-        self._wgrad(b.c3, a2, dy3)
-        g2 = self._dgrad(b.c3, dy3, [tuple(a.shape) for a in a2])
-        dy2, _ = self._bn_bwd(b.c2, g2, [s["y2"] for s in S], [s["c2"] for s in S], 1)
-        self._wgrad(b.c2, [s["a1"] for s in S], dy2)
-        g1 = self._dgrad(b.c2, dy2, [tuple(s["a1"].shape) for s in S])
-        dy1, _ = self._bn_bwd(b.c1, g1, [s["y1"] for s in S], [s["c1"] for s in S], 1)
-        self._wgrad(b.c1, xs, dy1)
-        return self._dgrad(b.c1, dy1, xshapes, resids=resid, resid_masks=resid_masks, resid_up=resid_up)
-
     def _rebuild(self, b, s):
         """The saved dict of a block the forward recomputes: y1, a1, y2, a2, y3, xsub, yd again from its input and the
         forward's scale / shift, by the forward's kernels with the forward's arguments, on the current stream.  No
@@ -1157,8 +1031,6 @@ class Engine(object):
         return r
 
     def _block_bwd(self, b, S, gs):
-        if S[0].get("fused3"):
-            return self._block_bwd_fused3(b, S, gs)
         if S[0].get("recompute"):
             out = self._block_bwd(b, [self._rebuild(b, s) for s in S], gs)
             # the weight gradients read the rebuilt tensors on the side stream: join, so that they are freed here
@@ -1447,7 +1319,7 @@ class Engine(object):
     # ------------------------------------------------------------------------------------------
     def graph_key(self, a1):
         return (tuple(a1.shape), self.world(), bool(self.sync), self.theta.data_ptr(), self.multi_stream,
-                self.overlap_wgrad, self.T, self.bwd32, self.fuse3, self.fuse3_max_planes, self.fused_mlp,
+                self.overlap_wgrad, self.T, self.bwd32, self.fused_mlp,
                 self.recompute_plan(a1.shape[0], a1.shape[2], a1.shape[3]))
 
     def prep_step(self, mean, training):

@@ -101,11 +101,6 @@ def holdout_indices(n, labelled, seed):
     return np.sort(np.random.default_rng([int(seed), 0x686f6c]).permutation(rest)[:k])
 
 
-def _check_fuse3():
-    if os.environ.get("BYOL_B200_FUSE3", "0") == "1":
-        raise ValueError("fine-tuning does not support BYOL_B200_FUSE3=1 (the fused block-output BatchNorm)")
-
-
 def _check_network(network):
     if network not in ("online", "target"):
         raise ValueError("network must be 'online' or 'target', got %r" % (network,))
@@ -134,7 +129,6 @@ class FineTune(object):
         if not isinstance(num_classes, int) or isinstance(num_classes, bool) or num_classes < 2:
             raise ValueError("num_classes must be an int >= 2, got %r" % (num_classes,))
         _check_network(network)
-        _check_fuse3()
         dev = _model_device(model)
         d = int(model.base_network_output_size)
         if d < 1 or d % 64 != 0:
@@ -297,7 +291,6 @@ def finetune_accuracy(model, loader, label_fraction=None, subset=None, epochs=30
     _positive_int(epochs, "epochs")
     _positive_int(batch_size, "batch_size")
     _check_network(network)
-    _check_fuse3()
     d = int(model.base_network_output_size)
     if d < 1 or d % 64 != 0:
         raise ValueError("the feature width D=%d must be a positive multiple of 64" % d)

@@ -221,8 +221,6 @@ class BYOL(nn.Module):
         if backward_precision == "fp32" and precision != "fp32":
             raise ValueError("backward_precision='fp32' needs precision='fp32' (an fp32 backward needs the fp32 "
                              "activations of the fp32-accurate forward), got precision=%r" % (precision,))
-        if backward_precision == "fp32" and self._engine.fuse3:
-            raise ValueError("backward_precision='fp32' does not support BYOL_B200_FUSE3=1")
         check_grouped_convs(self, precision)
         self.precision = precision
         self.backward_precision = backward_precision

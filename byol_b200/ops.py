@@ -272,26 +272,6 @@ def conv_wgrad(x, dy, dw, kh, kw, stride, pad, force_gather=False):
     return dw
 
 
-def gemm_fused(x2d, w_f, out=None, colscale=None, bias=None, resid=None, resid_mask=None, resid_colscale=None,
-               relu=False, mask_out=None, stats=None, no_store=False, bwd_reduce=False):
-    """1x1 / stride-1 convolution as a plain GEMM y[M, N] = x2d[M, K] @ w_f[N, K]^T with the fused BatchNorm epilogue
-    of byol_conv_igemm_fused: t = y*colscale + bias; out = act(t + resid_colscale * masked(resid)).
-    no_store: only `stats` (zeroed fp32 [2N]: column sum | sum of squares of bf16(y)) is produced.
-    bwd_reduce: only `stats` is produced: [sum dz | sum dz*t] with dz = masked(resid)."""
-    _chk(x2d, BF16, "x"); _chk(w_f, BF16, "w_f"); _chk(resid, BF16, "resid"); _chk(resid_mask, torch.uint8, "mask")
-    _chk(stats, F32, "stats"); _chk(mask_out, torch.uint8, "mask_out")
-    m, k = x2d.shape
-    n, ldw = w_f.shape
-    if out is None and not (no_store or bwd_reduce):
-        out = torch.empty((m, n), dtype=BF16, device=x2d.device)
-    cs = _ptr(stats)
-    cq = (stats.data_ptr() + 4 * n) if stats is not None else 0
-    check(lib.byol_conv_igemm_fused(_ptr(x2d), _ptr(w_f), _ptr(out), _ptr(resid), _ptr(resid_mask), _ptr(colscale),
-                                    _ptr(bias), _ptr(resid_colscale), _ptr(mask_out), cs, cq, m, k, n, ldw, n,
-                                    int(relu), int(no_store), int(bwd_reduce), _stream()), "byol_conv_igemm_fused")
-    return out
-
-
 def mlp_fused_supported(b, k1, h, o):
     return bool(lib.byol_mlp_fused_supported(b, k1, h, o))
 
@@ -318,25 +298,6 @@ def mlp_fused_fwd(x2d, w1, b1, gamma, beta, w2, b2, stats, running_mean, running
                                  _ptr(coeffs), _ptr(out), _ptr(hs), _ptr(as_), _ptr(grid_bar), b, k1, h, o, ldw1, ldw2,
                                  int(train), pp, world, rank, cap, ctr, _stream()), "byol_mlp_fused_fwd")
     return out, hs, as_
-
-
-def bn_bwd_prep(mean, invstd, out=None):
-    c = mean.numel()
-    if out is None:
-        out = torch.empty(2 * c, dtype=F32, device=mean.device)
-    check(lib.byol_bn_bwd_prep(_ptr(mean), _ptr(invstd), _ptr(out), c, _stream()), "byol_bn_bwd_prep")
-    return out
-
-
-def bn_bwd_coeffs(s12, coeffs, gamma, count, s12_local=None, dgamma=None, dbeta=None, out=None):
-    """[B | Cc | A] per channel so that dy = A*dz + B*y + Cc (see csrc/bn.cu); accumulates dgamma / dbeta."""
-    c = gamma.numel()
-    if out is None:
-        out = torch.empty(3 * c, dtype=F32, device=gamma.device)
-    check(lib.byol_bn_bwd_coeffs(_ptr(s12), _ptr(s12_local), _ptr(coeffs[2]), _ptr(coeffs[3]), _ptr(gamma),
-                                 float(count), _ptr(out), _ptr(dgamma), _ptr(dbeta), c, _stream()),
-          "byol_bn_bwd_coeffs")
-    return out
 
 
 def linear_fprop(x2d, w_f, bias=None, stats=None, relu=False, out_fp32=False, out=None):

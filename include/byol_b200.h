@@ -52,17 +52,6 @@ int byol_conv_wgrad(const void* src, const void* dy, float* dw, int Nimg, int Hs
                     int Ho, int Wo, int Cout, int ldy /* row pitch of dy, 0 = Cout */, int KH, int KW, int stride,
                     int pad, int force_gather, byol_stream_t stream);
 
-/* 1x1 / stride-1 convolution (plain GEMM out[M, Ndim] = src[M, C] x wt[Ndim, C]^T) with a fused BatchNorm epilogue:
- *   t = acc * colscale[n] + bias[n];  out = act(t + resid_colscale[n] * (resid_mask ? resid : 0)) -> dst, mask_out.
- * no_store = 1: only col_sum / col_sqsum (BatchNorm statistics) are produced — pass 1 of "statistics pass +
- * recompute": the block-output BatchNorm of a bottleneck (torchvision Bottleneck.bn3 + residual + ReLU, reached from
- * main.py:237) never materialises the raw conv output.  bwd_reduce = 1: the BatchNorm-backward sums of the recomputed
- * output: with dz = (resid_mask ? resid : 0): col_sum += sum dz, col_sqsum += sum dz * t. */
-int byol_conv_igemm_fused(const void* src, const void* wt, void* dst, const void* resid, const void* resid_mask,
-                          const float* colscale, const float* bias, const float* resid_colscale, void* mask_out,
-                          float* col_sum, float* col_sqsum, int M, int C, int Ndim, int ldw, int ldc, int relu,
-                          int no_store, int bwd_reduce, byol_stream_t stream);
-
 /* ---- stem (7x7 / stride 2 / pad 3, <= 4 input channels, 64 output channels, W <= 256): the torchvision ResNet
  *      conv1 reached from main.py:237.  The image is converted once to zero-padded NHWC4 bf16
  *      ([N][H+6][264][4]); the kernel forms the im2col rows with overlapping no-swizzle UMMA descriptors. ---- */
@@ -104,11 +93,6 @@ int byol_bn_bwd_apply(const void* g, const void* x, const void* act, const float
                       const float* mean, const float* invstd, const float* gamma, const float* s12, double count,
                       void* dy, void* dz_out, int M, int C, int mask_mode, const float* s12_local, float* dgamma,
                       float* dbeta, byol_stream_t stream);
-/* per-channel vectors for the BatchNorm backward of a recomputed 1x1 convolution (byol_conv_igemm_fused) */
-int byol_bn_bwd_prep(const float* mean, const float* invstd, float* out /* [2C] */, int C, byol_stream_t stream);
-int byol_bn_bwd_coeffs(const float* s12, const float* s12_local, const float* mean, const float* invstd,
-                       const float* gamma, double count, float* out /* [3C] */, float* dgamma, float* dbeta, int C,
-                       byol_stream_t stream);
 int byol_col_sum(const void* x, float* out, int M, int C, int ld, int is_f32, byol_stream_t stream);
 
 /* ---- layout / pooling: torchvision ResNet stem and tail reached from main.py:237 ---- */

@@ -118,7 +118,7 @@ def test_finetune_accuracy_rejects_bad_arguments(kw, match):
         F.finetune_accuracy(_model(), _loader(20), **dict(dict(batch_size=4), **kw))
 
 
-def test_finetune_accuracy_checks_splits_before_device_work(monkeypatch):
+def test_finetune_accuracy_checks_splits_before_device_work():
     with pytest.raises(ValueError, match="test split is empty"):
         F.finetune_accuracy(_model(), _loader(20, n_test=0), label_fraction=0.5, batch_size=4)
     with pytest.raises(ValueError, match="no image is left"):                 # all labelled, no valid/
@@ -127,9 +127,6 @@ def test_finetune_accuracy_checks_splits_before_device_work(monkeypatch):
         F.finetune_accuracy(_model(100), _loader(20), label_fraction=0.5, batch_size=4)
     with pytest.raises(ValueError, match="2 classes"):
         F.finetune_accuracy(_model(), _loader(20, classes=1), label_fraction=0.5, batch_size=4)
-    monkeypatch.setenv("BYOL_B200_FUSE3", "1")
-    with pytest.raises(ValueError, match="FUSE3"):
-        F.finetune_accuracy(_model(), _loader(20), label_fraction=0.5, batch_size=4)
 
 
 def test_valid_split_allows_a_fully_labelled_training_split():

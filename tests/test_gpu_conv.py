@@ -4,14 +4,11 @@ Inputs are bf16-representable, the oracle runs in fp32 on the same values, so th
 accumulation order (tolerance 2e-3 relative to the output scale, stated per test) and, where the kernel
 stores bf16, one bf16 rounding (2^-8 relative).
 """
-import numpy as np
 import pytest
 import torch
 
 from oracle import ops_ref as R
 from tests.util import assert_close
-
-BF = torch.bfloat16
 
 pytestmark = pytest.mark.gpu
 
@@ -270,63 +267,3 @@ def test_linear(cuda, case):
     torch.cuda.synchronize()
     refdw = dy.t() @ x
     assert_close("linear_wgrad[%s]" % name, dw, refdw, atol=2e-3 * float(refdw.abs().max()), rtol=0)
-
-
-@pytest.mark.parametrize("m,k,n", [(5000, 64, 256), (777, 512, 2048), (4096, 256, 128), (300, 128, 136)])
-def test_gemm_fused_bn_epilogues(cuda, m, k, n):
-    """byol_conv_igemm_fused: the 1x1 convolution whose BatchNorm (+ residual + ReLU) lives in the epilogue
-    (statistics pass / apply pass) and whose BatchNorm backward recomputes the conv output (reduce / apply)."""
-    from byol_b200 import ops
-    g = torch.Generator().manual_seed(m + k + n)
-    x = R.bf16_round(torch.randn(m, k, generator=g))
-    w = R.bf16_round(torch.randn(n, k, generator=g) * 0.1)
-    y = x.double() @ w.double().t()
-    xd, wd = x.to(cuda, BF), w.to(cuda, BF)
-    # (1) statistics only
-    stats = torch.zeros(2 * n, device=cuda)
-    out = ops.gemm_fused(xd, wd, stats=stats, no_store=True)
-    assert out is None
-    yb = R.bf16_round(y.float()).double()
-    assert_close("fused_stats_sum", stats[:n], yb.sum(0).float(), atol=2e-3 * float(yb.abs().sum(0).max()), rtol=1e-3)
-    assert_close("fused_stats_sq", stats[n:], (yb * yb).sum(0).float(), atol=0, rtol=2e-3)
-    # (2) apply: out = relu(y*scale + shift + resid), mask bits
-    scale, shift = torch.rand(n, generator=g) + 0.5, torch.randn(n, generator=g)
-    resid = R.bf16_round(torch.randn(m, n, generator=g))
-    mask = torch.zeros(m * n // 8, dtype=torch.uint8, device=cuda)
-    out = ops.gemm_fused(xd, wd, colscale=scale.to(cuda), bias=shift.to(cuda), resid=resid.to(cuda, BF), relu=True,
-                         mask_out=mask)
-    torch.cuda.synchronize()
-    ref = torch.relu(y * scale.double() + shift.double() + resid.double()).float()
-    assert_close("fused_apply", out, ref, atol=2e-2, rtol=1e-2)
-    bits = np.unpackbits(mask.cpu().numpy(), bitorder="little").reshape(m, n).astype(bool)
-    refpos = ref.numpy() > 0
-    disagree = bits != refpos
-    assert disagree.mean() < 1e-3 and np.all(np.abs(ref.numpy()[disagree]) < 1e-2)   # only at the ReLU boundary
-    # (3) BatchNorm-backward sums of the recomputed output
-    mean, invstd = y.mean(0).float(), (1.0 / torch.sqrt(y.var(0, unbiased=False) + 1e-5)).float()
-    gq = R.bf16_round(torch.randn(m, n, generator=g) * 0.01)
-    mbits = (torch.rand(m, n, generator=g) > 0.4)
-    mpacked = torch.from_numpy(np.packbits(mbits.numpy().reshape(-1), bitorder="little")).to(cuda)
-    prep = ops.bn_bwd_prep(mean.to(cuda), invstd.to(cuda))
-    s12 = torch.zeros(2 * n, device=cuda)
-    ops.gemm_fused(xd, wd, colscale=prep[:n], bias=prep[n:], resid=gq.to(cuda, BF), resid_mask=mpacked, stats=s12,
-                   bwd_reduce=True)
-    torch.cuda.synchronize()
-    dz = gq.double() * mbits.double()
-    xhat = (y - mean.double()) * invstd.double()
-    assert_close("fused_bwd_s1", s12[:n], dz.sum(0).float(), atol=1e-4 * float(dz.abs().sum(0).max()), rtol=1e-3)
-    assert_close("fused_bwd_s2", s12[n:], (dz * xhat).sum(0).float(), atol=2e-3 * float((dz * xhat).abs().sum(0).max()),
-                 rtol=2e-3)
-    # (4) BatchNorm-backward apply: dy = A*dz + B*y + Cc
-    gamma = torch.rand(n, generator=g) + 0.5
-    co = torch.stack([torch.zeros(n), torch.zeros(n), mean, invstd]).to(cuda)
-    s12ref = torch.cat([dz.sum(0), (dz * xhat).sum(0)]).float().to(cuda)
-    dgam, dbet = torch.zeros(n, device=cuda), torch.zeros(n, device=cuda)
-    abc = ops.bn_bwd_coeffs(s12ref, co, gamma.to(cuda), m, dgamma=dgam, dbeta=dbet)
-    dy = ops.gemm_fused(xd, wd, colscale=abc[:n], bias=abc[n:2 * n], resid=gq.to(cuda, BF), resid_mask=mpacked,
-                        resid_colscale=abc[2 * n:])
-    torch.cuda.synchronize()
-    dyref, dgref, dbref = R.bn_bwd_ref(dz, y, mean.double(), invstd.double(), gamma.double())
-    assert_close("fused_bwd_dy", dy, dyref.float(), atol=2e-2 * float(dyref.abs().max()), rtol=2e-2)
-    assert_close("fused_dgamma", dgam, dgref.float(), atol=1e-3 * float(dgref.abs().max()), rtol=1e-3)
-    assert_close("fused_dbeta", dbet, dbref.float(), atol=1e-3 * float(dbref.abs().max()), rtol=1e-3)

@@ -1,11 +1,10 @@
 """GPU: every convolution kernel route and epilogue bit for bit against float64.
 
 * Exact operands.  Activations, gradients and residuals are integers in [-2, 2], weights integers in [-1, 1] (sparse
-  where K is large), biases integers, and colscale / resid_colscale / BatchNorm-backward coefficients powers of two.
-  Every product and every fp32 partial sum is then an exact integer (or a small dyadic fraction) far below 2^24, in any
-  order and on any tile split, so a kernel output must equal the float64 reference rounded once to its dtype
-  (torch.equal): a dropped channel, tap or residual, or a residual added to the wrong pixel, shows.  The references run
-  in float64 on the device with cuDNN off (im2col + GEMM, exact on integers).
+  where K is large) and biases integers.  Every product and every fp32 partial sum is then an exact integer far below
+  2^24, in any order and on any tile split, so a kernel output must equal the float64 reference rounded once to its
+  dtype (torch.equal): a dropped channel, tap or residual, or a residual added to the wrong pixel, shows.  The
+  references run in float64 on the device with cuDNN off (im2col + GEMM, exact on integers).
 * Route table.  One row per (op, route, epilogue) at the edge of its host predicate (conv_igemm_impl and
   conv_wgrad_impl in csrc/conv_igemm.cu); one test checks under torch.profiler that each row launches the kernel it is
   meant for, so a row cannot drift to another route unnoticed.
@@ -18,8 +17,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests.util import gen as _gen, ints as _ints, pack_bits as _pack, pow2 as _pow2, report_mismatch, \
-    unpack_bits as _unpack
+from tests.util import gen as _gen, ints as _ints, pack_bits as _pack, report_mismatch
 
 pytestmark = pytest.mark.gpu
 BF = torch.bfloat16
@@ -274,61 +272,6 @@ def wgrad_case(dev, g, n, h, w, c, cin_real, cout, k, s, p, ldy=None, gather=Fal
     return Case(run, check, wgrad_route(n, h, w, c, cin_real, cout, ldy, k, s, p, gather, grouped))
 
 
-def gemm_case(dev, g, m, k, n, ldw=None, colscale=False, bias=False, resid=False, resid_mask=False,
-              resid_colscale=False, relu=False, mask_out=False, stats=False, no_store=False, bwd_reduce=False):
-    """ops.gemm_fused: t = (x @ w^T) * colscale + bias; out = act(t + resid_colscale * masked(resid)).
-    no_store: stats of bf16(t) only; bwd_reduce: [sum dz | sum dz * t] with dz = masked(resid) only."""
-    from byol_b200 import ops
-    ldw = ldw or k
-    d = _density(k, stats or bwd_reduce)
-    x = _ints((m, k), dev, g, 1 if stats else 2, d)
-    w = _ints((n, ldw), dev, g, 1, d)
-    cs = _pow2(n, dev, g) if colscale else None
-    b = _ints((n,), dev, g, 3) if bias else None
-    r = _ints((m, n), dev, g, 2) if resid else None
-    keep = (torch.rand(m, n, generator=g, device=dev) > 0.4) if resid_mask else None
-    rcs = _pow2(n, dev, g) if resid_colscale else None
-    xd, wd = x.to(BF), w.to(BF)
-    f32 = [t.float() if t is not None else None for t in (cs, b, rcs)]
-    rd, bits = (r.to(BF) if resid else None), (_pack(keep) if resid_mask else None)
-
-    def run():
-        st = torch.zeros(2 * n, device=dev) if (stats or bwd_reduce) else None
-        mo = torch.zeros(m * n // 8, dtype=torch.uint8, device=dev) if mask_out else None
-        out = ops.gemm_fused(xd, wd, colscale=f32[0], bias=f32[1], resid=rd, resid_mask=bits, resid_colscale=f32[2],
-                             relu=relu, mask_out=mo, stats=st, no_store=no_store, bwd_reduce=bwd_reduce)
-        return [out, st, mo]
-
-    def check(outs):
-        out, st, mo = outs
-        t = x @ w[:, :k].t()
-        if cs is not None:
-            t = t * cs
-        if b is not None:
-            t = t + b
-        dz = None
-        if resid:
-            dz = r * keep if resid_mask else r
-        if bwd_reduce:
-            assert out is None
-            _expect("s12", st, torch.cat([dz.sum(0), (dz * t).sum(0)]))
-            return
-        if no_store:
-            assert out is None
-            _expect("stats", st, _colstats(t.float().to(BF)))
-            return
-        ref = t + (dz * rcs if rcs is not None else dz) if resid else t
-        if relu:
-            ref = torch.relu(ref)
-        _expect("out", out, ref)
-        if stats:
-            _expect("stats", st, _colstats(_want(out, ref)))
-        if mask_out:
-            _expect("mask_out", _unpack(mo, (m, n)), ref > 0)
-
-    return Case(run, check, "gemm_fused")
-
-
 def stem_fprop_case(dev, g, n, h, w, stats=False):
     from byol_b200 import ops
     x = _ints((n, 3, h, w), dev, g, 1 if stats else 2, 0.5)
@@ -370,7 +313,7 @@ def stem_wgrad_case(dev, g, n, h, w, cin):
 # ------------------------------------------------------------------------------------------------------------------
 # the route table: one row per (op, route, epilogue), at the edge of its predicate
 # ------------------------------------------------------------------------------------------------------------------
-D, FP, W, G = dgrad_case, fprop_case, wgrad_case, gemm_case
+D, FP, W = dgrad_case, fprop_case, wgrad_case
 ROWS = {
     # dgrad: 1x1 bf16 hand-off (partial column tiles, M = 81)
     "dgrad_h16_n40": ("h16", D, dict(n=1, h=9, w=9, cin=40, cout=64, k=1, s=1, p=0)),
@@ -455,15 +398,6 @@ ROWS = {
                                                   stats=True)),
     "fprop_grouped_s2_stats": ("grouped", FP, dict(n=2, h=14, w=14, c=128, cout=128, k=3, s=2, p=1, cg=4,
                                                    stats=True)),
-    # ops.gemm_fused: the BatchNorm apply pass and the BatchNorm-backward apply dy = A*dz + B*y + C
-    "gemm_apply_tail": ("gemm_fused", G, dict(m=300, k=128, n=136, colscale=True, bias=True, resid=True,
-                                              resid_colscale=True, relu=True, mask_out=True)),
-    "gemm_apply": ("gemm_fused", G, dict(m=5000, k=64, n=256, colscale=True, bias=True, resid=True,
-                                         resid_colscale=True, relu=True, mask_out=True)),
-    "gemm_bn_bwd_apply_tail": ("gemm_fused", G, dict(m=300, k=128, n=136, colscale=True, bias=True, resid=True,
-                                                     resid_mask=True, resid_colscale=True)),
-    "gemm_bn_bwd_apply": ("gemm_fused", G, dict(m=5000, k=64, n=256, colscale=True, bias=True, resid=True,
-                                                resid_mask=True, resid_colscale=True)),
     # wgrad cases test_gpu_reductions does not have
     "wgrad_grouped_patch_cg4": ("wgrad_patch", W, dict(n=2, h=14, w=14, c=128, cin_real=4, cout=128, k=3, s=1, p=1,
                                                        grouped=True)),
@@ -551,27 +485,20 @@ def _recorders(calls):
     def conv_wgrad(x, dy, dw, kh, kw, stride, pad, force_gather=False):
         calls.add(("conv_wgrad", _shape(x), _shape(dy), _shape(dw), kh, kw, stride, pad, bool(force_gather)))
 
-    def gemm_fused(x2d, w_f, out=None, colscale=None, bias=None, resid=None, resid_mask=None, resid_colscale=None,
-                   relu=False, mask_out=None, stats=None, no_store=False, bwd_reduce=False):
-        calls.add(("gemm_fused", _shape(x2d), _shape(w_f), colscale is not None, bias is not None, resid is not None,
-                   resid_mask is not None, resid_colscale is not None, bool(relu), mask_out is not None,
-                   stats is not None, bool(no_store), bool(bwd_reduce)))
-
     def stem_conv_fprop(xs4, w_stem4, h, w, stats=None):
         calls.add(("stem_conv_fprop", xs4.shape[0], h, w, stats is not None))
 
     def stem_conv_wgrad(xs4, dy, dw, h, w):
         calls.add(("stem_conv_wgrad", xs4.shape[0], h, w, dw.shape[1]))
-    return dict(conv_fprop=conv_fprop, conv_dgrad=conv_dgrad, conv_wgrad=conv_wgrad, gemm_fused=gemm_fused,
+    return dict(conv_fprop=conv_fprop, conv_dgrad=conv_dgrad, conv_wgrad=conv_wgrad,
                 stem_conv_fprop=stem_conv_fprop, stem_conv_wgrad=stem_conv_wgrad)
 
 
-def _record_step(monkeypatch, dev, arch, rep, b, r, fuse3):
+def _record_step(monkeypatch, dev, arch, rep, b, r):
     from byol_b200 import ops, wiring
     from byol_b200.model import BYOL
     calls = set()
     with monkeypatch.context() as mp:
-        mp.setenv("BYOL_B200_FUSE3", "1" if fuse3 else "0")
         for name, rec in _recorders(calls).items():
             orig = getattr(ops, name)
 
@@ -618,18 +545,12 @@ def _replay_case(dev, g, sig, cg_by_c):
         n, h, w, c = xs
         grouped = dws[1] < c and c % 64 == 0
         return wgrad_case(dev, g, n, h, w, c, dws[1], dws[0], kh, s, p, ldy=dys[3], gather=gather, grouped=grouped)
-    if op == "gemm_fused":
-        _, xs, ws, cs, bias, resid, mask, rcs, relu, mo, stats, no_store, bwd = sig
-        return gemm_case(dev, g, xs[0], xs[1], ws[0], ldw=ws[1], colscale=cs, bias=bias, resid=resid,
-                         resid_mask=mask, resid_colscale=rcs, relu=relu, mask_out=mo, stats=stats, no_store=no_store,
-                         bwd_reduce=bwd)
     if op == "stem_conv_fprop":
         return stem_fprop_case(dev, g, sig[1], sig[2], sig[3], stats=sig[4])
     return stem_wgrad_case(dev, g, sig[1], sig[2], sig[3], sig[4])
 
 
-NETS = [("resnet18", 512, 8, 224, False), ("resnet:bottleneck:2,1,1,1", 2048, 8, 224, True),
-        ("resnet:bottleneck:2,1,1,1", 2048, 8, 224, False), ("resnext:32x4:1,1,1,1", 2048, 2, 112, False)]
+NETS = [("resnet18", 512, 8, 224), ("resnet:bottleneck:2,1,1,1", 2048, 8, 224), ("resnext:32x4:1,1,1,1", 2048, 2, 112)]
 
 
 def _dgrad_sig_route(sig):
@@ -641,8 +562,8 @@ def _dgrad_sig_route(sig):
 
 def test_replay_engine_calls_exactly(cuda, monkeypatch):
     calls = set()
-    for arch, rep, b, r, fuse3 in NETS:
-        calls |= _record_step(monkeypatch, cuda, arch, rep, b, r, fuse3)
+    for arch, rep, b, r in NETS:
+        calls |= _record_step(monkeypatch, cuda, arch, rep, b, r)
         torch.cuda.empty_cache()
     dgrads = [sig for sig in calls if sig[0] == "conv_dgrad"]
     resid_routes = {_dgrad_sig_route(sig) for sig in dgrads if sig[9] is not None}

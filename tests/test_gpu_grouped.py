@@ -5,8 +5,6 @@ Kernel parity runs on bf16-representable inputs against float64 grouped convolut
 tests/test_gpu_conv.py holds the dense kernels to.  The block and step tests reuse the criteria of
 tests/test_gpu_blocks.py and tests/test_gpu_step.py.
 """
-import os
-
 import numpy as np
 import pytest
 import torch
@@ -189,30 +187,6 @@ def test_resnext_graph_replay_bit_equal_to_eager(cuda):
     a, b = _train(arch, 2048, graphs=False), _train(arch, 2048, graphs=True)
     for key in a:
         assert torch.equal(a[key], b[key]), key
-
-
-def test_resnext_fuse3_step(cuda):
-    """One step with the block-output BatchNorm fused into the 1x1 GEMMs (BYOL_B200_FUSE3=1)."""
-    from byol_b200.model import BYOL
-    from byol_b200 import wiring
-    old = os.environ.get("BYOL_B200_FUSE3")
-    os.environ["BYOL_B200_FUSE3"] = "1"
-    try:
-        torch.manual_seed(5)
-        model = BYOL(2048, 256, 1000, 10, arch="resnext:32x4:2,1,1,1").cuda().train()
-        assert model._engine.fuse3
-        opt = wiring.build_optimizer(model, global_batch_size=256)
-        g = torch.Generator().manual_seed(6)
-        a1, a2 = torch.rand(8, 3, 64, 64, generator=g).cuda(), torch.rand(8, 3, 64, 64, generator=g).cuda()
-        lab = torch.randint(0, 1000, (8,), generator=g).cuda()
-        loss = wiring.train_step(model, opt, a1, a2, lab)["loss_mean"]
-        torch.cuda.synchronize()
-        assert torch.isfinite(loss) and torch.isfinite(model._engine.theta).all()
-    finally:
-        if old is None:
-            os.environ.pop("BYOL_B200_FUSE3")
-        else:
-            os.environ["BYOL_B200_FUSE3"] = old
 
 
 def test_resnext_eval_forward(cuda, monkeypatch):

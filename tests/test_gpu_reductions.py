@@ -149,43 +149,6 @@ def stem_stats_case(dev, exact, g, n, h, w):
     return run, ref
 
 
-def gemm_stats_case(dev, exact, g, m, k, n):
-    from byol_b200 import ops
-    x, w = _vals((m, k), exact, g, 1, 0.25), _vals((n, k), exact, g, 1, 0.5)
-    xd, wd = x.to(dev, BF), w.to(dev, BF)
-
-    def run():
-        st = torch.zeros(2 * n, device=dev)
-        assert ops.gemm_fused(xd, wd, stats=st, no_store=True) is None
-        return [st, ops.gemm_fused(xd, wd)]
-    return run, lambda o: [("y", o[1], x.double() @ w.double().t()), ("stats", o[0], _colstats(o[1]))]
-
-
-def gemm_bwd_reduce_case(dev, exact, g, m, k, n):
-    from byol_b200 import ops
-    x, w = _vals((m, k), exact, g, 1, 0.25), _vals((n, k), exact, g, 1, 0.5)
-    gq = _vals((m, n), exact, g, 2)
-    keep = torch.rand(m, n, generator=g) > 0.4
-    bits = ((keep.view(-1, 8).int() * (2 ** torch.arange(8, dtype=torch.int32))).sum(1)).to(torch.uint8)
-    if exact:
-        cs = torch.pow(2.0, torch.randint(-1, 2, (n,), generator=g).float())
-        bias = torch.randint(-3, 4, (n,), generator=g).float()
-    else:
-        cs, bias = torch.rand(n, generator=g) + 0.5, torch.randn(n, generator=g)
-    xd, wd, gqd, bitsd, csd, biasd = x.to(dev, BF), w.to(dev, BF), gq.to(dev, BF), bits.to(dev), cs.to(dev), bias.to(dev)
-
-    def run():
-        s12 = torch.zeros(2 * n, device=dev)
-        ops.gemm_fused(xd, wd, colscale=csd, bias=biasd, resid=gqd, resid_mask=bitsd, stats=s12, bwd_reduce=True)
-        return [s12]
-
-    def ref(o):
-        t = (x.double() @ w.double().t()) * cs.double() + bias.double()
-        dz = gq.double() * keep.double()
-        return [("s12", o[0], torch.cat([dz.sum(0), (dz * t).sum(0)]))]
-    return run, ref
-
-
 def wgrad_case(dev, exact, g, n, h, w, c, cout, k, s, p, gather):
     from byol_b200 import ops
     ho, wo = ops.conv_out_size(h, k, s, p), ops.conv_out_size(w, k, s, p)
@@ -320,10 +283,6 @@ EXACT = {
     "conv3x3_patch_30x26": (conv_stats_case, dict(n=3, h=30, w=26, c=64, cout=256, k=3, s=1, p=1, gather=False)),
     "stem_30x26": (stem_stats_case, dict(n=3, h=30, w=26)),
     "stem_real": (stem_stats_case, dict(n=6, h=224, w=224)),
-    "gemm_no_store_real": (gemm_stats_case, dict(m=REAL_M + 1000, k=64, n=256)),
-    "gemm_no_store_tail": (gemm_stats_case, dict(m=777, k=512, n=2048)),
-    "gemm_bwd_reduce_real": (gemm_bwd_reduce_case, dict(m=REAL_M + 1000, k=64, n=256)),
-    "gemm_bwd_reduce_tail": (gemm_bwd_reduce_case, dict(m=300, k=128, n=136)),
     "wgrad1x1_tma_real": (wgrad_case, dict(n=22, h=56, w=56, c=64, cout=256, k=1, s=1, p=0, gather=False)),
     "wgrad1x1_gather_real": (wgrad_case, dict(n=22, h=56, w=56, c=64, cout=256, k=1, s=1, p=0, gather=True)),
     "wgrad3x3_gather": (wgrad_case, dict(n=4, h=14, w=14, c=128, cout=128, k=3, s=1, p=1, gather=True)),
@@ -350,8 +309,6 @@ BITS = {
     "conv1x1_gather": (conv_stats_case, dict(n=8, h=28, w=28, c=64, cout=256, k=1, s=1, p=0, gather=True)),
     "conv3x3_patch": (conv_stats_case, dict(n=3, h=30, w=26, c=64, cout=256, k=3, s=1, p=1, gather=False)),
     "stem": (stem_stats_case, dict(n=3, h=64, w=64)),
-    "gemm_no_store": (gemm_stats_case, dict(m=5000, k=64, n=256)),
-    "gemm_bwd_reduce": (gemm_bwd_reduce_case, dict(m=5000, k=64, n=256)),
     "wgrad1x1_tma": (wgrad_case, dict(n=8, h=28, w=28, c=64, cout=256, k=1, s=1, p=0, gather=False)),
     "wgrad1x1_gather": (wgrad_case, dict(n=8, h=28, w=28, c=64, cout=256, k=1, s=1, p=0, gather=True)),
     "wgrad3x3_patch": (wgrad_case, dict(n=3, h=30, w=26, c=64, cout=64, k=3, s=1, p=1, gather=False)),
@@ -497,9 +454,9 @@ def test_special_values_bn_bwd_reduce(cuda, c):
 
 
 def test_special_values_gemm_epilogue_total_past_2_45(cuda):
-    """2^18 rows of y = 2^14 give a sum of squares of 2^46 through the implicit-GEMM and the fused-GEMM epilogues.
-    Both sum a warp's rows in fp32 registers until it moves to other columns, so each addend here is far above 2^20
-    and mostly lands in the fp64 side sum: the total must still equal fp64 exactly."""
+    """2^18 rows of y = 2^14 give a sum of squares of 2^46 through the implicit-GEMM epilogue.  It sums a warp's rows
+    in fp32 registers until it moves to other columns, so each addend here is far above 2^20 and mostly lands in the
+    fp64 side sum: the total must still equal fp64 exactly."""
     from byol_b200 import ops
     m, k, n = 1 << 18, 64, 128
     gen = _gen(41)
@@ -509,15 +466,11 @@ def test_special_values_gemm_epilogue_total_past_2_45(cuda):
     w[:, 0] = 0.0
     w[0, :], w[0, 0] = 0.0, 128.0                        # column 0 of y is 2^14 in every row
     xd, wd = x.to(cuda, BF), w.to(cuda, BF)
-    st = torch.zeros(2 * n, device=cuda)
-    ops.gemm_fused(xd, wd, stats=st, no_store=True)
-    y = ops.gemm_fused(xd, wd)
     st_ig = torch.zeros(2 * n, device=cuda)
     y_ig = ops.linear_fprop(xd, ops.prep_weight(w.to(cuda), want_dgrad=False)[0], stats=st_ig)
     torch.cuda.synchronize()
-    _expect_equal("fused-GEMM stats", st, _colstats(y))
     _expect_equal("implicit-GEMM stats", st_ig, _colstats(y_ig))
-    assert float(st[n]) == 2.0 ** 46 and float(st_ig[n]) == 2.0 ** 46
+    assert float(st_ig[n]) == 2.0 ** 46
 
 
 def test_special_values_col_sum_f32(cuda):

@@ -89,5 +89,3 @@ def test_recompute_plan_override_and_scope():
         e = _engine("resnet50", precision)
         e._mem_budget = 0
         assert e.recompute_plan(64, 128, 128) == frozenset()
-    eng.fuse3 = True
-    assert eng.recompute_plan(64, 128, 128) == frozenset()
