@@ -29,9 +29,10 @@ static constexpr int SGD_THREADS = 128;
 //                              = (m - xl) + log(s + e)  otherwise (the loss is >= 1)
 //   grad = exp(v - m) / (s + e) / B,  and -s / (s + e) / B at the label (softmax - 1 without cancellation)
 // The rank is the number of other columns whose logit is not <= the label's: for finite logits the strictly larger
-// ones (ce_topk_fwd_kernel's rule: the label is in the top k iff rank < k), and a NaN column ranks above the label.
-// A row whose label logit is NaN is a miss for every k, so diverged features or weights can not score hits.  A row
-// whose label is outside [0, C) is ignored: no loss, no hit, and a zero gradient.  Per-head loss sums go to
+// ones, and a NaN column ranks above the label; the label is in the top k iff rank < k.  A row whose label logit is
+// NaN is a miss for every k, so diverged features or weights can not score hits.  ce_topk_fwd_kernel (csrc/optim.cu)
+// ranks by the same rule.  A row whose label is outside [0, C) is ignored here: no loss, no hit, and a zero gradient
+// (ce_topk_fwd_kernel counts it as a miss with loss +inf).  Per-head loss sums go to
 // fixed-point accumulators and hit counts to integer counters, both order-independent, so every launch gives the
 // same bits.
 // ---------------------------------------------------------------------------------------------------------------------

@@ -14,10 +14,14 @@ namespace byol {
 // ---------------------------------------------------------------------------------------------
 // loss
 // sums[0] = |q1|^2  sums[1] = |q2|^2  sums[2] = |z1|^2  sums[3] = |z2|^2  sums[4] = <q1,z2>  sums[5] = <q2,z1>
+// Every block writes its six fp32 partial sums to its own fp64 slots, part[k * gridDim.x + block]; the finalize kernel
+// adds them in block order.  The result is deterministic and its precision relative, so the loss is invariant under
+// power-of-two scaling of its inputs at any scale (a fixed-point accumulator's absolute resolution would not be: with
+// predictions or targets of RMS ~1e-5 it would cost the loss whole fp32 ulps).
 // ---------------------------------------------------------------------------------------------
 __global__ void loss_fwd_partial_kernel(const float* __restrict__ q1, const float* __restrict__ q2,
                                         const float* __restrict__ z1, const float* __restrict__ z2,
-                                        Fix128* __restrict__ sums, int64_t n4) {
+                                        double* __restrict__ part, int64_t n4) {
   float acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
     const float4 a = __ldg(reinterpret_cast<const float4*>(q1) + i);
@@ -45,20 +49,27 @@ __global__ void loss_fwd_partial_kernel(const float* __restrict__ q1, const floa
     for (int k = 0; k < 6; ++k) {
       float v = lane < nw ? sh[k][lane] : 0.f;
       v = warp_sum(v);
-      if (lane == 0) fix_add(sums + k, v);   // fixed point: order-independent
+      if (lane == 0) part[k * gridDim.x + blockIdx.x] = (double)v;
     }
   }
 }
 
-// loss = -2/b * ( <q1,z2>/(|q1||z2|) + <q2,z1>/(|q2||z1|) );  also stores fp32 copies of the six sums
-__global__ void loss_finalize_kernel(Fix128* __restrict__ sums, float* __restrict__ loss,
+// loss = -2/b * ( <q1,z2>/(|q1||z2|) + <q2,z1>/(|q2||z1|) );  also stores fp32 copies of the six sums.
+// Thread k < 6 adds the nb block partials of sum k in block order and zeroes them (the slots live in the stream's
+// scratch, which its users leave zeroed).
+__global__ void loss_finalize_kernel(double* __restrict__ part, int nb, float* __restrict__ loss,
                                      float* __restrict__ saved, int rows) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) {
-    float v[6];
-    for (int k = 0; k < 6; ++k) {
-      v[k] = (float)fix_value(sums[k]);
-      sums[k] = Fix128{0ull, 0ll, 0.0};   // the scratch is left zeroed (fix_scratch)
+  __shared__ float v[6];
+  if (threadIdx.x < 6) {
+    double s = 0.0;
+    for (int b = 0; b < nb; ++b) {
+      s += part[threadIdx.x * nb + b];
+      part[threadIdx.x * nb + b] = 0.0;
     }
+    v[threadIdx.x] = (float)s;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
     const float nq1 = sqrtf(v[0]), nq2 = sqrtf(v[1]);
     const float nz1 = sqrtf(v[2]), nz2 = sqrtf(v[3]);
     const float s12 = v[4], s21 = v[5];
@@ -316,9 +327,12 @@ sgd_nesterov_kernel(const uint64_t* __restrict__ p_ptrs, const uint64_t* __restr
 // ---------------------------------------------------------------------------------------------
 // Linear-probe objective: softmax cross-entropy (mean over rows) + top-1 / top-5 accuracy of fp32 logits [R, C]
 // (/root/reference/main.py:596-598: F.cross_entropy + helpers.metrics.topk on the [2b, 1000] classifier output).
-// One warp per row: max, log-sum-exp, the label's logit and its rank (= number of strictly larger logits: the
-// label is in the top k iff rank < k).  Row results go to a scratch array; the last block to finish (ticket
-// counter) adds them up in row order, so the three outputs are deterministic.
+// One warp per row: max, log-sum-exp, the label's logit and its rank.  The rank is the number of other columns whose
+// logit is not <= the label's (linprobe_ce_kernel's rule): for finite logits the strictly larger ones, and a NaN
+// column ranks above the label; the label is in the top k iff rank < k.  A row whose label logit is NaN, or whose
+// label (compared as int64) is outside [0, C), is a miss for every k; the latter's loss is +inf.  Row results go to a
+// scratch array; the last block to finish (ticket counter) adds them up in row order, so the three outputs are
+// deterministic.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 ce_topk_fwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels, int LR, int R, int C, int ld,
@@ -328,18 +342,20 @@ ce_topk_fwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__
   const int r = blockIdx.x * (blockDim.x >> 5) + warp;
   if (r < R) {
     const float* __restrict__ x = logits + (int64_t)r * ld;
-    const int lab = (int)labels[r % LR];   // LR < R: the label vector repeats (two views per sample)
+    const int64_t lab64 = labels[r % LR];   // LR < R: the label vector repeats (two views per sample)
+    const bool lab_ok = lab64 >= 0 && lab64 < C;
+    const int lab = lab_ok ? (int)lab64 : -1;
     float mx = -INFINITY;
     for (int c = lane; c < C; c += 32) mx = fmaxf(mx, x[c]);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    const float xl = (lab >= 0 && lab < C) ? x[lab] : -INFINITY;
+    const float xl = lab_ok ? x[lab] : -INFINITY;
     float se = 0.f;
     int gt = 0;
     for (int c = lane; c < C; c += 32) {
       const float v = x[c];
       se += expf(v - mx);
-      gt += (v > xl) ? 1 : 0;
+      gt += (c != lab && !(v <= xl)) ? 1 : 0;
     }
     se = warp_sum(se);
 #pragma unroll
@@ -348,7 +364,7 @@ ce_topk_fwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__
       const float lse = mx + logf(se);
       row_lse[r] = lse;
       row_loss[r] = lse - xl;
-      row_rank[r] = gt;
+      row_rank[r] = lab_ok && !isnan(xl) ? gt : 0x7fffffff;   // a miss for every k
     }
   }
   __shared__ bool last;
@@ -399,7 +415,8 @@ ce_bwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labe
   const float* __restrict__ x = logits + (int64_t)r * ld;
   float* __restrict__ d = dlogits + (int64_t)r * ldd;
   const float lse = row_lse[r];
-  const int lab = (int)labels[r % LR];
+  const int64_t lab64 = labels[r % LR];
+  const int lab = lab64 >= 0 && lab64 < C ? (int)lab64 : -1;   // out of range: no one-hot term
   for (int c = lane; c < C; c += 32) d[c] = k * (expf(x[c] - lse) - (c == lab ? 1.f : 0.f));
 }
 
@@ -415,17 +432,22 @@ static inline int grid_for(int64_t n, int block, int max_blocks = 132 * 16) {
 using namespace byol;
 
 // q1,q2,z1,z2: [rows, dim] fp32 contiguous (rows*dim % 4 == 0).  workspace: 6 doubles (zeroed here).
-// loss: 1 float.  saved: 6 floats consumed by byol_loss_bwd.  The six sums are accumulated in fixed point in the
-// stream's scratch (fix_scratch); `workspace` is part of the ABI but no longer used.
+// loss: 1 float.  saved: 6 floats consumed by byol_loss_bwd.  The per-block partial sums (6 x at most 132 doubles) live
+// in the stream's zeroed scratch (fix_scratch, whose accumulators are three 8-byte words each, so zero bits read as
+// 0.0); `workspace` is part of the ABI but no longer used.
 extern "C" int byol_loss_fwd(const float* q1, const float* q2, const float* z1, const float* z2, int rows, int dim,
                              double* workspace, float* loss, float* saved, cudaStream_t stream) {
   BYOL_CHECK_ARG(q1 && q2 && z1 && z2 && workspace && loss && saved, "byol_loss_fwd: null pointer");
   const int64_t n = (int64_t)rows * dim;
   BYOL_CHECK_ARG(rows > 0 && dim > 0 && n % 4 == 0, "byol_loss_fwd: rows*dim must be a positive multiple of 4");
-  Fix128* sums = fix_scratch(stream, 6);
-  if (sums == nullptr) return -2;
-  loss_fwd_partial_kernel<<<grid_for(n / 4, 256, 132), 256, 0, stream>>>(q1, q2, z1, z2, sums, n / 4);
-  loss_finalize_kernel<<<1, 32, 0, stream>>>(sums, loss, saved, rows);
+  constexpr int kMaxBlocks = 132;
+  static_assert(sizeof(Fix128) == 3 * sizeof(double), "the partial slots are carved from the Fix128 scratch");
+  Fix128* scratch = fix_scratch(stream, 2 * kMaxBlocks);   // 6 * kMaxBlocks doubles
+  if (scratch == nullptr) return -2;
+  double* part = reinterpret_cast<double*>(scratch);
+  const int nb = grid_for(n / 4, 256, kMaxBlocks);
+  loss_fwd_partial_kernel<<<nb, 256, 0, stream>>>(q1, q2, z1, z2, part, n / 4);
+  loss_finalize_kernel<<<1, 32, 0, stream>>>(part, nb, loss, saved, rows);
   return fix_done(stream, check_launch("loss_fwd kernels"));
 }
 

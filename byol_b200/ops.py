@@ -502,16 +502,25 @@ def sgd_nesterov_step(table, lr_scale, momentum):
                                      float(lr_scale), float(momentum), _stream()), "byol_sgd_nesterov_step")
 
 
-def ce_topk_fwd(logits, labels, scratch=None):
-    """Softmax cross-entropy (mean) + top-1 / top-5 accuracy (%) of fp32 logits [R, C] in one launch; `labels` has R
-    entries or a divisor of R (row r uses labels[r % len]: both views of a sample share its label).
-    Returns (out fp32 [3] = loss, top1, top5; row_lse fp32 [R] for the backward pass)."""
-    _chk(logits, F32, "logits")
+def _ce_args(logits, labels):
+    """The checks both cross-entropy entry points share: fp32 CUDA logits [R, C] with unit column stride (rows may be
+    pitched, e.g. a column slice), contiguous CUDA int64 labels whose count divides R."""
+    if logits.dtype != F32 or not logits.is_cuda or logits.dim() != 2 or logits.stride(1) != 1:
+        raise ValueError("logits must be a CUDA fp32 matrix with unit column stride")
     if labels.dtype != torch.int64 or not labels.is_cuda or not labels.is_contiguous():
         raise ValueError("labels must be a contiguous CUDA int64 tensor")
     r, c = logits.shape
     if labels.numel() == 0 or r % labels.numel() != 0:
         raise ValueError("labels: %d entries do not tile %d rows" % (labels.numel(), r))
+    return r, c
+
+
+def ce_topk_fwd(logits, labels, scratch=None):
+    """Softmax cross-entropy (mean) + top-1 / top-5 accuracy (%) of fp32 logits [R, C] in one launch; `labels` has R
+    entries or a divisor of R (row r uses labels[r % len]: both views of a sample share its label).
+    Rows may be pitched (a column slice: unit column stride, row stride >= C).
+    Returns (out fp32 [3] = loss, top1, top5; row_lse fp32 [R] for the backward pass)."""
+    r, c = _ce_args(logits, labels)
     dev = logits.device
     fl = torch.empty(2 * r + 3, dtype=F32, device=dev)            # row_lse | row_loss | out
     it = torch.zeros(r + 1, dtype=torch.int32, device=dev)        # row_rank | ticket (must start at 0)
@@ -521,7 +530,12 @@ def ce_topk_fwd(logits, labels, scratch=None):
 
 
 def ce_bwd(logits, labels, row_lse, grad_out):
-    r, c = logits.shape
+    """dlogits fp32 [R, C] (contiguous) = grad_out / R * (softmax - onehot) from ce_topk_fwd's row_lse; the same
+    logits / labels checks as ce_topk_fwd."""
+    r, c = _ce_args(logits, labels)
+    _chk(row_lse, F32, "row_lse"); _chk(grad_out, F32, "grad_out")
+    if row_lse.numel() != r:
+        raise ValueError("row_lse: %d entries for %d rows" % (row_lse.numel(), r))
     d = torch.empty((r, c), dtype=F32, device=logits.device)
     check(lib.byol_ce_bwd(_ptr(logits), _ptr(labels), labels.numel(), _ptr(row_lse), _ptr(grad_out), r, c, logits.stride(0), _ptr(d), c,
                           _stream()), "byol_ce_bwd")

@@ -64,7 +64,8 @@ class DistributedDataParallelPassthrough(nn.Module):
 
 def topk(output, target, topk=(1,)):
     """helpers.metrics.topk (main.py:598) for k in {1, 5}: percentage of rows whose label is among the k largest
-    logits, from the fused kernel (rank of the label's logit = number of strictly larger logits)."""
+    logits, from the fused kernel (rank of the label's logit = number of other logits not <= it; a NaN label logit or
+    a label outside [0, classes) is a miss)."""
     from . import ops
     if any(k not in (1, 5) for k in topk):
         raise NotImplementedError("byol_b200.wiring.topk: k must be 1 or 5")

@@ -23,7 +23,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests.util import gen, ints, pack_bits, pow2, report_mismatch, unpack_bits
+from tests.util import _fma32, gen, ints, pack_bits, pow2, report_mismatch, unpack_bits
 
 pytestmark = pytest.mark.gpu
 BF, F32, F64, U8 = torch.bfloat16, torch.float32, torch.float64, torch.uint8
@@ -275,24 +275,6 @@ def bn_bwd_reduce_case(dev, g, m, c, mask_mode):
 
 
 # --- statistics -> coefficients: numpy restatement of the compiled arithmetic ------------------------------------
-def _rn32(fr):
-    """Fraction -> the nearest fp32 (ties to even), without double rounding."""
-    f = np.float32(float(fr))
-    if Fraction(float(f)) == fr or not np.isfinite(f):
-        return f
-    up = Fraction(float(f)) < fr
-    other = np.nextafter(f, np.float32(np.inf if up else -np.inf), dtype=np.float32)
-    mid = (Fraction(float(f)) + Fraction(float(other))) / 2
-    if fr == mid:
-        return f if (f.view(np.uint32) & 1) == 0 else other
-    return other if (fr > mid) == up else f
-
-
-def _fma32(a, b, c):
-    return np.array([_rn32(Fraction(float(x)) * Fraction(float(y)) + Fraction(float(z)))
-                     for x, y, z in zip(a, b, c)], dtype=np.float32)
-
-
 def _fma64(a, b, c):
     return np.array([float(Fraction(float(x)) * Fraction(float(y)) + Fraction(float(z))) for x, y, z in zip(a, b, c)])
 

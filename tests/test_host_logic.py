@@ -122,3 +122,23 @@ def test_lr_schedule_matches_reference_wiring():
     sched2 = EpochSchedule(opt, epochs=100, warmup=10)
     sched2.load_state_dict(st)
     assert sched2.get_last_lr() == sched.get_last_lr()
+
+
+def test_vectorised_fma32_rounds_once():
+    """tests.util.fma32 (the fused multiply-add of the numpy kernel restatements) equals the exact rational a*b + c
+    rounded once to fp32, on random operands, on sums that cancel and on ties."""
+    from tests.util import _fma32, fma32
+    rng = np.random.default_rng(3)
+    a = (rng.standard_normal(4000) * 2.0 ** rng.integers(-30, 30, 4000)).astype(np.float32)
+    b = (rng.standard_normal(4000) * 2.0 ** rng.integers(-30, 30, 4000)).astype(np.float32)
+    c = np.concatenate([(rng.standard_normal(2000) * 2.0 ** rng.integers(-60, 60, 2000)).astype(np.float32),
+                        -(a[2000:].astype(np.float64) * b[2000:]).astype(np.float32)])   # near-total cancellation
+    one = np.float32(1.0)
+    ties = np.array([1 + 2.0 ** -23, 1 + 2.0 ** -22], dtype=np.float32)          # 1 * x + 2^-24: ties to even
+    a = np.concatenate([a, ties, ties, [one, np.float32(np.inf), np.float32(np.nan)]])
+    b = np.concatenate([b, [one, one], [one, one], [np.float32(0), one, one]])
+    c = np.concatenate([c, np.float32([2.0 ** -24] * 2), np.float32([2.0 ** -24 + 2.0 ** -48] * 2),
+                        [np.float32(-0.0), np.float32(-np.inf), one]])
+    got, want = fma32(a, b, c), _fma32(a[:-2], b[:-2], c[:-2])
+    assert np.array_equal(got[:-2].view(np.uint32), want.view(np.uint32))
+    assert np.isnan(got[-2]) and np.isnan(got[-1])

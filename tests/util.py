@@ -1,4 +1,7 @@
 """Shared helpers for the parity tests."""
+from fractions import Fraction
+
+import numpy as np
 import torch
 
 
@@ -21,6 +24,43 @@ def pow2(n, dev, g, signed=False):
     if signed:
         v = v * (torch.randint(0, 2, (n,), generator=g, device=dev) * 2 - 1)
     return v
+
+
+# fp32 roundings for the numpy restatements of compiled kernel arithmetic (test_gpu_elementwise_exact,
+# test_gpu_optim_exact)
+def _rn32(fr):
+    """Fraction -> the nearest fp32 (ties to even), without double rounding."""
+    f = np.float32(float(fr))
+    if Fraction(float(f)) == fr or not np.isfinite(f):
+        return f
+    up = Fraction(float(f)) < fr
+    other = np.nextafter(f, np.float32(np.inf if up else -np.inf), dtype=np.float32)
+    mid = (Fraction(float(f)) + Fraction(float(other))) / 2
+    if fr == mid:
+        return f if (f.view(np.uint32) & 1) == 0 else other
+    return other if (fr > mid) == up else f
+
+
+def _fma32(a, b, c):
+    """fp32 fused multiply-add a*b + c, rounded once (elementwise over equal-length sequences)."""
+    return np.array([_rn32(Fraction(float(x)) * Fraction(float(y)) + Fraction(float(z)))
+                     for x, y, z in zip(a, b, c)], dtype=np.float32)
+
+
+def fma32(a, b, c):
+    """Vectorised _fma32 over fp32 arrays.  The fp64 product of two fp32 values is exact; the fp64 sum is turned into
+    its round-to-odd value with the exact TwoSum error, and rounding a round-to-odd fp64 value to fp32 is a correct
+    single rounding (53 >= 24 + 2 bits)."""
+    a, b, c = (np.asarray(v, dtype=np.float32).astype(np.float64) for v in np.broadcast_arrays(a, b, c))
+    with np.errstate(invalid="ignore", over="ignore"):
+        p = a * b
+        s = p + c
+        bb = s - p
+        e = (p - (s - bb)) + (c - bb)
+        odd = (s.view(np.int64) & 1) == 1
+        fix = np.isfinite(s) & (e != 0) & ~odd
+        s = np.where(fix, np.nextafter(s, np.where(e > 0, np.inf, -np.inf)), s)
+    return s.astype(np.float32)
 
 
 def pack_bits(keep):
