@@ -182,6 +182,83 @@ int fix_flush(Fix128* acc, float* dst, int64_t n, cudaStream_t stream) {
   return check_launch("fix_flush_kernel");
 }
 
+// Per-(device, stream) buffer of the wgrad partials.  Like fix_scratch it only grows and never frees a buffer a
+// captured graph may still reference; it holds no state between reductions.
+namespace {
+struct PartScratch {
+  int dev;
+  cudaStream_t stream;
+  float* p;
+  int64_t n;
+};
+static PartScratch g_part[256];
+static int g_part_count = 0;
+}  // namespace
+
+float* part_scratch(cudaStream_t stream, int64_t n) {
+  const int dev = device_slot();
+  PartScratch* e = nullptr;
+  for (int i = 0; i < g_part_count; ++i)
+    if (g_part[i].dev == dev && g_part[i].stream == stream) e = &g_part[i];
+  if (e == nullptr) {
+    if (g_part_count == 256) { set_last_error("part_scratch: too many streams"); return nullptr; }
+    e = &g_part[g_part_count++];
+    e->dev = dev; e->stream = stream; e->p = nullptr; e->n = 0;
+  }
+  if (e->n < n) {
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    cudaThreadExchangeStreamCaptureMode(&mode);
+    float* p = nullptr;
+    const int64_t want = n + n / 2;
+    cudaError_t err = cudaMalloc(&p, (size_t)want * sizeof(float));
+    cudaThreadExchangeStreamCaptureMode(&mode);
+    if (err != cudaSuccess) { set_last_error("part_scratch: cudaMalloc failed: %s", cudaGetErrorString(err)); return nullptr; }
+    e->p = p;   // the previous buffer is kept alive (see above)
+    e->n = want;
+  }
+  return e->p;
+}
+
+// Block pass: 256 / sl consecutive elements (coalesced loads), each summed by sl threads over every sl-th split; the
+// sl partial accumulators of an element are then added up (integer words wrap; the side sums of multiples of 2^20 are
+// exact), which gives the same words and side sum in any grouping.  sl > 1 keeps the SMs busy when there are few
+// elements and many splits.
+__global__ void wgrad_reduce_kernel(const float* __restrict__ part, int splits, float* __restrict__ dst, int64_t n,
+                                    int sl) {
+  __shared__ Fix128 acc[256];
+  const int per = 256 / sl;
+  const int e = threadIdx.x % per, j = threadIdx.x / per;
+  for (int64_t base = blockIdx.x * (int64_t)per; base < n; base += (int64_t)gridDim.x * per) {
+    const int64_t i = base + e;
+    Fix128 a{0ull, 0ll, 0.0};
+    if (i < n)
+      for (int s = j; s < splits; s += sl) fix_add_reg(a, __ldg(part + s * n + i));
+    acc[threadIdx.x] = a;
+    __syncthreads();
+    if (j == 0 && i < n) {
+      for (int k = 1; k < sl; ++k) {
+        const Fix128 b = acc[k * per + e];
+        a.lo += b.lo;
+        a.hi = (long long)((unsigned long long)a.hi + (unsigned long long)b.hi);
+        a.spill += b.spill;
+      }
+      atomicAdd(dst + i, (float)fix_value(a));   // two streams may add into one gradient
+    }
+    __syncthreads();
+  }
+}
+
+int wgrad_reduce(const float* part, int splits, float* dst, int64_t n, cudaStream_t stream) {
+  if (n <= 0) return 0;
+  int sl = 1;   // split lanes per element: about 2^18 threads in all, at most one per split
+  while (sl < 32 && 2 * sl <= splits && n * sl < (1 << 18)) sl *= 2;
+  const int per = 256 / sl;
+  int64_t blocks = (n + per - 1) / per;
+  if (blocks > 4 * 1024) blocks = 4 * 1024;
+  wgrad_reduce_kernel<<<(int)blocks, 256, 0, stream>>>(part, splits, dst, n, sl);
+  return check_launch("wgrad_reduce_kernel");
+}
+
 int fix_flush_stats(Fix128* acc, float* col_sum, float* col_sqsum, int64_t n, cudaStream_t stream) {
   const int rc = fix_flush(acc, col_sum, n, stream);
   if (rc != 0) return rc;

@@ -73,15 +73,21 @@ __device__ __forceinline__ void fix_add_words(Fix128* acc, unsigned long long lo
   atomicAdd(&acc->lo, lo);   // results unused: both compile to reductions
   atomicAdd(reinterpret_cast<unsigned long long*>(&acc->hi), (unsigned long long)hi);
 }
-// Sends the part of v the fixed-point words can not take to acc's fp64 side sum; false when nothing is left for them.
-__device__ __forceinline__ bool fix_take_spill(Fix128* acc, double& v) {
+// Takes from v the part the fixed-point words can not hold and hands it to add_spill (the fp64 side sum); false when
+// nothing is left for the words.  The one place of the 2^20 spill and NaN / Inf rule.
+template <class AddSpill>
+__device__ __forceinline__ bool fix_split_spill(double& v, AddSpill add_spill) {
   if (!(fabs(v) < kFixSplit)) {   // NaN, Inf, or a part too large for the fixed-point words
     const double big = isfinite(v) ? trunc(v * 0x1p-20) * 0x1p20 : v;
-    atomicAdd(&acc->spill, big);
+    add_spill(big);
     if (!isfinite(v)) return false;
     v -= big;                      // exact: the bits of v below 2^20, |v| < 2^20
   }
   return true;
+}
+// Sends the part of v the fixed-point words can not take to acc's fp64 side sum; false when nothing is left for them.
+__device__ __forceinline__ bool fix_take_spill(Fix128* acc, double& v) {
+  return fix_split_spill(v, [acc](double big) { atomicAdd(&acc->spill, big); });
 }
 // the two fixed-point words of v, |v| < kFixSplit
 __device__ __forceinline__ void fix_words(double v, unsigned long long& lo, long long& hi) {
@@ -114,6 +120,28 @@ __device__ __forceinline__ void fix_add_raw(Fix128* acc, const Fix128& v) {
 }
 __host__ __device__ __forceinline__ double fix_value(const Fix128& a) {
   return ((double)a.hi * 0x1p-18 + (double)a.lo * 0x1p-50) + a.spill;
+}
+// fix_add into accumulators held by the calling thread: from zeroed accumulators, the same words and side sum (so the
+// same fix_value) as fix_add of the same addends into the scratch, in any order
+__device__ __forceinline__ void fix_add_reg(Fix128& a, double v) {
+  if (!fix_split_spill(v, [&a](double big) { a.spill += big; })) return;
+  unsigned long long lo;
+  long long hi;
+  fix_words(v, lo, hi);
+  a.lo += lo;
+  a.hi = (long long)((unsigned long long)a.hi + (unsigned long long)hi);   // wraps like the 64-bit reductions
+}
+// The weight gradients' split-K reduction.  A wgrad CTA stores its fp32 partial of every dW element it covers to
+// part[split * n + element] (part_scratch: every entry is written before it is read, so the buffer needs no zeroing);
+// wgrad_reduce then adds each element's partials in fixed point (fix_add_reg) and its value to dst with ONE fp32
+// atomic addition, the same bits as fix_add of every partial followed by fix_flush.  With one split the kernel itself
+// adds fix_value of its single partial (wgrad_add_single).
+float* part_scratch(cudaStream_t stream, int64_t n);
+int wgrad_reduce(const float* part, int splits, float* dst, int64_t n, cudaStream_t stream);
+__device__ __forceinline__ void wgrad_add_single(float* dst, float v) {
+  Fix128 a{0ull, 0ll, 0.0};
+  fix_add_reg(a, v);
+  atomicAdd(dst, (float)fix_value(a));
 }
 
 #define BYOL_CHECK_ARG(cond, ...)                 \

@@ -712,8 +712,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
 //   A = dY  (MN-major: smem rows are pixels, 64-channel chunks along M)   via TMA
 //   B = src (MN-major: smem rows are pixels, 64-channel chunks along N)   via TMA (plain GEMM) or gather
 //   D[co 128][ci BN] accumulated in registers of two MMA warpgroups (co rows 0-63 / 64-127) over this CTA's pixel
-//   range, then atomically added from the registers to the fp32 gradient in the reference's [Cout][Cin][KH][KW]
-//   parameter layout.
+//   range, then stored from the registers as this split's partial of the fp32 gradient, in the reference's
+//   [Cout][Cin][KH][KW] parameter layout (wgrad_reduce), or with one split added to the gradient directly.
 //   warps 0-3: B gather (when B is not loaded by TMA), warps 4-11: MMA warpgroups, warp 12: TMA producer.
 // ---------------------------------------------------------------------------------------------
 struct WgradParams {
@@ -731,7 +731,8 @@ struct WgradParams {
   int groups;        // number of column groups: KH*KW taps, or KH in folded mode
   int fold_kw;       // 1: C == 8 and the KW taps are folded into the 64-wide column group: column = kw*8 + c
   int small_src;     // 1: 32-bit element offsets are safe
-  Fix128* fx;     // fixed-point accumulators over the whole dw (fix_scratch), flushed into dw after the kernel
+  float* part;       // splits > 1: [splits][Cout * Cin_real * KH * KW] fp32 partials (part_scratch), see wgrad_reduce
+  int64_t ndw;
   // split-operand plane layouts (byol_conv_wgrad_planes): the product terms are an outer K loop.  K-block kb belongs
   // to term kb / kb_per_term, which reads dY columns from term * dy_term on and src channels from src_term[term] on.
   // Plain bf16 operands: terms = 1, ldsrc = C.
@@ -767,7 +768,9 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
   uint64_t* full_bar = (uint64_t*)(smemB + STAGES * B_STAGE);
   uint64_t* empty_bar = full_bar + STAGES;
 
-  const int warp = threadIdx.x >> 5;
+  // a warp index ptxas knows is warp-uniform: derived straight from threadIdx.x, the MMA branch counts as divergent
+  // and ptxas serializes the wgmma of the TMA-operand variant (C7518)
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
   int bid = blockIdx.x;
   const int tile_n = bid % p.tiles_n;    bid /= p.tiles_n;
@@ -885,10 +888,14 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmapA, const __grid_consta
     }
     wg_wait<0>();
     wg_fence_acc(d);
-    // ---------------- epilogue: registers -> L2 reductions into the fp32 gradient ----------------
+    // ---------------- epilogue: registers -> this split's partials (or, with one split, the gradient) ----------------
     const int t = threadIdx.x & 127;
     const int r0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
-    auto add = [&](const float* q, float v) { fix_add(p.fx + (q - p.dw), v); };
+    float* const part = p.part != nullptr ? p.part + (int64_t)split * p.ndw : nullptr;
+    auto add = [&](float* q, float v) {
+      if (part != nullptr) part[q - p.dw] = v;
+      else wgrad_add_single(q, v);
+    };
     if (GROUPED) {
       // column c of warpgroup wg is input channel co0 + 64*wg + c
       const int gs = p.Cin_real;
@@ -1259,9 +1266,9 @@ static int conv_wgrad_impl(const void* src, const void* dy, float* dw, int Nimg,
   p.small_src = ((int64_t)Nimg * Hs * Ws * p.ldsrc < (1ll << 31) - (1ll << 24)) ? 1 : 0;
   const int taps = KH * KW;
   const int base_ctas = p.tiles_co * p.tiles_n;
-  // The epilogue adds 128 x BN values per CTA to the gradient with L2 reductions, so the split count trades
+  // Every split stores 128 x BN partials per CTA that wgrad_reduce reads back, so the split count trades
   // parallelism against reduction traffic: exactly one resident wave (one CTA per SM), rounded DOWN so that no
-  // second, nearly empty wave appears.
+  // second, nearly empty wave appears.  The split count fixes the bits of dW (each split is one fp32 partial).
   const int target_ctas = device_sm_count();
   int splits = target_ctas / base_ctas;
   int max_splits = (p.num_kb_total + 7) / 8;                // at least 8 k-blocks (512 pixels) per CTA
@@ -1285,13 +1292,16 @@ static int conv_wgrad_impl(const void* src, const void* dy, float* dw, int Nimg,
   } else {
     tb = ta;
   }
-  const int64_t ndw = (int64_t)Cout * Cin_real * taps;
-  p.fx = fix_scratch(stream, ndw);
-  if (p.fx == nullptr) return -2;
+  p.ndw = (int64_t)Cout * Cin_real * taps;
+  if (p.splits > 1) {
+    p.part = part_scratch(stream, p.splits * p.ndw);
+    if (p.part == nullptr) return -2;
+  }
   const int rc = gs > 0 ? launch_wgrad<128, false, true>(ta, tb, p, grid, stream)
                : BN == 128 ? (b_tma ? launch_wgrad<128, true>(ta, tb, p, grid, stream) : launch_wgrad<128, false>(ta, tb, p, grid, stream))
                            : (b_tma ? launch_wgrad<64, true>(ta, tb, p, grid, stream) : launch_wgrad<64, false>(ta, tb, p, grid, stream));
-  return fix_done(stream, rc != 0 ? rc : fix_flush(p.fx, dw, ndw, stream));
+  if (rc != 0 || p.splits == 1) return rc;
+  return wgrad_reduce(p.part, p.splits, dw, p.ndw, stream);
 }
 
 // Grouped 3x3 wgrad: dw[C][Cg][KH][KW] (fp32, the real parameter, accumulated) += the in-group entries of
@@ -1313,8 +1323,8 @@ extern "C" int byol_conv_wgrad(const void* src, const void* dy, float* dw, int N
 
 // fp32-accurate wgrad: dW (fp32) += sum over the T product terms of dY-plane^T x im2col(src-plane).
 // src: bf16 planes [Nimg, Hs, Ws, T*C], dy: bf16 planes [Nimg, Ho, Wo, T*ldy] (both in the activation pattern of
-// byol_split_planes; ldy >= Cout, a multiple of 8).  All terms accumulate into one fixed-point scratch and reach dw with
-// ONE fp32 addition per element.  Always the gather / TMA kernel (no 3x3 patch kernel); a 7x7 stem over 8 padded
+// byol_split_planes; ldy >= Cout, a multiple of 8).  All terms accumulate into one fixed-point sum per element and
+// reach dw with ONE fp32 addition per element.  Always the gather / TMA kernel (no 3x3 patch kernel); a 7x7 stem over 8 padded
 // channels keeps its folded (kw, c) columns.
 extern "C" int byol_conv_wgrad_planes(const void* src, const void* dy, float* dw, int Nimg, int Hs, int Ws, int C,
                                       int Cin_real, int Ho, int Wo, int Cout, int ldy, int KH, int KW, int stride,

@@ -558,8 +558,8 @@ int patch_conv_launch(const void* src, const void* wt, void* dst, const void* re
 //       beyond the image are out-of-bounds -> ZERO, so garbage rows contribute nothing
 //   B = X patch  [(TH+2)*(W+2) pixel rows][64*NB ci] MN-major; tap (kh,kw) = the same image shifted by kh*(W+2)+kw rows
 //   D[128 co][kw*64*NB + ci] for the three taps of ONE kh row per CTA, accumulated in the registers of two MMA
-//   warpgroups (co rows 0-63 / 64-127; warps 0-7) over the CTA's range of M-tiles, then added to the fp32 gradient
-//   with L2 reductions.  Warp 8 is the TMA producer.
+//   warpgroups (co rows 0-63 / 64-127; warps 0-7) over the CTA's range of M-tiles, then stored as this split's
+//   partial of the fp32 gradient (wgrad_reduce), or with one split added to it directly.  Warp 8 is the TMA producer.
 // Rows of the smem slots that TMA never writes (beyond the boxes) are zeroed once, so stale shared memory can not
 // inject Inf/NaN through the zero rows of A.
 // =================================================================================================
@@ -567,7 +567,8 @@ namespace byol {
 
 struct WPatchParams {
   float* dw;            // [Cout][Cin][3][3] fp32 (grouped: [Cout][gs][3][3])
-  Fix128* fx;        // fixed-point accumulators over the whole dw (fix_scratch)
+  float* part;          // splits > 1: [splits][ndw] fp32 partials (part_scratch), see wgrad_reduce
+  int64_t ndw;
   int Nimg, H, W, C, Cout;
   int Wp, TH, HB, num_mt;
   int co_tiles, ci_groups;
@@ -674,9 +675,14 @@ conv3x3_wgrad_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __gr
     wg_wait<0>();
 #pragma unroll
     for (int kw = 0; kw < 3; ++kw) wg_fence_acc(d[kw]);
-    // ---------------- epilogue: registers -> L2 reductions into dW[co][ci][kh][kw] ----------------
+    // ---------------- epilogue: registers -> this split's partials of dW[co][ci][kh][kw] ----------------
     const int t = threadIdx.x & 127;
     const int r0 = co0 + wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
+    float* const part = p.part != nullptr ? p.part + (int64_t)split * p.ndw : nullptr;
+    auto add = [&](int64_t i, float v) {
+      if (part != nullptr) part[i] = v;
+      else wgrad_add_single(p.dw + i, v);
+    };
     if (GROUPED) {
       const int gs = p.gs;
 #pragma unroll
@@ -686,7 +692,7 @@ conv3x3_wgrad_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __gr
           const int co = r0 + ((i & 2) ? 8 : 0);
           const int ci = ci0 + wg * 64 + 8 * (i >> 2) + 2 * (t & 3) + (i & 1);
           if (co < p.Cout && co / gs == ci / gs)
-            fix_add(p.fx + ((int64_t)co * gs + ci % gs) * 9 + kh * 3 + kw, d[kw][i]);
+            add(((int64_t)co * gs + ci % gs) * 9 + kh * 3 + kw, d[kw][i]);
         }
       }
       return;
@@ -697,7 +703,7 @@ conv3x3_wgrad_patch_kernel(const __grid_constant__ CUtensorMap tmapX, const __gr
       for (int i = 0; i < 32 * NB; ++i) {
         const int co = r0 + ((i & 2) ? 8 : 0);
         const int ci = ci0 + 8 * (i >> 2) + 2 * (t & 3) + (i & 1);
-        if (co < p.Cout && ci < p.C) fix_add(p.fx + ((int64_t)co * p.C + ci) * 9 + kh * 3 + kw, d[kw][i]);
+        if (co < p.Cout && ci < p.C) add(((int64_t)co * p.C + ci) * 9 + kh * 3 + kw, d[kw][i]);
       }
     }
   }
@@ -752,11 +758,14 @@ int patch_wgrad_launch(const void* x, const void* dy, float* dw, int Nimg, int H
   if (tmap_nhwc(&tx, x, Nimg, H, W, C, p.Wp, p.TH + 2, "conv3x3_wgrad_patch X") != 0) return -3;
   if (tmap_nhwc(&ty, dy, Nimg, H, W, Cout, p.Wp, p.TH, "conv3x3_wgrad_patch dY") != 0) return -3;
   const int grid = base * p.splits;
-  const int64_t ndw = (int64_t)Cout * (gs > 0 ? gs : C) * 9;
-  p.fx = fix_scratch(stream, ndw);
-  if (p.fx == nullptr) return -2;
+  p.ndw = (int64_t)Cout * (gs > 0 ? gs : C) * 9;
+  if (p.splits > 1) {
+    p.part = part_scratch(stream, p.splits * p.ndw);
+    if (p.part == nullptr) return -2;
+  }
   const int rc = gs > 0 ? launch_wpatch<2, true>(tx, ty, p, grid, stream) : launch_wpatch<NB>(tx, ty, p, grid, stream);
-  return fix_done(stream, rc != 0 ? rc : fix_flush(p.fx, dw, ndw, stream));
+  if (rc != 0 || p.splits == 1) return rc;
+  return wgrad_reduce(p.part, p.splits, dw, p.ndw, stream);
 }
 
 }  // namespace byol

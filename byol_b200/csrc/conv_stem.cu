@@ -231,7 +231,8 @@ stem_fprop_kernel(const __grid_constant__ CUtensorMap tmapY, const StemParams p)
 //   B (N-major, no swizzle)       = the input row itself: N = 8 window pixels x 4 channels, pixel k's window starts
 //     16 bytes after pixel k-1's (overlapping no-swizzle core matrices, as in the forward kernel)
 //   D = four accumulators [128 = 2 kh x 64 co][32 = (kw, c)] (row parity x chain), kept in registers for the CTA's
-//     whole contiguous range of units and added to the fp32 gradient with atomics at the end.
+//     whole contiguous range of units and stored at the end as this CTA's partial of the fp32 gradient (one split per
+//     CTA, wgrad_reduce), or with one CTA added to the gradient directly.
 // The dY ring has 11 slots + a mirror of slot 0 behind slot 10, so that "row oh-1, row oh" are always adjacent in smem.
 //   warps 0-7: two MMA warpgroups (warpgroup wg owns rows 64*wg .. +63 = the dY row tile wg of each pair), warp 8:
 //   producer.
@@ -248,7 +249,7 @@ static_assert(SW_BAR_OFF % 8 == 0 && SW_TOTAL <= 232448 - 1024, "stem wgrad smem
 struct StemWgradParams {
   const bf16* xs;   // [N][Hp][264][4]
   float* dw;        // [64][Cin][7][7] fp32, accumulated
-  Fix128* fx;    // fixed-point accumulators over the whole dw (fix_scratch)
+  float* part;   // gridDim.x > 1: [gridDim.x][64 * Cin * 49] fp32 partials (part_scratch), see wgrad_reduce
   int N, Ho, Wo, Hp, Cin;
   int num_units;    // N * Hp
   int ksteps;       // ceil(Wo / 16)
@@ -374,21 +375,25 @@ stem_wgrad_kernel(const __grid_constant__ CUtensorMap tmapDY, const StemWgradPar
     // ======================= epilogue (once): registers -> fp32 gradient ===================
     if (u_end > u_begin) {
       const int t = threadIdx.x & 127;
+      float* const part = p.part != nullptr ? p.part + (int64_t)blockIdx.x * (64 * p.Cin * 49) : nullptr;
       const int co = (t >> 5) * 16 + ((t & 31) >> 2);   // + 8 for the second row of a fragment pair
       const bool both = (u_end - u_begin) >= 2;
       const int only_par = (u_begin % p.Hp) & 1;
 #pragma unroll
       for (int a = 0; a < 4; ++a) {
         const int par = a >> 1, chain = a & 1;
-        if (!both && par != only_par) continue;   // this row parity never ran: the accumulator is uninitialised
+        const bool ran = both || par == only_par;   // else this row parity never ran: the accumulator is uninitialised
         const int kh = par + (chain == 0 ? (wg == 0 ? 2 : 0) : (wg == 0 ? 6 : 4));
-        if (kh > 6) continue;
+        if (kh > 6 || (!ran && part == nullptr)) continue;
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
           const int col = 8 * (i >> 2) + 2 * (t & 3) + (i & 1);
           const int row = co + ((i & 2) ? 8 : 0);
           const int kw = col >> 2, c = col & 3;
-          if (kw < 7 && c < p.Cin) fix_add(p.fx + ((row * p.Cin + c) * 7 + kh) * 7 + kw, d[a][i]);
+          if (kw >= 7 || c >= p.Cin) continue;
+          const int e = ((row * p.Cin + c) * 7 + kh) * 7 + kw;
+          if (part != nullptr) part[e] = ran ? d[a][i] : 0.f;   // a zero partial adds nothing to the fixed-point sum
+          else wgrad_add_single(p.dw + e, d[a][i]);
         }
       }
     }
@@ -514,12 +519,15 @@ extern "C" int byol_stem_conv_wgrad(const void* xs, const void* dy, float* dw, i
   const uint32_t box[4] = {64, 128, 1, 1};
   if (tmap_bf16(&tmDY, dy, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, "byol_stem_conv_wgrad dY") != 0) return -3;
   if (smem_opt_in((const void*)stem_wgrad_kernel, SW_TOTAL, "stem_wgrad_kernel") != 0) return -2;
-  int grid = device_sm_count();
+  int grid = device_sm_count();   // every CTA gets at least one unit
   if (grid > p.num_units) grid = p.num_units;
   const int64_t ndw = (int64_t)64 * Cin * 49;
-  p.fx = fix_scratch(stream, ndw);
-  if (p.fx == nullptr) return -2;
+  if (grid > 1) {
+    p.part = part_scratch(stream, grid * ndw);
+    if (p.part == nullptr) return -2;
+  }
   stem_wgrad_kernel<<<grid, SW_THREADS, SW_TOTAL, stream>>>(tmDY, p);
   const int rc = check_launch("stem_wgrad_kernel");
-  return fix_done(stream, rc != 0 ? rc : fix_flush(p.fx, dw, ndw, stream));
+  if (rc != 0 || grid == 1) return rc;
+  return wgrad_reduce(p.part, grid, dw, ndw, stream);
 }
