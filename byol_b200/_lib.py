@@ -113,6 +113,10 @@ _SIGNATURES = {
     "byol_augment_params_ragged": [c_void_p, c_void_p, c_int, c_int, c_int, ctypes.c_uint64, ctypes.c_uint64, c_float,
                                    c_float, c_float, c_float, c_float, c_void_p],
     "byol_augment_apply_ragged": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p],
+    "byol_augment_params_recipe": [c_void_p, c_int, c_int, c_int, ctypes.c_uint64, ctypes.c_uint64, c_float,
+                                   c_void_p, c_void_p],
+    "byol_augment_params_ragged_recipe": [c_void_p, c_void_p, c_int, c_int, c_int, ctypes.c_uint64, ctypes.c_uint64,
+                                          c_float, c_void_p, c_void_p],
     "byol_xchg_layout": [c_void_p, c_void_p, c_void_p],
     "byol_xchg_sum": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p],
     # k-NN evaluation, csrc/knn.cu
@@ -127,6 +131,14 @@ _SIGNATURES = {
     "byol_abi_version": [],
     "byol_device_sm_count": [],
 }
+
+
+
+class AugmentRecipe(ctypes.Structure):
+    """``byol_augment_recipe_t``"""
+    _fields_ = [("jitter", c_float * 4), ("p_flip", c_float), ("p_jitter", c_float), ("p_gray", c_float),
+                ("p_blur", c_float * 2), ("p_solarize", c_float * 2), ("bicubic", c_int)]
+
 
 EXPORTED_SYMBOLS = sorted(list(_SIGNATURES.keys()) + ["byol_last_error"])
 

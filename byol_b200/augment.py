@@ -7,33 +7,76 @@ in HBM: ``RandomResizedCrop(R)``, ``RandomHorizontalFlip(0.5)``, ``RandomApply([
     aug1, aug2 = aug(images)            # images: fp32 CUDA [N, 3, H, W] in [0, 1] -> two fp32 [N, 3, 224, 224]
     aug1, aug2 = aug([u8_0, u8_1])      # or a list of CUDA uint8 [3, H_i, W_i] images of any sizes (read as v / 255)
 
+``recipe="byol"`` gives the BYOL paper's views instead (Grill et al. 2020, Appendix B, Table 6): the crop resized with
+an antialiased bicubic filter (clamped to [0, 1]), ``ColorJitter(0.4s, 0.4s, 0.2s, 0.1s)``, blur with p 1.0 on view 1
+and 0.1 on view 2, and ``solarize(0.5)`` last with p 0.0 on view 1 and 0.2 on view 2; crop, flip, jitter p and
+grayscale are the reference's.  The views are asymmetric: the first output is always the paper's view 1.
+
 Every call draws fresh parameters from a counter-based RNG (seed, call counter, sample, view), so a run is
 reproducible and the two views of a sample are independent.  ``apply(images, params)`` and
 ``apply_ragged(images, params)`` run the pipeline on explicit parameter records (tests/test_gpu_augment.py checks every stage against torchvision on identical parameters).
 """
+import ctypes
+
 import torch
 
-from . import ops
+from . import _lib, ops
 from ._lib import lib, check
 
 RECORD = lib.byol_augment_record_floats()
+# record float 14: a flag word
+FLAG_GRAY, FLAG_SOLARIZE, FLAG_BICUBIC = 1, 2, 4
+
+# name -> colour-jitter factors (brightness, contrast, saturation, hue; times color_jitter_strength), blur and
+# solarize probabilities of (view 1, view 2), bicubic crop resize
+RECIPES = {
+    "reference": dict(jitter=(0.8, 0.8, 0.8, 0.2), p_blur=(0.5, 0.5), p_solarize=(0.0, 0.0), bicubic=False),
+    "byol": dict(jitter=(0.4, 0.4, 0.2, 0.1), p_blur=(1.0, 0.1), p_solarize=(0.0, 0.2), bicubic=True),
+}
+
+
+def _probability(name, v):
+    v = float(v)
+    if not 0.0 <= v <= 1.0:
+        raise ValueError("TwoViewAugment: %s must lie in [0, 1], got %r" % (name, v))
+    return v
+
+
+def _per_view(name, v):
+    """A probability for both views, or a (view 1, view 2) pair."""
+    if isinstance(v, (tuple, list)):
+        if len(v) != 2:
+            raise ValueError("TwoViewAugment: %s must be a probability or a (view 1, view 2) pair" % name)
+        return (_probability(name, v[0]), _probability(name, v[1]))
+    p = _probability(name, v)
+    return (p, p)
 
 
 class TwoViewAugment(object):
     def __init__(self, image_size=224, color_jitter_strength=1.0, seed=0, p_flip=0.5, p_jitter=0.8, p_gray=0.2,
-                 p_blur=0.5, blur=True):
+                 p_blur=None, blur=True, recipe="reference", p_solarize=None):
+        """``recipe``: "reference" or "byol" (module docstring).  ``p_blur`` / ``p_solarize``: a probability for both
+        views or a (view 1, view 2) pair; None takes the recipe's."""
+        if recipe not in RECIPES:
+            raise ValueError("TwoViewAugment: unknown recipe %r (expected one of %s)" % (recipe, sorted(RECIPES)))
+        rc = RECIPES[recipe]
+        self.recipe = recipe
         self.R = int(image_size)
         self.strength = float(color_jitter_strength)
         self.seed = int(seed)
-        self.p = (float(p_flip), float(p_jitter), float(p_gray), float(p_blur))
+        self.p = (_probability("p_flip", p_flip), _probability("p_jitter", p_jitter), _probability("p_gray", p_gray))
+        self.p_blur = _per_view("p_blur", rc["p_blur"] if p_blur is None else p_blur)
+        self.p_solarize = _per_view("p_solarize", rc["p_solarize"] if p_solarize is None else p_solarize)
+        self._recipe = _lib.AugmentRecipe(rc["jitter"], self.p[0], self.p[1], self.p[2], self.p_blur,
+                                          self.p_solarize, int(rc["bicubic"]))
         k = int(0.1 * self.R) if blur else 0      # main.py:396 kernel_size = int(0.1 * image_size); made odd
         self.ksize = (k | 1) if k > 0 else 0
         self.calls = 0
 
     def sample_params(self, n, hs, ws, device):
         params = torch.empty((2, n, RECORD), dtype=torch.float32, device=device)
-        check(lib.byol_augment_params(params.data_ptr(), n, hs, ws, self.seed, self.calls, self.strength, self.p[0],
-                                      self.p[1], self.p[2], self.p[3], ops._stream()), "byol_augment_params")
+        check(lib.byol_augment_params_recipe(params.data_ptr(), n, hs, ws, self.seed, self.calls, self.strength,
+                                             ctypes.byref(self._recipe), ops._stream()), "byol_augment_params_recipe")
         self.calls += 1
         return params
 
@@ -66,14 +109,16 @@ class TwoViewAugment(object):
             step = self.calls
             self.calls += 1
         params = torch.empty((2, n, RECORD), dtype=torch.float32, device=device)
-        check(lib.byol_augment_params_ragged(params.data_ptr(), hw.data_ptr(), n, int(n0), total, self.seed, int(step),
-                                             self.strength, self.p[0], self.p[1], self.p[2], self.p[3], ops._stream()),
-              "byol_augment_params_ragged")
+        check(lib.byol_augment_params_ragged_recipe(params.data_ptr(), hw.data_ptr(), n, int(n0), total, self.seed,
+                                                    int(step), self.strength, ctypes.byref(self._recipe),
+                                                    ops._stream()),
+              "byol_augment_params_ragged_recipe")
         return params
 
     def resize_params(self, sizes, device):
-        """Records that take the whole image, with no flip, jitter, grayscale or blur: ``Resize((R, R))``, antialiased,
-        as the reference's test transform (main.py:398), through the same kernels as the training views."""
+        """Records that take the whole image, with no flip, jitter, grayscale, blur or solarize: ``Resize((R, R))``,
+        antialiased bilinear whatever the recipe, as the reference's test transform (main.py:398), through the same
+        kernels as the training views."""
         params = torch.zeros((2, len(sizes), RECORD), dtype=torch.float32)
         params[:, :, 2:4] = torch.tensor([[float(h), float(w)] for h, w in sizes], dtype=torch.float32)
         params[:, :, 6:10] = torch.arange(4, dtype=torch.float32)

@@ -15,8 +15,10 @@ Train: every epoch the whole split is permuted with a generator seeded from ``(s
 ``num_replicas`` takes the ``r``-th of ``num_replicas`` equal contiguous parts of that permutation, and the
 remainder is dropped, so ``len(train_loader) == num_train_samples // num_replicas // batch_size``.  The two views are
 ``TwoViewAugment``'s recipe (RandomResizedCrop of the original image, flip, colour jitter, grayscale, blur) with
-``image_size_override`` and ``color_jitter_strength``; a sample's records are keyed by ``(seed, epoch, batch, its
-position in the global batch, view)``.  Test / valid: neither sharded nor shuffled, the last batch may be short, and
+``image_size_override`` and ``color_jitter_strength``, and ``augmentation`` names the recipe: "reference" (the
+default, also when the key is absent) or "byol", the BYOL paper's (bicubic crops, its colour jitter, per-view blur and
+solarization; see ``byol_b200.augment``).  A sample's records are keyed by ``(seed, epoch, batch, its position in the
+global batch, view)``.  Test / valid: neither sharded nor shuffled, the last batch may be short, and
 both views are the image resized to ``R x R`` (antialiased bilinear, the reference's ``Resize``).
 
 Per batch the file bytes are read by a small host thread pool, one batch ahead of the one being decoded.  Images are
@@ -32,7 +34,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import torch
 
-from .augment import TwoViewAugment
+from .augment import RECIPES, TwoViewAugment
 
 TASK = "multi_augment_image_folder"
 EXTENSIONS = (".jpg", ".jpeg", ".png", ".webp")
@@ -168,7 +170,9 @@ class ImageFolderTwoView(object):
     """The object ``main.py`` gets from ``get_loader``."""
 
     def __init__(self, data_dir, batch_size, image_size=224, color_jitter_strength=1.0, seed=0, rank=0, replicas=1,
-                 workers=2):
+                 workers=2, augmentation="reference"):
+        if augmentation not in RECIPES:
+            raise ValueError("get_loader: unknown augmentation %r (expected one of %s)" % (augmentation, sorted(RECIPES)))
         splits = {}
         for name in ("train", "test", "valid"):
             root = os.path.join(data_dir, name)
@@ -189,8 +193,10 @@ class ImageFolderTwoView(object):
         if self.num_train_samples // replicas < batch_size:
             raise ValueError("get_loader: %d training images cannot fill one batch of %d on each of %d replicas"
                              % (self.num_train_samples, batch_size, replicas))
-        train_aug = TwoViewAugment(image_size=image_size, color_jitter_strength=color_jitter_strength, seed=seed)
-        test_aug = TwoViewAugment(image_size=image_size, seed=seed)
+        self.augmentation = augmentation
+        train_aug = TwoViewAugment(image_size=image_size, color_jitter_strength=color_jitter_strength, seed=seed,
+                                   recipe=augmentation)
+        test_aug = TwoViewAugment(image_size=image_size, seed=seed)      # resize records only: the recipe is unused
         self.train_loader = ImageFolderLoader(splits["train"][1], batch_size, train_aug, True, seed, rank, replicas,
                                               workers)
         self.test_loader = ImageFolderLoader(splits["test"][1], batch_size, test_aug, False, workers=workers)
@@ -205,7 +211,7 @@ class ImageFolderTwoView(object):
 
 def get_loader(**kwargs):
     """``datasets.loader.get_loader`` for ``--task multi_augment_image_folder``; takes ``vars(args)`` plus the
-    transform lists, which are ignored (the recipe is fixed; see the module docstring)."""
+    transform lists, which are ignored (the recipe is named by ``augmentation``; see the module docstring)."""
     task = kwargs.get("task", TASK)
     if "dali" in task:
         raise ValueError("get_loader: DALI tasks are not supported (task %r); use %r" % (task, TASK))
@@ -215,10 +221,12 @@ def get_loader(**kwargs):
     if not data_dir or not os.path.isdir(data_dir):
         raise FileNotFoundError("get_loader: data directory %r does not exist" % (data_dir,))
     seed = kwargs.get("seed")
+    augmentation = kwargs.get("augmentation") or "reference"
     return ImageFolderTwoView(data_dir, int(kwargs.get("batch_size", 4096)),
                               image_size=int(kwargs.get("image_size_override") or 224),
                               color_jitter_strength=float(kwargs.get("color_jitter_strength", 1.0)),
                               seed=0 if seed is None else int(seed),
                               rank=int(kwargs.get("distributed_rank") or 0),
                               replicas=max(1, int(kwargs.get("num_replicas") or 1)),
-                              workers=max(2, int(kwargs.get("workers_per_replica") or 2)))
+                              workers=max(2, int(kwargs.get("workers_per_replica") or 2)),
+                              augmentation=augmentation)

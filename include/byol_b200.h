@@ -252,7 +252,7 @@ int byol_xchg_sum(void* vals, void* local_copy, int n, int is_f64, const uint64_
 /* ---- on-device two-view augmentation (main.py:386-397: RandomResizedCrop, flip, ColorJitter p = 0.8, grayscale
  *      p = 0.2, Gaussian blur p = 0.5) for decoded fp32 NCHW images resident in HBM.  params: fp32 [2, N, 16] records
  *      (view-major; byol_augment_record_floats() floats each: crop top / left / h / w, flip, jitter on, op order x 4,
- *      brightness, contrast, saturation, hue, gray on, blur sigma).  See csrc/augment.cu. ---- */
+ *      brightness, contrast, saturation, hue, flag word (bit 0 gray), blur sigma).  See csrc/augment.cu. ---- */
 int byol_augment_record_floats(void);
 int byol_augment_params(float* params, int N, int Hs, int Ws, uint64_t seed, uint64_t step, float strength,
                         float p_flip, float p_jitter, float p_gray, float p_blur, byol_stream_t stream);
@@ -268,6 +268,23 @@ int byol_augment_params_ragged(float* params /* [2, n, 16] */, const int* hw, in
 int byol_augment_apply_ragged(const uint8_t* const* srcs, const int* hw, const float* params,
                               float* out /* [2, N, 3, R, R] */, float* tmp, int N, int R, int ksize,
                               byol_stream_t stream);
+/* The samplers with the recipe spelled out: the BYOL paper's (Grill et al. 2020, Appendix B) is jitter {0.4, 0.4,
+ * 0.2, 0.1}, p_blur {1.0, 0.1}, p_solarize {0.0, 0.2}, bicubic; the reference's is jitter {0.8, 0.8, 0.8, 0.2},
+ * p_blur {0.5, 0.5}, p_solarize {0, 0}, bilinear, and gives byol_augment_params' records.  Record float 14 is a flag
+ * word: bit 0 grayscale, bit 1 solarize (x >= 0.5 -> 1 - x, after the blur), bit 2 bicubic resampling (clamped to
+ * [0, 1]); the apply entries above run records of either recipe.  A probability outside [0, 1] is rejected. */
+typedef struct {
+  float jitter[4];      /* brightness, contrast, saturation, hue factors; the kernel multiplies them by strength */
+  float p_flip, p_jitter, p_gray;
+  float p_blur[2];      /* view 1, view 2 */
+  float p_solarize[2];  /* view 1, view 2 */
+  int bicubic;          /* 1: antialiased bicubic crop resize, 0: antialiased bilinear */
+} byol_augment_recipe_t;
+int byol_augment_params_recipe(float* params /* [2, N, 16] */, int N, int Hs, int Ws, uint64_t seed, uint64_t step,
+                               float strength, const byol_augment_recipe_t* recipe /* host */, byol_stream_t stream);
+int byol_augment_params_ragged_recipe(float* params /* [2, n, 16] */, const int* hw, int n, int n0, int N,
+                                      uint64_t seed, uint64_t step, float strength,
+                                      const byol_augment_recipe_t* recipe /* host */, byol_stream_t stream);
 
 /* ---- weighted k-NN evaluation of frozen features (csrc/knn.cu; the similarity chunks come from byol_conv_igemm as a
  *      linear layer over bf16 rows).  Entries rank by similarity descending, then bank index ascending (-0 as +0, NaN
