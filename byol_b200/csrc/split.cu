@@ -36,8 +36,14 @@ static inline SplitPattern make_pattern(int T) {
   return p;
 }
 
+// A finite |x| >= 0x7F7F8000 (~3.3962e38) rounds to +-inf in bf16: x0 is then the largest finite bf16 of x's sign
+// instead, so that x - x0 stays exact (Sterbenz) and the planes still sum to x.  Non-finite x keeps its planes
+// (+-inf, NaN, NaN) / (NaN, NaN, NaN): every output such an element reaches is NaN.
 __device__ __forceinline__ void split3(float x, bf16 (&pl)[3]) {
-  pl[0] = __float2bfloat16_rn(x);
+  const uint32_t u = __float_as_uint(x);
+  // |x| in [0x7F7F8000, 0x7F7FFFFF]: truncating to the top 16 bits gives +-0x7F7F
+  pl[0] = (u & 0x7FFFFFFFu) - 0x7F7F8000u < 0x8000u ? __ushort_as_bfloat16((unsigned short)(u >> 16))
+                                                    : __float2bfloat16_rn(x);
   const float r1 = x - __bfloat162float(pl[0]);          // exact (Sterbenz-like: |r1| <= 2^-9 |x|)
   pl[1] = __float2bfloat16_rn(r1);
   const float r2 = r1 - __bfloat162float(pl[1]);         // exact

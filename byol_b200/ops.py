@@ -549,7 +549,8 @@ F64 = torch.float64
 
 
 def split_planes(x2d, T, cpad=None, want_copy=False, copy_out=None):
-    """fp32 [M, C] (unit column stride) -> bf16 planes [M, T*cpad] (+ the plain bf16 rounding [M, C])."""
+    """fp32 [M, C] (unit column stride) -> bf16 planes [M, T*cpad] (+ the plane x0 [M, C]: the bf16 rounding, saturated
+    at the largest finite bf16)."""
     if x2d.dtype != F32 or not x2d.is_cuda or x2d.stride(-1) != 1:
         raise ValueError("split_planes: need a CUDA fp32 matrix with unit column stride")
     m, c = x2d.shape

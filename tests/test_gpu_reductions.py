@@ -252,6 +252,38 @@ def stats_f32_case(dev, exact, g, m, c):
     return run, lambda o: [("stats64", o[0], _colstats(y))]
 
 
+def bn_bwd_reduce_f32_case(dev, exact, g, m, c, mask_mode):
+    """The fp32 path's BatchNorm-backward sums (fp64 partials per row block): dz = g, or g where y*scale + shift > 0
+    (mask_mode 1), or where the mask bits are set (3); s12 += [sum dz, sum dz * (y - mean) * invstd]."""
+    from byol_b200 import ops
+    from tests.util import pack_bits
+    gy, y = _vals((m, c), exact, g, 3) * 0.5, _vals((m, c), exact, g, 3)
+    mean = torch.randint(-2, 3, (c,), generator=g).float()
+    invstd = torch.pow(2.0, torch.randint(-1, 2, (c,), generator=g).float())
+    scale = torch.pow(2.0, torch.randint(-1, 2, (c,), generator=g).float())
+    scale = scale * (torch.randint(0, 2, (c,), generator=g) * 2 - 1)
+    shift = torch.randint(-2, 3, (c,), generator=g).float()
+    keep = None
+    if mask_mode == 1:
+        keep = y * scale + shift > 0
+    elif mask_mode == 3:
+        keep = torch.rand((m, c), generator=g) > 0.4
+    mk = pack_bits(keep).to(dev) if mask_mode == 3 else None
+    coeffs = torch.stack([scale, shift, mean, invstd]).to(dev)
+    gd, yd = gy.to(dev), y.to(dev)
+
+    def run():
+        s12 = torch.zeros(2 * c, dtype=F64, device=dev)
+        ops.bn_bwd_reduce_f32(gd, yd, coeffs, s12, mask_mode, mask=mk)
+        return [s12]
+
+    def ref(o):
+        dz = gy.double() * (keep.double() if keep is not None else 1.0)
+        xhat = (y.double() - mean.double()) * invstd.double()
+        return [("s12", o[0], torch.cat([dz.sum(0), (dz * xhat).sum(0)]))]
+    return run, ref
+
+
 def augment_case(dev, exact, g, n, hs, ws, r):
     from byol_b200.augment import TwoViewAugment
     imgs = torch.rand(n, 3, hs, ws, generator=g).to(dev)
@@ -295,6 +327,12 @@ EXACT = {
     "mlp_fused_24": (mlp_case, dict(b=24, k1=256, h=4096, o=256)),
     "loss_fwd": (loss_case, dict(rows=512, dim=256)),
     "stats_f32": (stats_f32_case, dict(m=1 << 18, c=64)),
+    # the fp32 path's backward sums: C below and above 256 (a second, partial column tile), row counts that leave the
+    # last row block short
+    "bn_bwd_reduce_f32_m0_c96": (bn_bwd_reduce_f32_case, dict(m=3001, c=96, mask_mode=0)),
+    "bn_bwd_reduce_f32_m1_c300": (bn_bwd_reduce_f32_case, dict(m=2999, c=300, mask_mode=1)),
+    "bn_bwd_reduce_f32_m3_c264": (bn_bwd_reduce_f32_case, dict(m=5003, c=264, mask_mode=3)),
+    "bn_bwd_reduce_f32_m3_c64": (bn_bwd_reduce_f32_case, dict(m=REAL_M + 37 * 8, c=64, mask_mode=3)),
 }
 
 # smaller shapes for the run-to-run checks (four launches each, plus a graph capture)

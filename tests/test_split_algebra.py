@@ -1,7 +1,7 @@
 """CPU: the arithmetic behind the fp32-accurate path (csrc/split.cu), restated with torch on the host.
 
-* the 3-way bf16 split is EXACT up to 2^-24 |x| (each residual is representable, so x0 + x1 + x2 loses at most the last
-  fp32 bit);
+* the 3-way bf16 split is EXACT: x0 + x1 + x2 == x for every finite fp32 |x| >= 2^-110 up to FLT_MAX (below, x2 can
+  fall under bf16's subnormal spacing 2^-133), with x0 clamped to the largest finite bf16 where x rounds to inf;
 * the plane patterns of the kernels (activation side A, weight side B) enumerate exactly the product terms
   x0w0, x0w1, x1w0, x1w1, x0w2, x2w0 (T = 6) / x0w0, x0w1, x1w0 (T = 3);
 * a dot product over those terms with fp32 accumulation matches float64 to ~1e-7 (T = 6) / ~1e-5 (T = 3), where
@@ -13,8 +13,13 @@ A6, B6 = (0, 0, 1, 1, 0, 2), (0, 1, 0, 1, 2, 0)
 A3, B3 = (0, 0, 1), (0, 1, 0)
 
 
+BF16_MAX = torch.finfo(torch.bfloat16).max
+
+
 def _planes(x):
+    """split3 (csrc/split.cu): a finite x that rounds to inf in bf16 takes x0 = the largest finite bf16 of its sign."""
     p0 = x.to(torch.bfloat16).float()
+    p0 = torch.where(torch.isinf(p0) & torch.isfinite(x), torch.sign(x) * BF16_MAX, p0)
     r1 = x - p0
     p1 = r1.to(torch.bfloat16).float()
     r2 = r1 - p1
@@ -34,6 +39,45 @@ def test_three_way_split_is_exact():
     assert rel <= 2.0 ** -24, rel
     two = p0.double() + p1.double()
     assert ((two - x.double()).abs() / x.double().abs()).max().item() <= 2.0 ** -16
+
+
+def _bits(v):
+    return torch.tensor(v, dtype=torch.int64).to(torch.int32).view(torch.float32)
+
+
+def test_three_way_split_is_exact_over_the_finite_range():
+    g = torch.Generator().manual_seed(2)
+    n = 1 << 18
+    # every exponent from the fp32 subnormals to FLT_MAX, random mantissas and signs, plus the edges of the bf16
+    # overflow: 0x7F7F8000 is the smallest finite value that rounds to inf
+    bits = torch.randint(0, 0x7F800000, (n,), generator=g, dtype=torch.int64)
+    edges = [0x7F7F7FFF, 0x7F7F8000, 0x7F7F8001, 0x7F7FC000, 0x7F7FFFFF, 0x7F000000, 0x00800000, 0x007FFFFF, 1,
+             0x0A800000, 0x0A800001, 0x0A7FFFFF, 0x0A000001]
+    bits[:len(edges)] = torch.tensor(edges)
+    x = _bits(bits.tolist())
+    x = torch.where(torch.rand(n, generator=g) < 0.5, -x, x)
+    (p0, p1, p2), r1, r2 = _planes(x)
+    for p in (p0, p1, p2):
+        assert bool(torch.isfinite(p).all()), "a finite value split into a non-finite plane"
+    assert torch.equal(p0[1:5].abs(), torch.full((4,), BF16_MAX)), "x0 of values past 0x7F7F8000 is not clamped"
+    assert torch.equal(p0[0], torch.tensor(BF16_MAX).copysign(x[0])), "0x7F7F7FFF rounds down to the largest bf16"
+    # exact for |x| >= 2^-110: the residual r2 is then a multiple of 2^-133, bf16's subnormal spacing
+    exact_from = 2.0 ** -110
+    back = p0.double() + p1.double() + p2.double()
+    big = x.abs() >= exact_from
+    assert torch.equal(back[big], x.double()[big])
+    # below 2^-110 the split loses at most 2^-134 (half of bf16's subnormal spacing), and it does lose bits there:
+    # 2^-111 (1 + 2^-23) = 0x08000001 splits into (2^-111, 0, 0)
+    assert float((back[~big] - x.double()[~big]).abs().max()) <= 2.0 ** -134
+    tiny = _bits([0x08000001])
+    (q0, q1, q2), _, _ = _planes(tiny)
+    assert float(tiny) < exact_from and float(q0 + q1 + q2) == 2.0 ** -111 != float(tiny)
+    # just above: 0x0A000001 = 2^-107 (1 + 2^-23) still splits exactly
+    assert float(x[12].abs()) >= exact_from and float(back[12]) == float(x[12])
+    # non-finite operands: +-inf splits into (+-inf, NaN, NaN), NaN into NaNs, so every product they reach is NaN
+    (i0, i1, i2), _, _ = _planes(torch.tensor([float("inf"), float("-inf"), float("nan")]))
+    assert torch.equal(i0[:2], torch.tensor([float("inf"), float("-inf")])) and bool(torch.isnan(i0[2]))
+    assert bool(torch.isnan(i1).all() and torch.isnan(i2).all())
 
 
 def test_plane_patterns_enumerate_the_product_terms():
