@@ -165,10 +165,7 @@ class Engine(object):
         self._side_stream = None
         self._side_used = False
         self._side_refs = []
-        self.overlap_wgrad = os.environ.get("BYOL_B200_OVERLAP_WGRAD", "1") != "0"
-        self.multi_stream = os.environ.get("BYOL_B200_MULTI_STREAM", "1") != "0"
-        self._fwd_streams = None
-        self._bwd_streams = None
+        self._lane_streams = None
         self._fin_events = None
         self._group_order = 0
         self._bwd_channel = 0
@@ -186,8 +183,6 @@ class Engine(object):
         # weight layouts of representations(): apart from the training step's, so that a call between a captured
         # forward and its backward leaves every buffer the graphs read untouched (allocated on first use)
         self.w_eval = self.s_eval = None
-        # projector / predictor forward as one cooperative kernel per lane (csrc/mlp_fused.cu); =0: four launches
-        self.fused_mlp = os.environ.get("BYOL_B200_FUSED_MLP", "1") != "0"
         self._mlp_bar = None
         # activation recomputation (recompute_plan): per geometry the set of blocks whose online lanes keep only the
         # block input, the BN coefficients and the output mask; _recompute_now is the set of the running forward
@@ -288,11 +283,10 @@ class Engine(object):
         self.bn_modules = [u.bn for u in self.units if u.bn is not None]
         self.bn_channels = sum(u.cout for u in self.units if u.bn is not None)
         self.sync = any(isinstance(b, nn.SyncBatchNorm) for b in self.bn_modules)
-        self._side_stream = torch.cuda.Stream(device=self.device) if self.overlap_wgrad else None
+        self._side_stream = torch.cuda.Stream(device=self.device)
         # the same two streams serve the forward lane pairs and the backward views: every extra stream is an extra
         # caching-allocator pool, and pools do not share their cached blocks
-        self._fwd_streams = [torch.cuda.Stream(device=self.device) for _ in range(2)]
-        self._bwd_streams = self._fwd_streams
+        self._lane_streams = [torch.cuda.Stream(device=self.device) for _ in range(2)]
         self.w_online = _Weights(self.units, self.device, True)
         self.w_target = _Weights(self.units, self.device, False)
         self.graphs = {}           # captured steps point into the old buffers
@@ -362,8 +356,20 @@ class Engine(object):
     def plan_is_current(self):
         return self.ready and self.is_flat() and self.module_key == self._module_key()
 
-    def world(self):
-        return comm.world_size()
+    def _nccl_statistics(self):
+        """True if this model's SyncBatchNorm statistics go over NCCL: then the fused MLP, the two-stream schedule
+        and graph capture are off.  A model without SyncBatchNorm never reaches comm.peer_exchange (collective on
+        its first call, so every rank must reach it at the same point)."""
+        return self.sync and comm.uses_nccl_for_statistics(self.device)
+
+    def _sum_over_ranks(self, stats, rows, channel=0, want_local=False):
+        """SyncBatchNorm: SUM the per-channel statistics `stats` (covering `rows` rows here) in place over the ranks
+        on exchange `channel`.  Returns (the row count the sums cover, this rank's own sums if want_local else None)."""
+        if not (self.sync and comm.world_size() > 1):
+            return rows, None
+        local = torch.empty_like(stats) if want_local else None
+        comm.allreduce_sum_(stats, local_out=local, channel=channel)
+        return rows * comm.world_size(), local
 
     def prep_weights(self, flat, wset, want_dgrad):
         """fp32 master (flat vector) -> bf16 tensor-core layouts of every conv / linear, one launch."""
@@ -472,7 +478,7 @@ class Engine(object):
         cache, read once per geometry: the GPU may be shared).  Only the bf16 path recomputes."""
         if self.T:
             return frozenset()
-        key = (n, h, w, lanes, target, mlps, self.world(), self._mem_budget)
+        key = (n, h, w, lanes, target, mlps, comm.world_size(), self._mem_budget)
         plan = self._plans.get(key)
         if plan is None:
             budget = self._mem_budget
@@ -508,11 +514,7 @@ class Engine(object):
         coeffs = self._cpool.take(L * 4 * C).view(L, 4, C)
         bn = u.bn
         if train:
-            rows = ys[0].numel() // C
-            count = rows
-            if self.sync and self.world() > 1:
-                comm.allreduce_sum_(stats, channel=self._group_order)
-                count = rows * self.world()
+            count, _ = self._sum_over_ranks(stats, ys[0].numel() // C, channel=self._group_order)
             fin = self._fin_events
             if fin is not None and self._group_order == 1:
                 torch.cuda.current_stream().wait_event(fin[u.idx])     # running stats: online pair first
@@ -586,7 +588,7 @@ class Engine(object):
 
     def _mlp_fused_ok(self, mlp, b):
         l1, l2 = mlp
-        if not self.fused_mlp or (self.sync and comm.uses_nccl_for_statistics(self.device)):
+        if self._nccl_statistics():
             return False            # the in-kernel statistics exchange needs the peer-memory channel
         return l1.bn is not None and l1.b_off >= 0 and l2.b_off >= 0 and \
             ops.mlp_fused_supported(b, l1.cin, l1.cout, l2.cout)
@@ -601,8 +603,8 @@ class Engine(object):
         if self._mlp_bar is None:
             self._mlp_bar = torch.zeros((comm.NUM_CHANNELS, 2), dtype=torch.int32, device=self.device)
         peer, world = None, 1
-        if train and self.sync and self.world() > 1:
-            peer, world = comm.peer_exchange(self.device)[ch], self.world()
+        if train and self.sync and comm.world_size() > 1:
+            peer, world = comm.peer_exchange(self.device)[ch], comm.world_size()
         fin = self._fin_events
         if train and fin is not None and ch == 1:
             torch.cuda.current_stream().wait_event(fin[l1.idx])      # running statistics: online pair first
@@ -687,8 +689,8 @@ class Engine(object):
         # under SyncBatchNorm over NCCL the per-layer all-reduces serialise the lane pairs anyway: run all four lanes
         # lock-step on one stream there, which halves the number of (latency-bound) NCCL calls.  The peer-memory
         # exchange (comm.PeerExchange) has one channel per stream, so the two-stream schedule stays.
-        two = self.multi_stream and L == 4 and not (self.sync and comm.uses_nccl_for_statistics(self.device))
-        groups = [(list(range(0, 2)), self._fwd_streams[0]), (list(range(2, 4)), self._fwd_streams[1])] if two \
+        two = L == 4 and not self._nccl_statistics()
+        groups = [(list(range(0, 2)), self._lane_streams[0]), (list(range(2, 4)), self._lane_streams[1])] if two \
             else [(list(range(L)), main)]
         self._fin_events = {} if (two and train) else None
         results = [None] * L
@@ -756,7 +758,7 @@ class Engine(object):
         # ranks: two of them from different streams must never be schedulable in different orders on different ranks
         # (rank X resident with stream A's kernel, rank Y with stream B's -> circular wait).  So the second lane pair
         # enters its MLP section only after the first pair has left it: A-head, A-pred, B-head, B-pred everywhere.
-        gate = train and self.sync and self.world() > 1 and self._fin_events is not None and \
+        gate = train and self.sync and comm.world_size() > 1 and self._fin_events is not None and \
             self._mlp_fused_ok(self.mlps[0], reps_b[0].shape[0])
         if gate and self._group_order == 1:
             torch.cuda.current_stream().wait_event(self._fin_events["mlp_gate"])
@@ -796,11 +798,7 @@ class Engine(object):
         coeffs = torch.empty((L, 4, C), dtype=F32, device=self.device)
         bn = u.bn
         if train:
-            rows = ys[0].numel() // C
-            count = rows
-            if self.sync and self.world() > 1:
-                comm.allreduce_sum_(stats)
-                count = rows * self.world()
+            count, _ = self._sum_over_ranks(stats, ys[0].numel() // C)
             ops.bn_finalize_lanes_f64(stats, count, [flat[u.g_off:u.g_off + C] for flat, _, _ in lanes],
                                       [flat[u.beta_off:u.beta_off + C] for flat, _, _ in lanes], bn.running_mean,
                                       bn.running_var, bn.momentum, bn.eps, coeffs)
@@ -931,12 +929,7 @@ class Engine(object):
         for i in range(L):
             ops.bn_bwd_reduce(gs[i].view(-1, C), ys[i].view(-1, C), cs[i], s12[i * 2 * C:(i + 1) * 2 * C], mask_mode,
                               act=None if acts is None else (acts[i] if mask_mode == 3 else acts[i].view(-1, C)))
-        rows = ys[0].numel() // C
-        count, local = rows, None
-        if self.sync and self.world() > 1:
-            local = torch.empty_like(s12)
-            comm.allreduce_sum_(s12, local_out=local, channel=self._bwd_channel)
-            count = rows * self.world()
+        count, local = self._sum_over_ranks(s12, ys[0].numel() // C, channel=self._bwd_channel, want_local=True)
         gamma = self.theta[u.g_off:u.g_off + C]
         dys, dzs = [], []
         for i in range(L):
@@ -958,15 +951,10 @@ class Engine(object):
         planes: xs / dys are split-operand planes (fp32-accurate backward)."""
         dw = self._gview(u.w_off, u.w_numel).view(u.cout, u.cin // u.groups, u.k, u.k)
         launch = self._launch_wgrad_planes if planes else self._launch_wgrad
-        main = torch.cuda.current_stream()
-        side = self._side_stream
-        if side is None:
-            launch(u, xs, dys, dw, unit_stride)
-            return
         ev = torch.cuda.Event()
-        ev.record(main)
-        side.wait_event(ev)
-        with torch.cuda.stream(side):
+        ev.record(torch.cuda.current_stream())
+        self._side_stream.wait_event(ev)
+        with torch.cuda.stream(self._side_stream):
             launch(u, xs, dys, dw, unit_stride)
         # keep the operands alive until the launching stream has joined the side stream (no record_stream: that would
         # add an allocator event per tensor); after the join, reuse by the owning stream is ordered behind the reads
@@ -991,7 +979,7 @@ class Engine(object):
                 ops.conv_wgrad_planes(xp, dyp, dw, u.k, u.k, u.stride, u.pad, self.T)
 
     def _join_side_stream(self):
-        if self._side_stream is not None and self._side_used:
+        if self._side_used:
             ev = torch.cuda.Event()
             ev.record(self._side_stream)
             torch.cuda.current_stream().wait_event(ev)
@@ -1112,11 +1100,7 @@ class Engine(object):
         for i in range(L):
             ops.bn_bwd_reduce_f32(gs[i].view(-1, C), ys[i].view(-1, C), cs[i], s12[i * 2 * C:(i + 1) * 2 * C],
                                   mask_mode, mask=None if masks is None else masks[i])
-        count, local = ys[0].numel() // C, None
-        if self.sync and self.world() > 1:
-            local = torch.empty_like(s12)
-            comm.allreduce_sum_(s12, local_out=local)
-            count *= self.world()
+        count, local = self._sum_over_ranks(s12, ys[0].numel() // C, want_local=True)
         gamma = self.theta[u.g_off:u.g_off + C]
         # dgamma / dbeta: the lanes' rank-local fp64 sums are added first, so the flat gradient takes ONE fp32 rounding
         # (by the last lane's apply kernel)
@@ -1251,21 +1235,21 @@ class Engine(object):
         if self.bwd32:
             self._backward_group_split(saved, d_reps, d_projs, d_preds)
             return
-        if not (self.multi_stream and L == 2) or (self.sync and comm.uses_nccl_for_statistics(self.device)):
+        if L != 2 or self._nccl_statistics():
             self._bwd_channel = 0
             self._backward_group(saved, d_reps, d_projs, d_preds)
             return
         ev = torch.cuda.Event()
         ev.record(main)
         for i in range(L):
-            stream = self._bwd_streams[i]
+            stream = self._lane_streams[i]
             stream.wait_event(ev)
             with torch.cuda.stream(stream):
                 self._bwd_channel = i      # one exchange channel per view / stream
                 self._backward_group([saved[i]], [d_reps[i]], [d_projs[i]], [d_preds[i]])
         for i in range(L):
             e2 = torch.cuda.Event()
-            e2.record(self._bwd_streams[i])
+            e2.record(self._lane_streams[i])
             main.wait_event(e2)
 
     def _backward_group(self, saved, d_reps, d_projs, d_preds):
@@ -1318,8 +1302,7 @@ class Engine(object):
     # CUDA-graph replay of the training step (forward of the 4 lanes + classifier, backward of the 2 online views)
     # ------------------------------------------------------------------------------------------
     def graph_key(self, a1):
-        return (tuple(a1.shape), self.world(), bool(self.sync), self.theta.data_ptr(), self.multi_stream,
-                self.overlap_wgrad, self.T, self.bwd32, self.fused_mlp,
+        return (tuple(a1.shape), comm.world_size(), bool(self.sync), self.theta.data_ptr(), self.T, self.bwd32,
                 self.recompute_plan(a1.shape[0], a1.shape[2], a1.shape[3]))
 
     def prep_step(self, mean, training):
@@ -1360,7 +1343,7 @@ class Engine(object):
         launches plus a handful of small eager kernels (input layout, loss, EMA, LARS) on the host."""
         if not self.use_graphs:
             return None
-        if self.sync and comm.uses_nccl_for_statistics(self.device):
+        if self._nccl_statistics():
             return None          # per-layer NCCL collectives stay eager; the peer-memory exchange is capturable
         key = self.graph_key(a1)
         st = self.graphs.get(key)
