@@ -15,6 +15,16 @@ grayscale are the reference's.  The views are asymmetric: the first output is al
 Every call draws fresh parameters from a counter-based RNG (seed, call counter, sample, view), so a run is
 reproducible and the two views of a sample are independent.  ``apply(images, params)`` and
 ``apply_ragged(images, params)`` run the pipeline on explicit parameter records (tests/test_gpu_augment.py checks every stage against torchvision on identical parameters).
+
+Test and validation images take no random draw: ``eval_params(sizes, device)`` builds, on the host, the records of
+the object's ``eval_transform`` (``EVAL_TRANSFORMS``), and both views are the same image.  "resize" (the default) is
+the reference's ``Resize((R, R))`` of the whole image (antialiased bilinear, ``resize_params``).  "byol" is the BYOL
+paper's test transform (Grill et al. 2020, Appendix C.1; ``centre_crop_params``): the shorter side resized to
+S = (8R + 3) // 7 (256 at R = 224) by antialiased bicubic (clamped to [0, 1]), then the centre R x R crop, i.e.
+torchvision's ``CenterCrop(R)(Resize(S, BICUBIC)(x))`` on float images, the geometry computed as torchvision computes it
+(``centre_crop_geometry``).  Its records are window records: flag bit 3 says that floats 0-3 are (top, left, Sh, Sw),
+the R x R window at (top, left) of the whole image resized to Sh x Sw, whose border pixels take taps from outside the
+window; without the bit they are a crop box (top, left, h, w) resized to R x R.
 """
 import ctypes
 
@@ -24,8 +34,8 @@ from . import _lib, ops
 from ._lib import lib, check
 
 RECORD = lib.byol_augment_record_floats()
-# record float 14: a flag word
-FLAG_GRAY, FLAG_SOLARIZE, FLAG_BICUBIC = 1, 2, 4
+# record float 14: a flag word (bit 3: floats 0-3 are a window of the resized image, see the module docstring)
+FLAG_GRAY, FLAG_SOLARIZE, FLAG_BICUBIC, FLAG_WINDOW = 1, 2, 4, 8
 
 # name -> colour-jitter factors (brightness, contrast, saturation, hue; times color_jitter_strength), blur and
 # solarize probabilities of (view 1, view 2), bicubic crop resize
@@ -52,15 +62,32 @@ def _per_view(name, v):
     return (p, p)
 
 
+def centre_crop_geometry(h, w, image_size):
+    """(top, left, Sh, Sw) of the "byol" eval transform for an h x w image: torchvision's ``Resize(S)`` with
+    S = (8R + 3) // 7 (the shorter side to S, the longer one to ``int(S * long / short)``), then ``CenterCrop(R)``
+    (offsets ``int(round((size - R) / 2.0))``, Python's round half to even)."""
+    R = int(image_size)
+    S = (8 * R + 3) // 7
+    short, long = (w, h) if w <= h else (h, w)
+    new_short, new_long = S, int(S * long / short)
+    sh, sw = (new_long, new_short) if w <= h else (new_short, new_long)
+    return int(round((sh - R) / 2.0)), int(round((sw - R) / 2.0)), sh, sw
+
+
 class TwoViewAugment(object):
     def __init__(self, image_size=224, color_jitter_strength=1.0, seed=0, p_flip=0.5, p_jitter=0.8, p_gray=0.2,
-                 p_blur=None, blur=True, recipe="reference", p_solarize=None):
+                 p_blur=None, blur=True, recipe="reference", p_solarize=None, eval_transform="resize"):
         """``recipe``: "reference" or "byol" (module docstring).  ``p_blur`` / ``p_solarize``: a probability for both
-        views or a (view 1, view 2) pair; None takes the recipe's."""
+        views or a (view 1, view 2) pair; None takes the recipe's.  ``eval_transform``: what ``eval_params`` builds,
+        "resize" or "byol" (``EVAL_TRANSFORMS``)."""
         if recipe not in RECIPES:
             raise ValueError("TwoViewAugment: unknown recipe %r (expected one of %s)" % (recipe, sorted(RECIPES)))
+        if eval_transform not in EVAL_TRANSFORMS:
+            raise ValueError("TwoViewAugment: unknown eval_transform %r (expected one of %s)"
+                             % (eval_transform, sorted(EVAL_TRANSFORMS)))
         rc = RECIPES[recipe]
         self.recipe = recipe
+        self.eval_transform = eval_transform
         self.R = int(image_size)
         self.strength = float(color_jitter_strength)
         self.seed = int(seed)
@@ -124,6 +151,21 @@ class TwoViewAugment(object):
         params[:, :, 6:10] = torch.arange(4, dtype=torch.float32)
         return params.to(device)
 
+    def centre_crop_params(self, sizes, device):
+        """Window records of the BYOL paper's test transform (Appendix C.1): the shorter side resized to
+        (8R + 3) // 7 with antialiased bicubic resampling (clamped to [0, 1]), then the centre R x R crop
+        (``centre_crop_geometry``); no flip, jitter, grayscale, blur or solarize."""
+        params = torch.zeros((2, len(sizes), RECORD), dtype=torch.float32)
+        params[:, :, 0:4] = torch.tensor([[float(v) for v in centre_crop_geometry(h, w, self.R)] for h, w in sizes],
+                                         dtype=torch.float32).reshape(-1, 4)
+        params[:, :, 6:10] = torch.arange(4, dtype=torch.float32)
+        params[:, :, 14] = float(FLAG_BICUBIC | FLAG_WINDOW)
+        return params.to(device)
+
+    def eval_params(self, sizes, device):
+        """The records of this object's ``eval_transform`` for test / validation images of sizes ``sizes``."""
+        return EVAL_TRANSFORMS[self.eval_transform](self, sizes, device)
+
     def apply_ragged(self, images, params):
         """``images``: a list of CUDA uint8 ``[3, H_i, W_i]`` tensors (values read as v / 255) -> two fp32
         ``[N, 3, R, R]`` views, computed exactly as ``apply`` computes them on ``[u8.float() / 255]``."""
@@ -147,6 +189,13 @@ class TwoViewAugment(object):
             return self.apply_ragged(images, self.sample_params_ragged([tuple(t.shape[1:]) for t in images], device))
         n, _, hs, ws = images.shape
         return self.apply(images, self.sample_params(n, hs, ws, images.device))
+
+
+# name -> the record maker of a test / validation transform (TwoViewAugment.eval_params)
+EVAL_TRANSFORMS = {
+    "resize": TwoViewAugment.resize_params,          # the reference's Resize((R, R)) (main.py:398)
+    "byol": TwoViewAugment.centre_crop_params,       # Resize((8R + 3) // 7, BICUBIC) + CenterCrop(R)
+}
 
 
 def _check_ragged(images):

@@ -8,7 +8,8 @@
 // work.  Two kinds of input: one fp32 NCHW batch in [0, 1] of equal-sized images, or a table of uint8 CHW images of
 // any sizes, as a GPU JPEG decoder returns them (read as v / 255; the arithmetic after that is the same).  Three kinds of kernels:
 //   augment_params_kernel : per (sample, view) the random parameters (Philox counter RNG keyed by seed / step / sample)
-//   augment_gray_mean_kernel + augment_apply_kernel : crop + bilinear or bicubic resize + flip + colour ops in the
+//   augment_gray_mean_kernel + augment_apply_kernel : crop + bilinear or bicubic resize (or resize + window, for the
+//       evaluation transforms' records) + flip + colour ops in the
 //       sampled order (adjust_contrast blends with the MEAN grey level of the image as it stands before that op, hence
 //       the small reduction pass) + grayscale (+ solarize, for the samples the blur does not reach)
 //   augment_blur_kernel   : separable Gaussian with reflect padding, only for the samples that drew it (+ solarize on
@@ -24,9 +25,11 @@ namespace byol {
 static constexpr int AP = 16;   // floats per (sample, view) parameter record
 // record layout: 0 top, 1 left, 2 crop_h, 3 crop_w, 4 flip, 5 jitter_on, 6..9 op order (0 brightness, 1 contrast,
 // 2 saturation, 3 hue), 10 brightness, 11 contrast, 12 saturation, 13 hue, 14 flag word, 15 blur sigma (0 = no blur).
-// Flag word bits: grayscale, solarize, bicubic resampling.  The reference recipe sets only the grayscale bit, so its
-// records hold 0 or 1 there, as before the word had other bits.
-static constexpr int FLAG_GRAY = 1, FLAG_SOLARIZE = 2, FLAG_BICUBIC = 4;
+// Flag word bits: grayscale, solarize, bicubic resampling, window.  The reference recipe sets only the grayscale bit,
+// so its records hold 0 or 1 there, as before the word had other bits.  A window record (bit 3, made on the host for
+// the evaluation transforms) reads floats 0-3 as (top, left, Sh, Sw): the R x R window at (top, left) of the whole
+// image resized to Sh x Sw, i.e. a resize followed by a crop, where a crop record (bit 3 clear) crops, then resizes.
+static constexpr int FLAG_GRAY = 1, FLAG_SOLARIZE = 2, FLAG_BICUBIC = 4, FLAG_WINDOW = 8;
 
 // what the sampler draws from: colour-jitter factors (multiplied by color_jitter_strength, as ColorJitter(0.8s, ...)),
 // the switches' probabilities, per view where the recipe makes the views differ
@@ -192,17 +195,23 @@ __device__ __forceinline__ float tap_w(const AxisTaps& t, int j) {
 __device__ __forceinline__ float load_px(const float* p) { return __ldg(p); }
 __device__ __forceinline__ float load_px(const uint8_t* p) { return (float)__ldg(p) / 255.f; }
 
+// A crop record resizes the box (top, left, h, w) to R x R: output pixel (y, x) has the taps of (y, x) over the box,
+// which is where they stop.  A window record's output pixel (y, x) is pixel (y + top, x + left) of the whole image
+// resized to (Sh, Sw): its taps run over the whole image, also outside the window.  Flip mirrors the output.
 template <typename F, typename T>
-__device__ __forceinline__ void sample_crop(const T* __restrict__ src, int Hs, int Ws, const float* q, int R, int y,
-                                            int x, float& r, float& g, float& b) {
-  const int top = (int)q[0], left = (int)q[1], ch = (int)q[2], cw = (int)q[3];
+__device__ __forceinline__ void sample_crop(const T* __restrict__ src, int Hs, int Ws, const float* q, int flags, int R,
+                                            int y, int x, float& r, float& g, float& b) {
+  const int top = (int)q[0], left = (int)q[1], qh = (int)q[2], qw = (int)q[3];
   const int xx = q[4] != 0.f ? (R - 1 - x) : x;
-  const AxisTaps ty = axis_taps<F>(y, ch, R), tx = axis_taps<F>(xx, cw, R);
+  const bool window = flags & FLAG_WINDOW;
+  const AxisTaps ty = axis_taps<F>(window ? y + top : y, window ? Hs : qh, window ? qh : R),
+                 tx = axis_taps<F>(window ? xx + left : xx, window ? Ws : qw, window ? qw : R);
+  const int y0 = window ? 0 : top, x0 = window ? 0 : left;
   const int64_t plane = (int64_t)Hs * Ws;
   float v[3] = {0.f, 0.f, 0.f};
   for (int jy = 0; jy < ty.n; ++jy) {
     const float wy = tap_w<F>(ty, jy);
-    const T* row = src + (int64_t)(top + ty.lo + jy) * Ws + left + tx.lo;
+    const T* row = src + (int64_t)(y0 + ty.lo + jy) * Ws + x0 + tx.lo;
     float h[3] = {0.f, 0.f, 0.f};
     for (int jx = 0; jx < tx.n; ++jx) {
       const float wx = tap_w<F>(tx, jx);
@@ -215,16 +224,17 @@ __device__ __forceinline__ void sample_crop(const T* __restrict__ src, int Hs, i
   r = v[0]; g = v[1]; b = v[2];
 }
 
-// the record's crop + resize: bicubic values are clamped to [0, 1] before any colour op, as a uint8 / PIL pipeline
-// stores them (colour ops on an overshooting value would leave [0, 1], and solarize would turn it negative)
+// the record's crop + resize (or resize + window): bicubic values are clamped to [0, 1] before any colour op, as a
+// uint8 / PIL pipeline stores them (colour ops on an overshooting value would leave [0, 1], and solarize would turn it
+// negative)
 template <typename T>
 __device__ __forceinline__ void resample(const T* __restrict__ src, int Hs, int Ws, const float* q, int flags, int R,
                                          int y, int x, float& r, float& g, float& b) {
   if (flags & FLAG_BICUBIC) {
-    sample_crop<Cubic>(src, Hs, Ws, q, R, y, x, r, g, b);
+    sample_crop<Cubic>(src, Hs, Ws, q, flags, R, y, x, r, g, b);
     r = clamp01(r); g = clamp01(g); b = clamp01(b);
   } else {
-    sample_crop<Triangle>(src, Hs, Ws, q, R, y, x, r, g, b);
+    sample_crop<Triangle>(src, Hs, Ws, q, flags, R, y, x, r, g, b);
   }
 }
 // torchvision solarize(x, 0.5) on float input
@@ -330,10 +340,12 @@ __global__ void augment_gray_mean_kernel(Src src, const float* __restrict__ para
 }
 
 // out[view][n, c, y, x] (fp32 NCHW): crop / resize / flip, colour jitter, grayscale, and solarize when the blur stage
-// (blur_on) will not blur this sample (augment_blur_kernel solarizes the blurred ones)
+// (blur_on) will not blur this sample (augment_blur_kernel solarizes the blurred ones).  At most 64 registers, so that
+// four 256-thread blocks fit on an SM
 template <typename Src>
-__global__ void augment_apply_kernel(Src src, const float* __restrict__ params, const Fix128* __restrict__ gray_sum,
-                                     float* __restrict__ out, int N, int R, int blur_on) {
+__global__ void __launch_bounds__(256, 4)
+augment_apply_kernel(Src src, const float* __restrict__ params, const Fix128* __restrict__ gray_sum,
+                     float* __restrict__ out, int N, int R, int blur_on) {
   const int sv = blockIdx.y;
   const int n = sv % N;
   const float* q = params + (int64_t)sv * AP;

@@ -18,8 +18,12 @@ remainder is dropped, so ``len(train_loader) == num_train_samples // num_replica
 ``image_size_override`` and ``color_jitter_strength``, and ``augmentation`` names the recipe: "reference" (the
 default, also when the key is absent) or "byol", the BYOL paper's (bicubic crops, its colour jitter, per-view blur and
 solarization; see ``byol_b200.augment``).  A sample's records are keyed by ``(seed, epoch, batch, its position in the
-global batch, view)``.  Test / valid: neither sharded nor shuffled, the last batch may be short, and
-both views are the image resized to ``R x R`` (antialiased bilinear, the reference's ``Resize``).
+global batch, view)``.  Test / valid: neither sharded nor shuffled, the last batch may be short, and both views are
+the same image, transformed by ``eval_transform``: "resize" (the default, also when the key is absent) resizes the whole
+image to ``R x R`` (antialiased bilinear, the reference's ``Resize``); "byol" is the BYOL paper's test transform, the
+shorter side resized to (8R + 3) // 7 (256 at R = 224) by antialiased bicubic and the centre ``R x R`` crop (see
+``byol_b200.augment``).  It is independent of ``augmentation``, and the evaluations (``knn_accuracy``,
+``linear_accuracy``, ``finetune_accuracy``) read their images through it.
 
 Per batch the file bytes are read by a small host thread pool, one batch ahead of the one being decoded.  Images are
 decoded and augmented in sub-batches of ``DECODE_BATCH``, each into its slice of the output before the next is
@@ -34,7 +38,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import torch
 
-from .augment import RECIPES, TwoViewAugment
+from .augment import EVAL_TRANSFORMS, RECIPES, TwoViewAugment
 
 TASK = "multi_augment_image_folder"
 EXTENSIONS = (".jpg", ".jpeg", ".png", ".webp")
@@ -157,7 +161,7 @@ class ImageFolderLoader(object):
                 params = self.augment.sample_params_ragged(sizes, device, n0=self.rank * self.batch_size + s,
                                                            total=self.replicas * self.batch_size, step=step)
             else:
-                params = self.augment.resize_params(sizes, device)
+                params = self.augment.eval_params(sizes, device)
             v1, v2 = self.augment.apply_ragged(images, params)
             out[0, s:s + len(images)].copy_(v1)
             out[1, s:s + len(images)].copy_(v2)
@@ -170,9 +174,12 @@ class ImageFolderTwoView(object):
     """The object ``main.py`` gets from ``get_loader``."""
 
     def __init__(self, data_dir, batch_size, image_size=224, color_jitter_strength=1.0, seed=0, rank=0, replicas=1,
-                 workers=2, augmentation="reference"):
+                 workers=2, augmentation="reference", eval_transform="resize"):
         if augmentation not in RECIPES:
             raise ValueError("get_loader: unknown augmentation %r (expected one of %s)" % (augmentation, sorted(RECIPES)))
+        if eval_transform not in EVAL_TRANSFORMS:
+            raise ValueError("get_loader: unknown eval_transform %r (expected one of %s)"
+                             % (eval_transform, sorted(EVAL_TRANSFORMS)))
         splits = {}
         for name in ("train", "test", "valid"):
             root = os.path.join(data_dir, name)
@@ -193,10 +200,11 @@ class ImageFolderTwoView(object):
         if self.num_train_samples // replicas < batch_size:
             raise ValueError("get_loader: %d training images cannot fill one batch of %d on each of %d replicas"
                              % (self.num_train_samples, batch_size, replicas))
-        self.augmentation = augmentation
+        self.augmentation, self.eval_transform = augmentation, eval_transform
         train_aug = TwoViewAugment(image_size=image_size, color_jitter_strength=color_jitter_strength, seed=seed,
                                    recipe=augmentation)
-        test_aug = TwoViewAugment(image_size=image_size, seed=seed)      # resize records only: the recipe is unused
+        # eval_transform records only: the recipe is unused
+        test_aug = TwoViewAugment(image_size=image_size, seed=seed, eval_transform=eval_transform)
         self.train_loader = ImageFolderLoader(splits["train"][1], batch_size, train_aug, True, seed, rank, replicas,
                                               workers)
         self.test_loader = ImageFolderLoader(splits["test"][1], batch_size, test_aug, False, workers=workers)
@@ -211,7 +219,8 @@ class ImageFolderTwoView(object):
 
 def get_loader(**kwargs):
     """``datasets.loader.get_loader`` for ``--task multi_augment_image_folder``; takes ``vars(args)`` plus the
-    transform lists, which are ignored (the recipe is named by ``augmentation``; see the module docstring)."""
+    transform lists, which are ignored (the training recipe is named by ``augmentation``, the test / validation
+    transform by ``eval_transform``; see the module docstring)."""
     task = kwargs.get("task", TASK)
     if "dali" in task:
         raise ValueError("get_loader: DALI tasks are not supported (task %r); use %r" % (task, TASK))
@@ -222,6 +231,7 @@ def get_loader(**kwargs):
         raise FileNotFoundError("get_loader: data directory %r does not exist" % (data_dir,))
     seed = kwargs.get("seed")
     augmentation = kwargs.get("augmentation") or "reference"
+    eval_transform = kwargs.get("eval_transform") or "resize"
     return ImageFolderTwoView(data_dir, int(kwargs.get("batch_size", 4096)),
                               image_size=int(kwargs.get("image_size_override") or 224),
                               color_jitter_strength=float(kwargs.get("color_jitter_strength", 1.0)),
@@ -229,4 +239,4 @@ def get_loader(**kwargs):
                               rank=int(kwargs.get("distributed_rank") or 0),
                               replicas=max(1, int(kwargs.get("num_replicas") or 1)),
                               workers=max(2, int(kwargs.get("workers_per_replica") or 2)),
-                              augmentation=augmentation)
+                              augmentation=augmentation, eval_transform=eval_transform)

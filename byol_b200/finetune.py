@@ -27,8 +27,10 @@ Protocol (this module's choices):
   paid once per batch.  Nesterov SGD, momentum 0.9, the weight decay on every fine-tuned parameter, the lr decayed to 0
   by a cosine over all steps with no warm-up; BatchNorm in train mode (batch statistics, running statistics updated once
   per step);
-* evaluation: images resized whole to R x R (as k-NN and linear evaluation), features from the copy's
-  ``representations()`` (eval-mode BatchNorm), then its classifier;
+* evaluation: validation and test images through the loader's eval transform (as k-NN and linear evaluation:
+  the whole image resized to R x R by default; ``get_loader(..., eval_transform="byol")`` gives the paper's resize to
+  (8R + 3) // 7 = 256 at R = 224 and centre R x R crop), features from the copy's ``representations()`` (eval-mode
+  BatchNorm), then its classifier;
 * selection: the best validation top-1, ties to the earlier run; a run whose parameters went non-finite is never chosen.
 """
 import math
@@ -283,6 +285,10 @@ def finetune_accuracy(model, loader, label_fraction=None, subset=None, epochs=30
     "runs": [{"lr", "weight_decay", "val_top1", "val_top5", "finite", "test_top1", "test_top5"}, ...]} in lr-major
     order.  Exactly one of `label_fraction` (the paper: 0.01 or 0.1) and `subset` (training-image base names) is
     given.  ValueError when every run diverged.
+
+    Validation and test images come from the loader's eval transform (``loader.test_loader.augment``): the whole
+    image resized to R x R by default; ``get_loader(..., eval_transform="byol")`` gives the paper's protocol, the
+    shorter side resized to 256 (at R = 224) by bicubic and the centre R x R crop.
 
     The copies run precision="bf16" whatever `model`'s precision is.  `model` is not changed (weights, running
     statistics, num_batches_tracked, the EMA and its step, captured CUDA graphs).  Under torch.distributed it runs on

@@ -202,7 +202,7 @@ def knn_classify(bank_feats, bank_labels, query_feats, num_classes, k=20, temper
 
 def _extract(model, samples, batch_size, augment, network):
     """(bf16 normalised features [len(samples), D], int64 labels) of one pass over `samples` in file order, view 1
-    (the whole image resized to R x R)."""
+    (the eval transform of `augment`)."""
     from .data import ImageFolderLoader
     feats, labels = [], []
     for img, _, lab in ImageFolderLoader(samples, batch_size, augment, train=False):
@@ -215,10 +215,13 @@ def knn_accuracy(model, loader, k=20, temperature=0.07, network="online", batch_
     """k-NN top-1 / top-5 accuracy (%) of `model`'s frozen encoder on the test split of `loader` (the
     ``ImageFolderTwoView`` from ``byol_b200.data.get_loader``): {"knn_top1": float, "knn_top5": float}.
 
-    The bank is the whole training split in file order, unsharded, each image resized to R x R as the test split is
-    (not augmented); features come from ``model.representations(images, network)`` and are kept as L2-normalised bf16
-    rows with int64 labels (5.25 GB for ImageNet-1k at D = 2048).  Under torch.distributed it runs on the calling rank
-    alone, with no collective, so every rank that calls it gets the same result."""
+    The bank is the whole training split in file order, unsharded, each image taken through the loader's eval
+    transform as the test split is (``loader.test_loader.augment``; not augmented): the whole image resized to R x R
+    by default, or with ``get_loader(..., eval_transform="byol")`` the paper's protocol, the shorter side resized to
+    256 (at R = 224) by bicubic and the centre R x R crop.  Features come from ``model.representations(images,
+    network)`` and are kept as L2-normalised bf16 rows with int64 labels (5.25 GB for ImageNet-1k at D = 2048).
+    Under torch.distributed it runs on the calling rank alone, with no collective, so every rank that calls it gets the
+    same result."""
     _check_k(k)
     if not (float(temperature) > 0.0 and float(temperature) < float("inf")):
         raise ValueError("temperature must be positive and finite, got %r" % (temperature,))

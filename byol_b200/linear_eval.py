@@ -349,8 +349,8 @@ def train_linear_heads(train_feats, train_labels, val_feats, val_labels, num_cla
 
 
 def _extract(model, samples, batch_size, augment, network):
-    """(bf16 features [len(samples), D], int64 labels) of one pass over `samples` in file order, view 1 (the whole
-    image resized to R x R, as knn._extract)."""
+    """(bf16 features [len(samples), D], int64 labels) of one pass over `samples` in file order, view 1 (the
+    eval transform of `augment`, as knn._extract)."""
     from .data import ImageFolderLoader
     feats, labels = [], []
     for img, _, lab in ImageFolderLoader(samples, batch_size, augment, train=False):
@@ -370,8 +370,11 @@ def linear_accuracy(model, loader, epochs=80, batch_size=1024, lrs=DEFAULT_LRS, 
     max(1, min(10 000, N // 10)) training images (``holdout_split``), which are then not trained on.  The reported
     head is the one with the best validation top-1 (ties: the earlier head) among the heads with finite weights (a
     NaN logit never counts as a hit; ValueError if every head diverged); every head's validation and test accuracy
-    is returned as well.  Validation and test images are resized whole to R x R (as in ``knn_accuracy``; not the
-    paper's resize-256 + centre-crop), and their features come from ``model.representations(images, network)``.
+    is returned as well.  Validation and test images come from the loader's eval transform
+    (``loader.test_loader.augment``, as in ``knn_accuracy``), and their features from
+    ``model.representations(images, network)``.  By default that transform resizes the whole image to R x R; for the
+    paper's protocol, the shorter side resized to 256 (at R = 224) by bicubic and the centre R x R crop, build the
+    loader with ``get_loader(..., eval_transform="byol")``.
 
     augment=False (the default): the training features are extracted once the same way, kept on the device as bf16
     (5.25 GB for ImageNet-1k at D = 2048) and trained on for `epochs` (``train_linear_heads``).
