@@ -128,6 +128,19 @@ _SIGNATURES = {
                          c_void_p],
     "byol_linprobe_sgd": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float, c_int, c_int,
                           c_int, c_int, c_void_p],
+    # transfer linear evaluation, csrc/logreg.cu
+    "byol_logreg_vec_blocks": [c_int, c_int],
+    "byol_logreg_ce": [c_void_p, c_int64, c_void_p, c_int, c_int, c_int, c_int, c_double, c_void_p, c_void_p, c_void_p,
+                       c_void_p, c_void_p, c_void_p],
+    "byol_logreg_grad": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                         c_void_p, c_void_p, c_int, c_void_p],
+    "byol_logreg_dots": [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                         c_int, c_void_p],
+    "byol_logreg_accept": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                           c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
+    "byol_logreg_twoloop": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                            c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    "byol_logreg_trial": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "byol_abi_version": [],
     "byol_device_sm_count": [],
 }

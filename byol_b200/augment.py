@@ -22,7 +22,9 @@ the reference's ``Resize((R, R))`` of the whole image (antialiased bilinear, ``r
 paper's test transform (Grill et al. 2020, Appendix C.1; ``centre_crop_params``): the shorter side resized to
 S = (8R + 3) // 7 (256 at R = 224) by antialiased bicubic (clamped to [0, 1]), then the centre R x R crop, i.e.
 torchvision's ``CenterCrop(R)(Resize(S, BICUBIC)(x))`` on float images, the geometry computed as torchvision computes it
-(``centre_crop_geometry``).  Its records are window records: flag bit 3 says that floats 0-3 are (top, left, Sh, Sw),
+(``centre_crop_geometry``).  "byol_transfer" is the preprocessing of the paper's transfer evaluation (Appendix C.2,
+after Kornblith et al. 2019; ``transfer_crop_params``): the shorter side resized to R itself by the same filter, then
+the centre R x R crop.  Their records are window records: flag bit 3 says that floats 0-3 are (top, left, Sh, Sw),
 the R x R window at (top, left) of the whole image resized to Sh x Sw, whose border pixels take taps from outside the
 window; without the bit they are a crop box (top, left, h, w) resized to R x R.
 """
@@ -62,12 +64,15 @@ def _per_view(name, v):
     return (p, p)
 
 
-def centre_crop_geometry(h, w, image_size):
-    """(top, left, Sh, Sw) of the "byol" eval transform for an h x w image: torchvision's ``Resize(S)`` with
-    S = (8R + 3) // 7 (the shorter side to S, the longer one to ``int(S * long / short)``), then ``CenterCrop(R)``
-    (offsets ``int(round((size - R) / 2.0))``, Python's round half to even)."""
+def centre_crop_geometry(h, w, image_size, resize=None):
+    """(top, left, Sh, Sw) of a centre-crop eval transform for an h x w image: torchvision's ``Resize(S)`` (the shorter
+    side to S, the longer one to ``int(S * long / short)``), then ``CenterCrop(R)`` (offsets
+    ``int(round((size - R) / 2.0))``, Python's round half to even).  ``resize`` is S: by default (8R + 3) // 7, the
+    "byol" transform; R for "byol_transfer"."""
     R = int(image_size)
-    S = (8 * R + 3) // 7
+    S = (8 * R + 3) // 7 if resize is None else int(resize)
+    if S < R:
+        raise ValueError("centre_crop_geometry: the resize target %d is smaller than the crop %d" % (S, R))
     short, long = (w, h) if w <= h else (h, w)
     new_short, new_long = S, int(S * long / short)
     sh, sw = (new_long, new_short) if w <= h else (new_short, new_long)
@@ -79,7 +84,7 @@ class TwoViewAugment(object):
                  p_blur=None, blur=True, recipe="reference", p_solarize=None, eval_transform="resize"):
         """``recipe``: "reference" or "byol" (module docstring).  ``p_blur`` / ``p_solarize``: a probability for both
         views or a (view 1, view 2) pair; None takes the recipe's.  ``eval_transform``: what ``eval_params`` builds,
-        "resize" or "byol" (``EVAL_TRANSFORMS``)."""
+        "resize", "byol" or "byol_transfer" (``EVAL_TRANSFORMS``)."""
         if recipe not in RECIPES:
             raise ValueError("TwoViewAugment: unknown recipe %r (expected one of %s)" % (recipe, sorted(RECIPES)))
         if eval_transform not in EVAL_TRANSFORMS:
@@ -151,16 +156,21 @@ class TwoViewAugment(object):
         params[:, :, 6:10] = torch.arange(4, dtype=torch.float32)
         return params.to(device)
 
-    def centre_crop_params(self, sizes, device):
+    def centre_crop_params(self, sizes, device, resize=None):
         """Window records of the BYOL paper's test transform (Appendix C.1): the shorter side resized to
-        (8R + 3) // 7 with antialiased bicubic resampling (clamped to [0, 1]), then the centre R x R crop
-        (``centre_crop_geometry``); no flip, jitter, grayscale, blur or solarize."""
+        (8R + 3) // 7 (or to ``resize``) with antialiased bicubic resampling (clamped to [0, 1]), then the centre R x R
+        crop (``centre_crop_geometry``); no flip, jitter, grayscale, blur or solarize."""
         params = torch.zeros((2, len(sizes), RECORD), dtype=torch.float32)
-        params[:, :, 0:4] = torch.tensor([[float(v) for v in centre_crop_geometry(h, w, self.R)] for h, w in sizes],
-                                         dtype=torch.float32).reshape(-1, 4)
+        params[:, :, 0:4] = torch.tensor([[float(v) for v in centre_crop_geometry(h, w, self.R, resize)]
+                                          for h, w in sizes], dtype=torch.float32).reshape(-1, 4)
         params[:, :, 6:10] = torch.arange(4, dtype=torch.float32)
         params[:, :, 14] = float(FLAG_BICUBIC | FLAG_WINDOW)
         return params.to(device)
+
+    def transfer_crop_params(self, sizes, device):
+        """Window records of the paper's transfer-evaluation preprocessing (Appendix C.2): the shorter side resized to
+        R by antialiased bicubic, then the centre R x R crop."""
+        return self.centre_crop_params(sizes, device, resize=self.R)
 
     def eval_params(self, sizes, device):
         """The records of this object's ``eval_transform`` for test / validation images of sizes ``sizes``."""
@@ -195,6 +205,7 @@ class TwoViewAugment(object):
 EVAL_TRANSFORMS = {
     "resize": TwoViewAugment.resize_params,          # the reference's Resize((R, R)) (main.py:398)
     "byol": TwoViewAugment.centre_crop_params,       # Resize((8R + 3) // 7, BICUBIC) + CenterCrop(R)
+    "byol_transfer": TwoViewAugment.transfer_crop_params,   # Resize(R, BICUBIC) + CenterCrop(R)
 }
 
 

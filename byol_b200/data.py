@@ -22,8 +22,9 @@ global batch, view)``.  Test / valid: neither sharded nor shuffled, the last bat
 the same image, transformed by ``eval_transform``: "resize" (the default, also when the key is absent) resizes the whole
 image to ``R x R`` (antialiased bilinear, the reference's ``Resize``); "byol" is the BYOL paper's test transform, the
 shorter side resized to (8R + 3) // 7 (256 at R = 224) by antialiased bicubic and the centre ``R x R`` crop (see
-``byol_b200.augment``).  It is independent of ``augmentation``, and the evaluations (``knn_accuracy``,
-``linear_accuracy``, ``finetune_accuracy``) read their images through it.
+``byol_b200.augment``); "byol_transfer" is the paper's transfer-evaluation preprocessing, the shorter side resized to
+R by antialiased bicubic and the centre ``R x R`` crop.  It is independent of ``augmentation``, and the evaluations
+(``knn_accuracy``, ``linear_accuracy``, ``finetune_accuracy``, ``transfer_accuracy``) read their images through it.
 
 Per batch the file bytes are read by a small host thread pool, one batch ahead of the one being decoded.  Images are
 decoded and augmented in sub-batches of ``DECODE_BATCH``, each into its slice of the output before the next is

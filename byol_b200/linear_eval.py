@@ -348,13 +348,14 @@ def train_linear_heads(train_feats, train_labels, val_feats, val_labels, num_cla
         return heads, select_heads(heads, val_feats, val_labels)
 
 
-def _extract(model, samples, batch_size, augment, network):
+def _extract(model, samples, batch_size, augment, network, fp32=False):
     """(bf16 features [len(samples), D], int64 labels) of one pass over `samples` in file order, view 1 (the
-    eval transform of `augment`, as knn._extract)."""
+    eval transform of `augment`, as knn._extract); fp32=True keeps the fp32 representations."""
     from .data import ImageFolderLoader
     feats, labels = [], []
     for img, _, lab in ImageFolderLoader(samples, batch_size, augment, train=False):
-        feats.append(ops.cast_bf16(model.representations(img, network)))
+        rep = model.representations(img, network)
+        feats.append(rep if fp32 else ops.cast_bf16(rep))
         labels.append(lab)
     return torch.cat(feats), torch.cat(labels)
 

@@ -324,6 +324,46 @@ int byol_linprobe_sgd(float* params, float* grads, float* momentum_buf, void* we
                       const float* wd, float lr_scale, float momentum, int H, int C, int Cp, int D,
                       byol_stream_t stream);
 
+/* ---- transfer linear evaluation (csrc/logreg.cu): H L2-regularised multinomial logistic regressions fitted together
+ *      by full-batch L-BFGS.  Parameters: one fp32 buffer of [H * Cp, D] weights followed by [H, Cp] biases (the layout
+ *      of the linear-evaluation heads); head h's vector is its Cp weight rows and its Cp biases.  Fixed-point
+ *      accumulators (loss_acc [H], bias_acc [H * Cp]) are 24-byte records, zeroed by the caller.  mode: int32 [H] per-head
+ *      state (0 stopped, 1 line search, 2 accept + new direction, 3 starting point, 4 accept + stop); a vector kernel acts
+ *      on the heads whose mode bit is set in mask.  part: fp64 scratch of at least 8 * H * byol_logreg_vec_blocks(Cp, D)
+ *      entries.  Every reduction has a fixed order that depends on Cp and D only. ---- */
+/* blocks per head of the vector kernels (slices of 16384 elements of a head's Cp * D + Cp parameters) */
+int byol_logreg_vec_blocks(int Cp, int D);
+/* logits fp32 [B, >= H * Cp] (pitch ld, 16-byte aligned), labels int64 [B].  Fit: planes bf16 [B, 6 * H * Cp] = the
+ * six activation-pattern split planes of (softmax - onehot) / n_total (0 in padding columns and rows whose label is
+ * outside [0, C)); loss_acc += the per-head row losses; bias_acc += the column sums of the same fp32 gradient.
+ * Evaluation: class_hits int64 [H, Cp] += top-1 hits per label (a NaN label logit is a miss); class_count int64 [Cp]
+ * += the rows per label. */
+int byol_logreg_ce(const float* logits, int64_t ld, const int64_t* labels, int B, int H, int C, int Cp,
+                   double n_total, void* planes, void* loss_acc, void* bias_acc, long long* class_hits,
+                   long long* class_count, byol_stream_t stream);
+/* gt (weights: the data term's gradient at xt) += l2[h] * W; gt biases = bias_acc; out[h * ldo + 0..2] = (loss sum,
+ * max |gt|, ||W||^2) in fp64 */
+int byol_logreg_grad(const float* xt, float* gt, const void* loss_acc, const void* bias_acc, const double* l2,
+                     const int* mode, int mask, int H, int C, int Cp, int D, double* part, double* out, int ldo,
+                     byol_stream_t stream);
+/* out[h * ldo + k] = fp64 dot product of head h's parts of u[k] and v[k], k < K <= 8 (host arrays of device pointers) */
+int byol_logreg_dots(const void* const* u, const void* const* v, int K, const int* mode, int mask, int H, int C, int Cp,
+                     int D, double* part, double* out, int ldo, byol_stream_t stream);
+/* modes 2 / 4: s = xt - x and y = gt - g into the free history slot, x = xt, g = gt; mode 3: x = xt, g = gt.  Mode 2
+ * keeps the pair when s.y > 1e-10 y.y (rho = 1 / s.y, gamma = s.y / y.y; hist int32 [H, 2] = (oldest slot, count) of
+ * a ring of m + 1 slots in S, Y [m + 1, buffer]). */
+int byol_logreg_accept(float* x, const float* xt, float* g, const float* gt, float* S, float* Y, int* hist,
+                       double* rho, double* gamma, const int* mode, int m, int H, int C, int Cp, int D, double* part,
+                       byol_stream_t stream);
+/* d = -H g by the two-loop recursion over the stored pairs (scaled by gamma; -g / ||g||_2 without pairs); alpha fp64
+ * [H, m + 1] scratch */
+int byol_logreg_twoloop(const float* g, float* d, const float* S, const float* Y, const int* hist, const double* rho,
+                        const double* gamma, double* alpha, double* part, const int* mode, int mask, int m, int H,
+                        int C, int Cp, int D, byol_stream_t stream);
+/* xt = x + fp32(t[h]) * d */
+int byol_logreg_trial(const float* x, const float* d, float* xt, const double* t, const int* mode, int mask, int H,
+                      int C, int Cp, int D, byol_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
