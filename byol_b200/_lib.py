@@ -141,6 +141,18 @@ _SIGNATURES = {
     "byol_logreg_twoloop": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                             c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "byol_logreg_trial": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
+    # GroupNorm and weight standardisation, csrc/groupnorm.cu
+    "byol_ws_fwd": [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p],
+    "byol_ws_bwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p],
+    "byol_gn_stats": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p],
+    "byol_gn_apply": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                      c_void_p, c_int, c_int, c_int, c_int, c_void_p],
+    "byol_gn_relu_maxpool_fwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                 c_int, c_int, c_int, c_int, c_void_p],
+    "byol_gn_bwd_reduce": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                           c_int, c_int, c_int, c_int, c_void_p],
+    "byol_gn_bwd_apply": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                          c_int, c_int, c_int, c_int, c_void_p],
     "byol_abi_version": [],
     "byol_device_sm_count": [],
 }

@@ -17,6 +17,7 @@ Reference semantics reproduced (file:line are /root/reference):
 Data layout: activations NHWC bf16; conv outputs are stored raw ("y") and normalised copies ("a") are
 materialised by a fused BN-apply(+residual)+ReLU kernel; BN statistics come from the conv epilogue.
 """
+import collections
 import gc
 import os
 
@@ -28,11 +29,15 @@ from . import comm, ops
 BF16 = torch.bfloat16
 F32 = torch.float32
 
+# GroupNorm "coefficients" of one lane: the layer's gamma / beta (views of the lane's parameter vector) and the conv
+# output's per-(image, group) fp32 (mean, rstd) [N, 32, 2].  BatchNorm layers carry a [4, C] tensor instead.
+_GN = collections.namedtuple("_GN", "gamma beta stats")
+
 
 class _Unit(object):
     """One conv/linear (+ optional BN) layer: static geometry plus offsets into the flat parameter vector."""
     __slots__ = ("idx", "kind", "cin", "cout", "cpad", "k", "stride", "pad", "w_off", "w_numel", "b_off", "bn",
-                 "g_off", "beta_off", "name", "want_dgrad", "fold", "kcols", "groups")
+                 "g_off", "beta_off", "name", "want_dgrad", "fold", "kcols", "groups", "gn", "ws", "ws_off")
 
 
 class _Block(object):
@@ -42,7 +47,14 @@ class _Block(object):
 class _Weights(object):
     """bf16 tensor-core layouts of one weight set (online or target)."""
 
-    def __init__(self, units, device, want_dgrad):
+    def __init__(self, units, device, want_dgrad, ws=None):
+        # ws = (numel, rows) of the standardised conv weights (weight-standardised nets): this set's standardised fp32
+        # weights, their per-row (mean, rstd) and, with want_dgrad, the gradient the wgrad kernels write for them
+        self.ws_w = self.ws_stats = self.ws_grad = None
+        if ws is not None:
+            self.ws_w = torch.empty(ws[0], dtype=F32, device=device)
+            self.ws_stats = torch.empty((ws[1], 2), dtype=F32, device=device)
+            self.ws_grad = torch.zeros(ws[0], dtype=F32, device=device) if want_dgrad else None
         # grouped units (ResNeXt conv2) keep block-diagonal tiles [C/64, 64, 9*64] in both layouts
         nf = sum(u.cout * u.kcols for u in units)
         self.pool_f = torch.empty(nf, dtype=BF16, device=device)
@@ -80,24 +92,36 @@ class _Weights(object):
         self.grouped_max_c = max([u.cout for u in grouped] or [0])
         self.gdesc_with_dgrad = self.gdesc_fprop_only = None
         if grouped:
-            rows = [[u.w_off, self.off_f[u.idx], -1, u.cout, u.cin // u.groups] for u in grouped]
+            assert ws is None or all(u.ws for u in grouped)
+            rows = [[u.ws_off if u.ws else u.w_off, self.off_f[u.idx], -1, u.cout, u.cin // u.groups]
+                    for u in grouped]
             self.gdesc_fprop_only = torch.tensor(rows, dtype=torch.int64, device=device)
             for r, u in zip(rows, grouped):
                 r[2] = self.off_d[u.idx]
             self.gdesc_with_dgrad = torch.tensor(rows, dtype=torch.int64, device=device)
-        # descriptor tables for the one-launch weight conversion (with and without the dgrad layouts)
-        rows_d, rows_n = [], []
+        # descriptor tables for the one-launch weight conversion (with and without the dgrad layouts); the
+        # standardised weights have tables of their own (source: ws_w instead of the parameter vector)
+        tables = {False: ([], []), True: ([], [])}
         for u in units:
             if u.groups > 1:
                 continue
+            rows_d, rows_n = tables[bool(u.ws)]
             fold = (u.k * 16 + u.k) if u.fold else 0
-            base = [u.w_off, self.off_f[u.idx], -1, u.cout, u.cin, u.cpad, u.k * u.k, fold]
+            base = [u.ws_off if u.ws else u.w_off, self.off_f[u.idx], -1, u.cout, u.cin, u.cpad, u.k * u.k, fold]
             rows_n.append(list(base))
             base[2] = self.off_d[u.idx] if (u.want_dgrad and not u.fold) else -1
             rows_d.append(base)
-        self.desc_with_dgrad = torch.tensor(rows_d, dtype=torch.int64, device=device)
-        self.desc_fprop_only = torch.tensor(rows_n, dtype=torch.int64, device=device)
+        self.desc_with_dgrad = self.desc_fprop_only = self.ws_desc_with_dgrad = self.ws_desc_fprop_only = None
+        rows_d, rows_n = tables[False]
+        if rows_n:
+            self.desc_with_dgrad = torch.tensor(rows_d, dtype=torch.int64, device=device)
+            self.desc_fprop_only = torch.tensor(rows_n, dtype=torch.int64, device=device)
         self.prep_blocks = ops.prep_blocks(rows_n)      # same shapes in both tables
+        rows_d, rows_n = tables[True]
+        if rows_n:
+            self.ws_desc_with_dgrad = torch.tensor(rows_d, dtype=torch.int64, device=device)
+            self.ws_desc_fprop_only = torch.tensor(rows_n, dtype=torch.int64, device=device)
+        self.ws_prep_blocks = ops.prep_blocks(rows_n)
         # dedicated stem kernel layout ([7][4][64][8]) when the first conv is the torchvision 7x7/2 stem
         st = units[0]
         self.stem4_ok = (st.kind == "conv" and st.k == 7 and st.stride == 2 and st.pad == 3 and st.cin <= 4 and
@@ -270,7 +294,14 @@ class Engine(object):
         u.w_off = self.offsets[id(mod.weight)]
         u.w_numel = mod.weight.numel()
         u.bn = bn
-        if bn is not None:
+        u.gn = None
+        u.ws = getattr(mod, "standardized", False)     # WSConv2d (model.py): weight-standardised conv
+        u.ws_off = -1
+        if isinstance(bn, nn.GroupNorm):
+            assert bn.affine and bn.num_groups == ops.GN_GROUPS, "unsupported GroupNorm: %s" % name
+            u.bn, u.gn = None, bn
+            u.g_off, u.beta_off = self.offsets[id(bn.weight)], self.offsets[id(bn.bias)]
+        elif bn is not None:
             assert bn.affine and bn.track_running_stats and bn.momentum is not None, "unsupported BN: %s" % name
             u.g_off, u.beta_off = self.offsets[id(bn.weight)], self.offsets[id(bn.bias)]
         u.want_dgrad = u.cout % 8 == 0 and u.cin % 8 == 0
@@ -283,12 +314,20 @@ class Engine(object):
         self.bn_modules = [u.bn for u in self.units if u.bn is not None]
         self.bn_channels = sum(u.cout for u in self.units if u.bn is not None)
         self.sync = any(isinstance(b, nn.SyncBatchNorm) for b in self.bn_modules)
+        self.group_norm = any(u.gn is not None for u in self.units)
+        if self.T and (self.group_norm or self.ws_rows):
+            raise ValueError("byol_b200: GroupNorm / weight-standardised layers run with bf16 operands only")
+        ws = (self.ws_numel, self.ws_rows) if self.ws_rows else None
+        self.ws_desc = None
+        if ws is not None:
+            self.ws_desc = torch.tensor([[u.w_off, u.ws_off, u.cout, u.w_numel // u.cout, r] for u, r in
+                                         self._ws_units], dtype=torch.int64, device=self.device)
         self._side_stream = torch.cuda.Stream(device=self.device)
         # the same two streams serve the forward lane pairs and the backward views: every extra stream is an extra
         # caching-allocator pool, and pools do not share their cached blocks
         self._lane_streams = [torch.cuda.Stream(device=self.device) for _ in range(2)]
-        self.w_online = _Weights(self.units, self.device, True)
-        self.w_target = _Weights(self.units, self.device, False)
+        self.w_online = _Weights(self.units, self.device, True, ws)
+        self.w_target = _Weights(self.units, self.device, False, ws)
         self.graphs = {}           # captured steps point into the old buffers
         self._plans = {}
         self.s_online = self.s_target = None
@@ -310,7 +349,7 @@ class Engine(object):
         self.units, self.blocks = [], []
         children = list(model.base_network.children())
         convs = [c for c in children if isinstance(c, nn.Conv2d)]
-        bns = [c for c in children if isinstance(c, nn.modules.batchnorm._BatchNorm)]
+        bns = [c for c in children if isinstance(c, (nn.modules.batchnorm._BatchNorm, nn.GroupNorm))]
         pools = [c for c in children if isinstance(c, nn.MaxPool2d)]
         assert len(convs) == 1 and len(bns) == 1 and len(pools) == 1, "unexpected ResNet stem"
         self.stem = self._unit(convs[0], bns[0], "stem")
@@ -337,6 +376,14 @@ class Engine(object):
             self.mlps.append((self._unit(l1, bn, "l1"), self._unit(l2, None, "l2")))
         self.cls = self._unit(model.linear_classifier, None, "classifier")
         self.cls.want_dgrad = False
+        # weight-standardised convs: offsets of their standardised weights (and gradients) and their first row
+        self._ws_units, self.ws_numel, self.ws_rows = [], 0, 0
+        for u in self.units:
+            if u.ws:
+                u.ws_off = self.ws_numel
+                self._ws_units.append((u, self.ws_rows))
+                self.ws_numel += u.w_numel
+                self.ws_rows += u.cout
         # Tensor-core layouts: bf16 activations are moved by TMA (16-byte row pitch), so every layer width on the
         # path must be a multiple of 8 — except the 3-channel image (padded on conversion) and the classifier's
         # class count (fp32 logits, pitched gradient), so that any dataset's label space works (main.py:208).
@@ -372,16 +419,27 @@ class Engine(object):
         return rows * comm.world_size(), local
 
     def prep_weights(self, flat, wset, want_dgrad):
-        """fp32 master (flat vector) -> bf16 tensor-core layouts of every conv / linear, one launch."""
+        """fp32 master (flat vector) -> bf16 tensor-core layouts of every conv / linear, one launch.  A
+        weight-standardised net first standardises its conv weights (ws_fwd, one launch) and converts those."""
         with_d = want_dgrad and wset.pool_d is not None
+        src = flat
+        if wset.ws_w is not None:
+            ops.ws_fwd(flat, self.ws_desc, self.ws_rows, wset.ws_w, wset.ws_stats)
+            src = wset.ws_w
+            if wset.ws_desc_fprop_only is not None:
+                ops.prep_weights_multi(src, wset.pool_f, wset.pool_d,
+                                       wset.ws_desc_with_dgrad if with_d else wset.ws_desc_fprop_only,
+                                       wset.ws_prep_blocks)
         desc = wset.desc_with_dgrad if with_d else wset.desc_fprop_only
-        ops.prep_weights_multi(flat, wset.pool_f, wset.pool_d, desc, wset.prep_blocks)
+        if desc is not None:
+            ops.prep_weights_multi(flat, wset.pool_f, wset.pool_d, desc, wset.prep_blocks)
         if wset.grouped_max_c:
-            ops.prep_weights_grouped(flat, wset.pool_f, wset.pool_d,
+            ops.prep_weights_grouped(src, wset.pool_f, wset.pool_d,
                                      wset.gdesc_with_dgrad if with_d else wset.gdesc_fprop_only, wset.grouped_max_c)
         if wset.stem4_ok:
             st = self.stem
-            ops.prep_weight_stem4(flat[st.w_off:st.w_off + st.w_numel].view(st.cout, st.cin, st.k, st.k),
+            off = st.ws_off if st.ws else st.w_off
+            ops.prep_weight_stem4((src if st.ws else flat)[off:off + st.w_numel].view(st.cout, st.cin, st.k, st.k),
                                   out=wset.w_stem4)
 
     # ------------------------------------------------------------------------------------------
@@ -495,8 +553,24 @@ class Engine(object):
     def _down_as_gemm(u, h, w):
         return u.k == 1 and u.stride == 2 and u.pad == 0 and h % 2 == 0 and w % 2 == 0
 
+    def _conv_gn(self, u, xs, lanes, stem4=None, unit_stride=None):
+        """raw conv outputs + GroupNorm coefficients (_GN) per lane.  The statistics are per image: train and eval
+        compute the same thing, and nothing is exchanged between ranks."""
+        C = u.cout
+        ys, cs = [], []
+        for i, (flat, wset, _) in enumerate(lanes):
+            if stem4 is not None:
+                y = ops.stem_conv_fprop(stem4[0][i], wset.w_stem4, stem4[1][i][0], stem4[1][i][1])
+            else:
+                y = self._conv(u, xs[i], wset, unit_stride)
+            ys.append(y)
+            cs.append(_GN(flat[u.g_off:u.g_off + C], flat[u.beta_off:u.beta_off + C], ops.gn_stats(y, u.gn.eps)))
+        return ys, cs
+
     def _conv_bn(self, u, xs, lanes, train, stem4=None, unit_stride=None):
         """raw conv/linear outputs + BN coefficients [scale, shift, mean, invstd] per lane."""
+        if u.gn is not None:
+            return self._conv_gn(u, xs, lanes, stem4, unit_stride)
         L, C = len(lanes), u.cout
         stats = self._zpool.take(L * 2 * C) if train else None
         ys = []
@@ -538,6 +612,8 @@ class Engine(object):
 
     @staticmethod
     def _apply(y, c, relu, resid=None, rc=None, mask=None):
+        if isinstance(c, _GN):
+            return ops.gn_apply(y, c.gamma, c.beta, c.stats, relu, resid=resid, rgn=rc, mask_out=mask)
         C = y.shape[-1]
         out = torch.empty_like(y)
         ops.bn_apply(y.view(-1, C), c[0], c[1], relu, resid=None if resid is None else resid.view(-1, C),
@@ -686,6 +762,11 @@ class Engine(object):
             # the lanes that save nothing are the target pair
             self._recompute_now = self.recompute_plan(img.shape[0], x8[0][2], x8[0][3], saving, L > saving,
                                                       not reps_only)
+            if self._recompute_now and self.group_norm:
+                self._recompute_now = frozenset()
+                raise RuntimeError("byol_b200: a GroupNorm net at %d images per view and %dx%d does not fit in device "
+                                   "memory with stored activations, and GroupNorm nets do not recompute activations: "
+                                   "use a smaller batch size" % (img.shape[0], x8[0][2], x8[0][3]))
         # under SyncBatchNorm over NCCL the per-layer all-reduces serialise the lane pairs anyway: run all four lanes
         # lock-step on one stream there, which halves the number of (latency-bound) NCCL calls.  The peer-memory
         # exchange (comm.PeerExchange) has one channel per stream, so the two-stream schedule stays.
@@ -731,8 +812,12 @@ class Engine(object):
         xs = []
         for i, (_, _, saved) in enumerate(lanes):
             # stem: BN-apply + ReLU + max-pool fused (the normalised 112x112 map is never written)
-            p, idx = ops.bn_relu_maxpool_fwd(y0[i], c0[i][0], c0[i][1], self.pool_k, self.pool_s, self.pool_p,
-                                             want_idx=saved is not None)
+            if st.gn is not None:
+                p, idx = ops.gn_relu_maxpool_fwd(y0[i], *c0[i], k=self.pool_k, s=self.pool_s, p=self.pool_p,
+                                                 want_idx=saved is not None)
+            else:
+                p, idx = ops.bn_relu_maxpool_fwd(y0[i], c0[i][0], c0[i][1], self.pool_k, self.pool_s, self.pool_p,
+                                                 want_idx=saved is not None)
             xs.append(p)
             if saved is not None:
                 saved.update({"x8": x8[i] if xs4[i] is None else (xs4[i], hw[i][0], hw[i][1]),
@@ -923,7 +1008,22 @@ class Engine(object):
     # ------------------------------------------------------------------------------------------
     # backward building blocks (online lanes only)
     # ------------------------------------------------------------------------------------------
+    def _gn_bwd(self, u, gs, ys, cs, mask_mode, acts=None, want_dz=False):
+        C = u.cout
+        dys, dzs = [], []
+        for i, c in enumerate(cs):
+            act = None if acts is None else acts[i]
+            s12 = torch.zeros((ys[i].shape[0], ops.GN_GROUPS, 2), dtype=F32, device=self.device)
+            ops.gn_bwd_reduce(gs[i], ys[i], c.gamma, c.beta, c.stats, s12, mask_mode, act=act,
+                              dgamma=self._gview(u.g_off, C), dbeta=self._gview(u.beta_off, C))
+            dz = torch.empty_like(ys[i]) if want_dz else None
+            dys.append(ops.gn_bwd_apply(gs[i], ys[i], c.gamma, c.beta, c.stats, s12, mask_mode, act=act, dz_out=dz))
+            dzs.append(dz)
+        return dys, dzs
+
     def _bn_bwd(self, u, gs, ys, cs, mask_mode, acts=None, want_dz=False):
+        if u.gn is not None:
+            return self._gn_bwd(u, gs, ys, cs, mask_mode, acts, want_dz)
         L, C = len(gs), u.cout
         s12 = self._bpool.take(L * 2 * C)
         for i in range(L):
@@ -949,7 +1049,10 @@ class Engine(object):
         """dW += dY^T * im2col(X) on the side stream: the weight-gradient GEMMs only feed the flat gradient buffer, so
         they overlap with the HBM-bound BatchNorm-backward kernels of the next layer on the main stream.
         planes: xs / dys are split-operand planes (fp32-accurate backward)."""
-        dw = self._gview(u.w_off, u.w_numel).view(u.cout, u.cin // u.groups, u.k, u.k)
+        if u.ws:      # the gradient of the standardised weight; ws_bwd maps it to the parameter's
+            dw = self.w_online.ws_grad[u.ws_off:u.ws_off + u.w_numel].view(u.cout, u.cin // u.groups, u.k, u.k)
+        else:
+            dw = self._gview(u.w_off, u.w_numel).view(u.cout, u.cin // u.groups, u.k, u.k)
         launch = self._launch_wgrad_planes if planes else self._launch_wgrad
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream())
@@ -1231,14 +1334,25 @@ class Engine(object):
         if notify:
             self.notify_backward()
         L = len(saved)
-        main = torch.cuda.current_stream()
         if self.bwd32:
             self._backward_group_split(saved, d_reps, d_projs, d_preds)
             return
+        ws = self.w_online.ws_grad
+        if ws is not None:
+            ws.zero_()
         if L != 2 or self._nccl_statistics():
             self._bwd_channel = 0
             self._backward_group(saved, d_reps, d_projs, d_preds)
-            return
+        else:
+            self._backward_views(saved, d_reps, d_projs, d_preds)
+        if ws is not None:
+            # after both views and their weight gradients: the parameter gradient of every standardised conv weight
+            w = self.w_online
+            ops.ws_bwd(ws, w.ws_w, w.ws_stats, self.ws_desc, self.ws_rows, self.grad)
+
+    def _backward_views(self, saved, d_reps, d_projs, d_preds):
+        L = len(saved)
+        main = torch.cuda.current_stream()
         ev = torch.cuda.Event()
         ev.record(main)
         for i in range(L):
@@ -1328,7 +1442,7 @@ class Engine(object):
             wset = self.s_eval
         else:
             if self.w_eval is None:
-                self.w_eval = _Weights(enc, self.device, False)
+                self.w_eval = _Weights(enc, self.device, False, (self.ws_numel, self.ws_rows) if self.ws_rows else None)
             self.prep_weights(flat, self.w_eval, want_dgrad=False)
             wset = self.w_eval
         res, _ = self.forward_lanes([images], [(flat, wset, None)], False, reps_only=True)

@@ -139,7 +139,7 @@ class FineTune(object):
         self.lr, self.weight_decay, self.momentum = lr, weight_decay, float(momentum)
         with torch.random.fork_rng(devices=[]):           # the copy's (discarded) initialisation draws from torch's RNG
             copy = BYOL(d, model.head[-1].out_features, num_classes, 1, arch=model.arch,
-                        head_latent_size=model.head[0].out_features)
+                        head_latent_size=model.head[0].out_features, norm=model.norm)
         self.model = copy.to(dev).train()
         eng = self.eng = copy._engine
         eng.flatten()

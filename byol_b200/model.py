@@ -10,6 +10,7 @@ reference; none of the torch modules' ``forward`` methods is ever called.
 import numpy as np
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 import torchvision.models as models
 
 from . import ops
@@ -48,20 +49,62 @@ class CosEMA(nn.Module):
         return x
 
 
-def _resnet(arch):
+class WSConv2d(nn.Conv2d):
+    """Weight-standardised convolution (Qiao et al. 2019), the encoder conv of ``BYOL(norm="group_ws")``: every output
+    channel's weights w_o are replaced by (w_o - mean(w_o)) / sqrt(var(w_o) + 1e-5) over its fan-in
+    Cin/groups * kh * kw, with the biased variance.  The parameters are those of ``nn.Conv2d``.  This ``forward`` is
+    the torch definition the tests compare against; the engine runs the same arithmetic in csrc/groupnorm.cu."""
+    standardized = True
+    eps = 1e-5
+
+    def standardized_weight(self):
+        w = self.weight.reshape(self.weight.shape[0], -1)
+        mean = w.mean(1, keepdim=True)
+        var = w.var(1, unbiased=False, keepdim=True)
+        return ((w - mean) / torch.sqrt(var + self.eps)).view_as(self.weight)
+
+    def forward(self, x):
+        return F.conv2d(x, self.standardized_weight(), self.bias, self.stride, self.padding, self.dilation, self.groups)
+
+
+def _group_norm(c):
+    # a width 32 does not divide gets a one-group placeholder, so that _encoder can name the layer in its error
+    return nn.GroupNorm(32 if c % 32 == 0 else 1, c)
+
+
+def _resnet(arch, norm_layer=None):
+    # norm_layer only when given: the default construction is the unchanged torchvision call
+    kw = {} if norm_layer is None else {"norm_layer": norm_layer}
     if arch in models.__dict__:
-        return models.__dict__[arch](weights=None)
+        return models.__dict__[arch](weights=None, **kw)
     from torchvision.models.resnet import ResNet, Bottleneck, BasicBlock
     if arch == "resnet200":   # BASELINE.json config 5: bottleneck [3, 24, 36, 3]; not a torchvision constructor
-        return ResNet(Bottleneck, [3, 24, 36, 3])
+        return ResNet(Bottleneck, [3, 24, 36, 3], **kw)
     if arch.startswith("resnet:"):   # custom depth: "resnet:<basic|bottleneck>:d1,d2,d3,d4"
         _, kind, depths = arch.split(":")
-        return ResNet(Bottleneck if kind == "bottleneck" else BasicBlock, [int(d) for d in depths.split(",")])
+        return ResNet(Bottleneck if kind == "bottleneck" else BasicBlock, [int(d) for d in depths.split(",")], **kw)
     if arch.startswith("resnext:"):  # custom ResNeXt: "resnext:<groups>x<width per group>:d1,d2,d3,d4"
         _, gw, depths = arch.split(":")
         g, w = gw.split("x")
-        return ResNet(Bottleneck, [int(d) for d in depths.split(",")], groups=int(g), width_per_group=int(w))
+        return ResNet(Bottleneck, [int(d) for d in depths.split(",")], groups=int(g), width_per_group=int(w), **kw)
     raise ValueError("unknown arch %r" % arch)
+
+
+def _encoder(arch, norm):
+    """The torchvision ResNet children[:-1].  norm="group_ws": GroupNorm(32, C) layers and every Conv2d turned into a
+    WSConv2d in place (a new module would draw from the RNG), so the parameters and their initial values are the
+    BatchNorm net's."""
+    if norm == "batch":
+        return nn.Sequential(*list(_resnet(arch).children())[:-1])
+    net = nn.Sequential(*list(_resnet(arch, _group_norm).children())[:-1])
+    for name, m in net.named_modules():
+        if isinstance(m, nn.GroupNorm) and m.num_groups != 32:
+            raise ValueError("byol_b200: norm='group_ws' needs every normalised layer's channel count divisible by 32 "
+                             "(GroupNorm with 32 groups): layer base_network.%s has %d channels" % (name, m.num_channels))
+    for m in net.modules():
+        if type(m) is nn.Conv2d:
+            m.__class__ = WSConv2d
+    return net
 
 
 def check_grouped_convs(module, precision):
@@ -177,12 +220,21 @@ class BYOL(nn.Module):
 
     def __init__(self, base_network_output_size, projection_output_size, classifier_output_size,
                  total_training_steps, base_decay=0.996, arch="resnet50", head_latent_size=4096, precision="bf16",
-                 backward_precision="bf16"):
+                 backward_precision="bf16", norm="batch"):
         super(BYOL, self).__init__()
+        # norm: "batch" = BatchNorm after every encoder conv (the reference); "group_ws" = GroupNorm(32) with
+        # weight-standardised convs (WSConv2d), whose statistics are per image: batch-independent representations
+        # ("BYOL works even without batch statistics", Richemond et al. 2020).  The heads keep BatchNorm1d either way.
+        if norm not in ("batch", "group_ws"):
+            raise ValueError("norm must be 'batch' or 'group_ws', got %r" % (norm,))
+        if norm == "group_ws" and precision != "bf16":
+            raise ValueError("norm='group_ws' needs precision='bf16' (GroupNorm runs with bf16 operands only), got "
+                             "precision=%r" % (precision,))
+        self.norm = norm
         self.base_network_output_size = base_network_output_size
         self.arch = arch
         # identical construction order to main.py:190-208 => identical parameter order and default initialisation
-        self.base_network = nn.Sequential(*list(_resnet(arch).children())[:-1])
+        self.base_network = _encoder(arch, norm)
         self.head = nn.Sequential(
             nn.Linear(base_network_output_size, head_latent_size),
             nn.BatchNorm1d(head_latent_size),
@@ -256,7 +308,8 @@ class BYOL(nn.Module):
         average-pooled encoder output of fp32 NCHW CUDA `images` (values in [0, 1], any batch size and resolution the
         stem supports).  network="target" runs the EMA weights (``target_network.mean``).
 
-        Always eval-mode BatchNorm (running statistics), whatever ``self.training`` is; it updates nothing (no EMA step,
+        Always eval-mode BatchNorm (running statistics), whatever ``self.training`` is (GroupNorm layers of a
+        norm="group_ws" model normalise each image by its own statistics, in training and evaluation alike); it updates nothing (no EMA step,
         no running statistics, no ``num_batches_tracked``) and computes no gradient.  Only the encoder runs (no
         projector, predictor or classifier), so the result equals ``model.eval(); model(x, x)["online_representation1"]``
         (``"target_representation1"``) bit for bit, at about a quarter of its cost.  It may be called anywhere in a

@@ -402,6 +402,89 @@ def col_sum(x2d, out):
 
 
 # ------------------------------------------------------------------------------------------------
+# GroupNorm (32 groups) and weight standardisation (BYOL(norm="group_ws"); csrc/groupnorm.cu)
+# ------------------------------------------------------------------------------------------------
+GN_GROUPS = 32
+
+
+def ws_fwd(flat, desc, num_rows, w_out, stats):
+    """Standardise every weight row listed in `desc` (device int64 [units, 5] = src offset in flat, offset in w_out,
+    Cout, fan-in, first row): w_out[row] = (w - mean) / sqrt(var + 1e-5) (biased variance); stats fp32 [rows, 2] =
+    (mean, rstd)."""
+    _chk(flat, F32, "flat"); _chk(w_out, F32, "w_out"); _chk(stats, F32, "stats")
+    check(lib.byol_ws_fwd(_ptr(flat), _ptr(desc), desc.shape[0], int(num_rows), _ptr(w_out), _ptr(stats), _stream()),
+          "byol_ws_fwd")
+
+
+def ws_bwd(dwhat, what, stats, desc, num_rows, grad):
+    """grad[row] (flat fp32, at the row's src offset) += rstd * (dw^ - mean(dw^) - w^ * mean(dw^ * w^))."""
+    _chk(dwhat, F32, "dwhat"); _chk(what, F32, "what"); _chk(stats, F32, "stats"); _chk(grad, F32, "grad")
+    check(lib.byol_ws_bwd(_ptr(dwhat), _ptr(what), _ptr(stats), _ptr(desc), desc.shape[0], int(num_rows), _ptr(grad),
+                          _stream()), "byol_ws_bwd")
+
+
+def gn_stats(y, eps, out=None, sums64=None):
+    """y bf16 [N, H, W, C] -> fp32 [N, 32, 2] (mean, rstd) per (image, group); sums64 (fp64 [N, 32, 2], optional)
+    receives the sums and sums of squares."""
+    _chk(y, BF16, "y"); _chk(sums64, F64, "sums64")
+    n, c = y.shape[0], y.shape[-1]
+    if out is None:
+        out = torch.empty((n, GN_GROUPS, 2), dtype=F32, device=y.device)
+    check(lib.byol_gn_stats(_ptr(y), _ptr(out), _ptr(sums64), n, y.numel() // (n * c), c, float(eps), _stream()),
+          "byol_gn_stats", kernels=2)
+    return out
+
+
+def gn_apply(x, gamma, beta, stats, relu, resid=None, rgn=None, out=None, mask_out=None):
+    """act(x*scale + shift (+ resid | + GroupNorm(resid))) of bf16 [N, H, W, C] with scale = gamma*rstd, shift =
+    beta - mean*scale per (image, channel); rgn = (gamma, beta, stats) of a GroupNorm-applied residual."""
+    _chk(x, BF16, "x"); _chk(resid, BF16, "resid"); _chk(mask_out, torch.uint8, "mask_out")
+    n, c = x.shape[0], x.shape[-1]
+    if out is None:
+        out = torch.empty_like(x)
+    rg, rb, rs = rgn if rgn is not None else (None, None, None)
+    check(lib.byol_gn_apply(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(stats), _ptr(resid), _ptr(rg), _ptr(rb), _ptr(rs),
+                            _ptr(out), _ptr(mask_out), n, x.numel() // (n * c), c, int(relu), _stream()),
+          "byol_gn_apply")
+    return out
+
+
+def gn_relu_maxpool_fwd(x, gamma, beta, stats, k=3, s=2, p=1, want_idx=True):
+    """maxpool(relu(GroupNorm(x))) in one pass (stem); bit-identical to gn_apply(relu) + maxpool_fwd."""
+    _chk(x, BF16, "x")
+    n, h, w, c = x.shape
+    ho, wo = conv_out_size(h, k, s, p), conv_out_size(w, k, s, p)
+    y = torch.empty((n, ho, wo, c), dtype=BF16, device=x.device)
+    idx = torch.empty((n, ho, wo, c), dtype=torch.uint8, device=x.device) if want_idx else None
+    check(lib.byol_gn_relu_maxpool_fwd(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(stats), _ptr(y), _ptr(idx), n, h, w, c,
+                                       k, s, p, _stream()), "byol_gn_relu_maxpool_fwd")
+    return y, idx
+
+
+def gn_bwd_reduce(g, x, gamma, beta, stats, s12, mask_mode, act=None, dgamma=None, dbeta=None):
+    """s12 (zeroed fp32 [N, 32, 2]) += per (image, group) [sum gamma*dz, sum gamma*dz*xhat]; dgamma / dbeta += the
+    per-channel sums dz*xhat / dz.  mask_mode as bn_bwd_reduce."""
+    _chk(g, BF16, "g"); _chk(x, BF16, "x"); _chk(act, torch.uint8 if mask_mode == 3 else BF16, "act")
+    _chk(s12, F32, "s12")
+    n, c = x.shape[0], x.shape[-1]
+    check(lib.byol_gn_bwd_reduce(_ptr(g), _ptr(x), _ptr(act), _ptr(gamma), _ptr(beta), _ptr(stats), _ptr(s12),
+                                 _ptr(dgamma), _ptr(dbeta), n, x.numel() // (n * c), c, mask_mode, _stream()),
+          "byol_gn_bwd_reduce", kernels=2 if dgamma is None else 4)
+    return s12
+
+
+def gn_bwd_apply(g, x, gamma, beta, stats, s12, mask_mode, act=None, dy=None, dz_out=None):
+    """dy = rstd*(gamma*dz - s1/m - xhat*s2/m) per (image, group), m = H*W*C/32; dz_out (optional) receives dz."""
+    _chk(g, BF16, "g"); _chk(x, BF16, "x"); _chk(act, torch.uint8 if mask_mode == 3 else BF16, "act")
+    n, c = x.shape[0], x.shape[-1]
+    if dy is None:
+        dy = torch.empty_like(x)
+    check(lib.byol_gn_bwd_apply(_ptr(g), _ptr(x), _ptr(act), _ptr(gamma), _ptr(beta), _ptr(stats), _ptr(s12), _ptr(dy),
+                                _ptr(dz_out), n, x.numel() // (n * c), c, mask_mode, _stream()), "byol_gn_bwd_apply")
+    return dy
+
+
+# ------------------------------------------------------------------------------------------------
 # pooling
 # ------------------------------------------------------------------------------------------------
 def maxpool_fwd(x, k=3, s=2, p=1, want_idx=True):

@@ -95,6 +95,37 @@ int byol_bn_bwd_apply(const void* g, const void* x, const void* act, const float
                       float* dbeta, byol_stream_t stream);
 int byol_col_sum(const void* x, float* out, int M, int C, int ld, int is_f32, byol_stream_t stream);
 
+/* ---- GroupNorm (32 groups) and weight standardisation: BYOL(norm="group_ws") ---- */
+/* desc: device int64 [num_units][5] = {src offset in flat, offset in w_out / dwhat, Cout, fan-in, first row}, rows in
+ * unit order.  w_out[row] = (w - mean) / sqrt(var + 1e-5) (biased variance, fp64, rounded once); stats [rows][2] =
+ * fp32 (mean, rstd) */
+int byol_ws_fwd(const float* flat, const int64_t* desc, int num_units, int64_t num_rows, float* w_out, float* stats,
+                byol_stream_t stream);
+/* grad[row] += rstd * (dw^ - mean(dw^) - w^ * mean(dw^ * w^)) with w^ = w_out and stats of byol_ws_fwd */
+int byol_ws_bwd(const float* dwhat, const float* what, const float* stats, const int64_t* desc, int num_units,
+                int64_t num_rows, float* grad, byol_stream_t stream);
+/* y [N, HW, C] bf16 (C % 32 == 0, C % 8 == 0) -> stats [N][32][2] = fp32 (mean, rstd) per (image, group); sums64
+ * (optional, fp64 [N][32][2]) receives the sum and sum of squares */
+int byol_gn_stats(const void* y, float* stats, double* sums64, int N, int HW, int C, float eps, byol_stream_t stream);
+/* y = act(x*scale + shift (+ resid | + resid*rscale + rshift)), scale[n,c] = gamma[c]*rstd[n,g], shift[n,c] =
+ * beta[c] - mean[n,g]*scale[n,c]; the residual's (rscale, rshift) come from (rgamma, rbeta, rstats) when given;
+ * mask_out (optional, uint8 [N*HW*C/8]) as byol_bn_apply */
+int byol_gn_apply(const void* x, const float* gamma, const float* beta, const float* stats, const void* resid,
+                  const float* rgamma, const float* rbeta, const float* rstats, void* y, void* mask_out, int N, int HW,
+                  int C, int relu, byol_stream_t stream);
+/* stem fusion: y = maxpool(relu(gn(x))); values and argmax indices equal byol_gn_apply + byol_maxpool_fwd */
+int byol_gn_relu_maxpool_fwd(const void* x, const float* gamma, const float* beta, const float* stats, void* y,
+                             void* idx, int N, int H, int W, int C, int k, int s, int p, byol_stream_t stream);
+/* s12 (zeroed fp32 [N][32][2]) += per (image, group) (sum gamma*dz, sum gamma*dz*xhat); dgamma / dbeta (optional,
+ * together) += per-channel sum dz*xhat / sum dz; mask_mode as byol_bn_bwd_reduce */
+int byol_gn_bwd_reduce(const void* g, const void* x, const void* act, const float* gamma, const float* beta,
+                       const float* stats, float* s12, float* dgamma, float* dbeta, int N, int HW, int C, int mask_mode,
+                       byol_stream_t stream);
+/* dy = rstd*(gamma*dz - s1/m - xhat*s2/m), m = HW*C/32; dz_out (optional) receives dz */
+int byol_gn_bwd_apply(const void* g, const void* x, const void* act, const float* gamma, const float* beta,
+                      const float* stats, const float* s12, void* dy, void* dz_out, int N, int HW, int C, int mask_mode,
+                      byol_stream_t stream);
+
 /* ---- layout / pooling: torchvision ResNet stem and tail reached from main.py:237 ---- */
 int byol_nchw_to_nhwc8(const float* x, void* y, int N, int Cin, int H, int W, byol_stream_t stream);
 int byol_prep_weight(const float* w, void* w_fprop, void* w_dgrad, int Cout, int Cin, int Cpad, int KH, int KW,
