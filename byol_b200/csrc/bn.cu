@@ -179,9 +179,17 @@ __global__ void bn_apply_kernel(const bf16* __restrict__ x, const float* __restr
   }
 }
 
+// Vectors in flight per thread of bn_apply_fixed_kernel<*, false>: each thread loads the 16-byte vectors i, i + T,
+// ..., i + (kFixedVecs - 1) T of the grid's T threads (every operand) before any arithmetic, so each warp still reads
+// and writes 512 contiguous bytes per vector and each thread stays on one channel group.  Its grid is at most one wave
+// of resident blocks (fixed_wave_grid).
+static constexpr int kFixedVecs = 4;
+
 // Same as bn_apply_kernel, for launches where (gridDim.x * blockDim.x) % (C/8) == 0: every thread then stays on
 // ONE 8-channel group for its whole grid-stride loop and keeps the per-channel coefficients in registers
 // (the generic kernel re-loads them per vector, which makes it LSU-bound rather than HBM-bound).
+// <true, true> (block outputs with a downsample-BN residual) already ran at 85 % of the HBM bound with one vector per
+// thread and the fixed_grid launch, and kFixedVecs vectors on one wave did not make it faster: it keeps that schedule.
 template <bool RESID, bool RAFFINE>
 __global__ void __launch_bounds__(256)
 bn_apply_fixed_kernel(const bf16* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ shift,
@@ -199,24 +207,39 @@ bn_apply_fixed_kernel(const bf16* __restrict__ x, const float* __restrict__ scal
     rs[e] = RAFFINE ? rscale[g * 8 + e] : 1.f;
     rb[e] = RAFFINE ? rshift[g * 8 + e] : 0.f;
   }
+  constexpr int V = RAFFINE ? 1 : kFixedVecs;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = tid; i < nvec; i += stride) {
-    float xv[8], o[8];
-    unpack8(__ldg(reinterpret_cast<const uint4*>(x) + i), xv);
+  for (int64_t i = tid; i < nvec; i += V * stride) {
+    uint4 xq[V], rq[V];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) o[e] = xv[e] * sc[e] + sh[e];
-    if (RESID) {
-      float rv[8];
-      unpack8(__ldg(reinterpret_cast<const uint4*>(resid) + i), rv);
-#pragma unroll
-      for (int e = 0; e < 8; ++e) o[e] += RAFFINE ? (rv[e] * rs[e] + rb[e]) : rv[e];
+    for (int u = 0; u < V; ++u) {
+      const int64_t j = i + u * stride;
+      const bool ok = j < nvec;
+      xq[u] = ok ? __ldg(reinterpret_cast<const uint4*>(x) + j) : make_uint4(0u, 0u, 0u, 0u);
+      if (RESID) rq[u] = ok ? __ldg(reinterpret_cast<const uint4*>(resid) + j) : make_uint4(0u, 0u, 0u, 0u);
     }
-    if (relu) {
 #pragma unroll
-      for (int e = 0; e < 8; ++e) o[e] = fmaxf(o[e], 0.f);
+    for (int u = 0; u < V; ++u) {
+      const int64_t j = i + u * stride;
+      if (j < nvec) {
+        float xv[8], o[8];
+        unpack8(xq[u], xv);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) o[e] = xv[e] * sc[e] + sh[e];
+        if (RESID) {
+          float rv[8];
+          unpack8(rq[u], rv);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) o[e] += RAFFINE ? (rv[e] * rs[e] + rb[e]) : rv[e];
+        }
+        if (relu) {
+#pragma unroll
+          for (int e = 0; e < 8; ++e) o[e] = fmaxf(o[e], 0.f);
+        }
+        reinterpret_cast<uint4*>(y)[j] = pack8(o);
+        if (mask_out != nullptr) mask_out[j] = positive_bits(o);
+      }
     }
-    reinterpret_cast<uint4*>(y)[i] = pack8(o);
-    if (mask_out != nullptr) mask_out[i] = positive_bits(o);
   }
 }
 
@@ -361,78 +384,123 @@ __global__ void bn_bwd_reduce_kernel(const bf16* __restrict__ g, const bf16* __r
   }
 }
 
-// Same reduction with the access pattern of the "fixed" elementwise kernels: the whole grid sweeps the tensor front to
-// back (grid-stride over 8-channel vectors; (gridDim.x * blockDim.x) % (C/8) == 0 pins every thread to ONE channel
-// group), instead of one private row range per block.  1184 private sequential streams per operand cost DRAM row
-// locality: the row-range kernel reads more slowly than the sweeping kernels.
+// Same reduction with the access pattern of the "fixed" elementwise kernels: the grid sweeps the tensor front to back
+// instead of giving each block a private row range (1184 private sequential streams per operand cost DRAM row
+// locality).  Its result is defined by S = `chains` = fixed_grid(nvec, C/8) * 256 fp32 partial sums: chain t < S sums
+// the 8-channel vectors t, t+S, t+2S, ... in that order, four vectors per iteration (past the end an iteration adds
+// zero gradients), and every chain's a1[e] / a2[e] goes into fixed point.  Fixed-point addition is exact and
+// order-free, so how chains map onto threads and blocks does not change a bit:
+//  - a warp runs 32 consecutive chains (512 contiguous bytes per vector and operand); chain t is on channel group
+//    t % (C/8), so warps whose first chain is equal modulo C/8 ("class": one of max(C/256, 1)) have the same channels
+//    in every lane and the 8 warps of a block are always of one class;
+//  - a warp runs `rounds` such chain sets one after another, and the grid is at most one wave of resident blocks;
+//  - each thread turns a finished chain into fixed-point words in registers and adds them, as plain 64-bit integers,
+//    to its own slots of a shared-memory slab (the part of an addend beyond the words goes straight to the fp64 side
+//    sum in global memory, fix_take_spill); at the end the block adds the slots of each channel, over its warps and
+//    the lanes that share the channel, and issues one fix_add_words per channel and sum.
+// The integer sums wrap mod 2^64 in any grouping, so s1 / s2 end with the same words and side sums as when every
+// chain went to them on its own.
+static constexpr int kReduceWarps = 8;
+static constexpr int kReduceSlab = 2 * kReduceWarps * 16 * 32;   // lo and hi words: [2][warp][16 sums][32 lanes]
 template <int MASK>
 __global__ void __launch_bounds__(256)
 bn_bwd_reduce_fixed_kernel(const bf16* __restrict__ g, const bf16* __restrict__ x, const bf16* __restrict__ act,
                            const float* __restrict__ scale, const float* __restrict__ shift,
                            const float* __restrict__ mean, const float* __restrict__ invstd, Fix128* __restrict__ s1,
-                           Fix128* __restrict__ s2, int64_t nvec, int C) {
-  extern __shared__ Fix128 red[];                   // [2][C]
-  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) red[c] = Fix128{0ull, 0ll, 0.0};
-  __syncthreads();
+                           Fix128* __restrict__ s2, int64_t nvec, int C, int64_t chains, int rounds) {
+  extern __shared__ unsigned long long slab[];
   const int groups = C >> 3;
-  const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  const int gi = (int)(tid % groups);
-  float a1[8], a2[8], mu[8], is[8], sc[8], sh[8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int classes = groups > 32 ? groups / 32 : 1;
+  const int cls = (int)(blockIdx.x % classes);
+  const int64_t per_class = chains / 32 / classes;                       // warps of chains in each class
+  const int64_t first = (int64_t)(blockIdx.x / classes) * rounds * kReduceWarps;
+  unsigned long long* lo_w = slab + warp * 16 * 32 + lane;               // this thread's 16 slots, 32 words apart
+  unsigned long long* hi_w = lo_w + kReduceSlab / 2;
+#pragma unroll
+  for (int v = 0; v < 16; ++v) { lo_w[32 * v] = 0ull; hi_w[32 * v] = 0ull; }
+  const int gi = (cls * 32 + lane) % groups;
+  float mu[8], is[8], sc[8], sh[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
-    a1[e] = 0.f; a2[e] = 0.f;
     mu[e] = mean[gi * 8 + e];
     is[e] = invstd[gi * 8 + e];
     sc[e] = MASK == 1 ? scale[gi * 8 + e] : 0.f;
     sh[e] = MASK == 1 ? shift[gi * 8 + e] : 0.f;
   }
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = tid; i < nvec; i += 4 * stride) {
-    uint4 gq[4], xq[4], aq[4];
-    uint32_t mb[4];
+  for (int k = 0; k < rounds; ++k) {
+    const int64_t wj = first + (int64_t)k * kReduceWarps + warp;
+    if (wj >= per_class) break;
+    const int64_t t = (wj * classes + cls) * 32 + lane;                  // this thread's chain
+    float a1[8], a2[8];
 #pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int64_t j = i + u * stride;
-      const bool ok = j < nvec;
-      const int64_t off = ok ? j : i;
-      gq[u] = ok ? __ldg(reinterpret_cast<const uint4*>(g) + off) : make_uint4(0u, 0u, 0u, 0u);
-      xq[u] = __ldg(reinterpret_cast<const uint4*>(x) + off);
-      if (MASK == 3) mb[u] = __ldg(reinterpret_cast<const uint8_t*>(act) + off);
-      if (MASK == 2) aq[u] = __ldg(reinterpret_cast<const uint4*>(act) + off);
-    }
+    for (int e = 0; e < 8; ++e) { a1[e] = 0.f; a2[e] = 0.f; }
+    // Two of the chain's four-vector iterations per pass, all 8 loads issued first (short chains wait on memory
+    // half as often).  The second iteration is added only when the chain has it; within an iteration a vector past
+    // the end loads a zero gradient and the x of the iteration's first vector, exactly as one iteration at a time.
+    for (int64_t i0 = t; i0 < nvec; i0 += 8 * chains) {
+      uint4 gq[8], xq[8], aq[8];
+      uint32_t mb[8];
+      const bool second = i0 + 4 * chains < nvec;
 #pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      float gv[8], xv[8];
-      unpack8(gq[u], gv);
-      unpack8(xq[u], xv);
-      if (MASK == 3) {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) gv[e] = ((mb[u] >> e) & 1u) ? gv[e] : 0.f;
-      } else if (MASK == 2) {
-        float av[8];
-        unpack8(aq[u], av);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) gv[e] = av[e] > 0.f ? gv[e] : 0.f;
-      } else if (MASK == 1) {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) gv[e] = (xv[e] * sc[e] + sh[e]) > 0.f ? gv[e] : 0.f;
+      for (int u = 0; u < 8; ++u) {
+        const int64_t i = u < 4 ? i0 : i0 + 4 * chains;
+        const int64_t j = i + (u & 3) * chains;
+        const bool ok = j < nvec;
+        const bool in_chain = u < 4 || second;
+        const int64_t off = ok ? j : (in_chain ? i : i0);
+        gq[u] = ok ? __ldg(reinterpret_cast<const uint4*>(g) + off) : make_uint4(0u, 0u, 0u, 0u);
+        xq[u] = __ldg(reinterpret_cast<const uint4*>(x) + off);
+        if (MASK == 3) mb[u] = __ldg(reinterpret_cast<const uint8_t*>(act) + off);
+        if (MASK == 2) aq[u] = __ldg(reinterpret_cast<const uint4*>(act) + off);
       }
 #pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        a1[e] += gv[e];
-        a2[e] += gv[e] * (xv[e] - mu[e]) * is[e];
+      for (int u = 0; u < 8; ++u) {
+        if (u >= 4 && !second) break;
+        float gv[8], xv[8];
+        unpack8(gq[u], gv);
+        unpack8(xq[u], xv);
+        if (MASK == 3) {
+#pragma unroll
+          for (int e = 0; e < 8; ++e) gv[e] = ((mb[u] >> e) & 1u) ? gv[e] : 0.f;
+        } else if (MASK == 2) {
+          float av[8];
+          unpack8(aq[u], av);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) gv[e] = av[e] > 0.f ? gv[e] : 0.f;
+        } else if (MASK == 1) {
+#pragma unroll
+          for (int e = 0; e < 8; ++e) gv[e] = (xv[e] * sc[e] + sh[e]) > 0.f ? gv[e] : 0.f;
+        }
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          a1[e] += gv[e];
+          a2[e] += gv[e] * (xv[e] - mu[e]) * is[e];
+        }
       }
     }
-  }
 #pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    fix_add(red + gi * 8 + e, a1[e]);
-    fix_add(red + C + gi * 8 + e, a2[e]);
+    for (int v = 0; v < 16; ++v) {
+      double a = v < 8 ? (double)a1[v] : (double)a2[v - 8];
+      if (!fix_take_spill((v < 8 ? s1 : s2) + gi * 8 + (v & 7), a)) continue;
+      unsigned long long lo;
+      long long hi;
+      fix_words(a, lo, hi);
+      lo_w[32 * v] += lo;
+      hi_w[32 * v] += (unsigned long long)hi;
+    }
   }
   __syncthreads();
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    fix_add_raw(s1 + c, red[c]);
-    fix_add_raw(s2 + c, red[C + c]);
+  const int win = groups < 32 ? groups : 32;                             // channel groups of the block
+  for (int idx = threadIdx.x; idx < 16 * win; idx += blockDim.x) {
+    const int v = idx / win, p = idx - v * win;
+    unsigned long long lo = 0ull, hi = 0ull;
+    for (int w = 0; w < kReduceWarps; ++w)
+      for (int l = p; l < 32; l += win) {
+        lo += slab[(w * 16 + v) * 32 + l];
+        hi += slab[kReduceSlab / 2 + (w * 16 + v) * 32 + l];
+      }
+    fix_add_words((v < 8 ? s1 : s2) + (cls * 32 + p) * 8 + (v & 7), lo, (long long)hi);
   }
 }
 
@@ -514,6 +582,16 @@ static inline int fixed_grid(int64_t nvec, int groups) {
   return (int)b;
 }
 
+// launch grid of bn_apply_fixed_kernel<*, false>: enough blocks for kFixedVecs vectors per thread, at most
+// `resident` (one wave), a multiple of the blocks per channel period so that (grid*256) % groups == 0
+static inline int fixed_wave_grid(int64_t nvec, int groups, int resident) {
+  const int unit = groups > 256 ? groups / 256 : 1;
+  int64_t b = (nvec + 256 * kFixedVecs - 1) / (256 * kFixedVecs);
+  if (b > resident) b = resident;
+  b = b / unit * unit;
+  return (int)(b < unit ? unit : b);
+}
+
 static inline int grid_for(int64_t n, int block, int max_blocks = 132 * 16) {
   int64_t b = (n + block - 1) / block;
   if (b > max_blocks) b = max_blocks;
@@ -575,12 +653,15 @@ extern "C" int byol_bn_apply(const void* x, const float* scale, const float* shi
   const int fg = (y != nullptr && y_f32 == nullptr) ? fixed_grid(nvec, C / 8) : 0;
   if (fg > 0) {
     const bf16 *xp = (const bf16*)x, *rp = (const bf16*)resid;
-    if (resid == nullptr)
-      bn_apply_fixed_kernel<false, false><<<fg, 256, 0, stream>>>(xp, scale, shift, rp, rscale, rshift, (bf16*)y, mo, nvec, C, relu);
-    else if (rscale == nullptr)
-      bn_apply_fixed_kernel<true, false><<<fg, 256, 0, stream>>>(xp, scale, shift, rp, rscale, rshift, (bf16*)y, mo, nvec, C, relu);
-    else
+    if (rscale != nullptr) {
       bn_apply_fixed_kernel<true, true><<<fg, 256, 0, stream>>>(xp, scale, shift, rp, rscale, rshift, (bf16*)y, mo, nvec, C, relu);
+      return check_launch("bn_apply_fixed_kernel");
+    }
+    const auto kern = resid == nullptr ? bn_apply_fixed_kernel<false, false> : bn_apply_fixed_kernel<true, false>;
+    const int resident = resident_blocks((const void*)kern, 256, 0, "bn_apply_fixed_kernel");
+    if (resident <= 0) return -2;
+    kern<<<fixed_wave_grid(nvec, C / 8, resident), 256, 0, stream>>>(xp, scale, shift, rp, rscale, rshift, (bf16*)y,
+                                                                     mo, nvec, C, relu);
     return check_launch("bn_apply_fixed_kernel");
   }
   bn_apply_kernel<<<grid_for(nvec, 256), 256, 0, stream>>>((const bf16*)x, scale, shift, (const bf16*)resid, rscale,
@@ -611,8 +692,20 @@ extern "C" int byol_bn_bwd_reduce(const void* g, const void* x, const void* act,
         bn_bwd_reduce_fixed_kernel<0>, bn_bwd_reduce_fixed_kernel<1>, bn_bwd_reduce_fixed_kernel<2>,
         bn_bwd_reduce_fixed_kernel<3>};
     const auto kern = fixed_kernels[mask_mode];
-    if (smem_opt_in((const void*)kern, (int)red_bytes, "bn_bwd_reduce_fixed_kernel") != 0) return -2;
-    kern<<<fg, 256, red_bytes, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, nvec, C);
+    const int slab = kReduceSlab * (int)sizeof(unsigned long long);
+    if (smem_opt_in((const void*)kern, slab, "bn_bwd_reduce_fixed_kernel") != 0) return -2;
+    const int resident = resident_blocks((const void*)kern, 256, slab, "bn_bwd_reduce_fixed_kernel");
+    if (resident <= 0) return -2;
+    // fixed_grid defines the chains (and so the bits); the launch is the fewest rounds that fit in one wave: at most
+    // resident / classes blocks per class, and at least one (a device holding fewer blocks than there are classes
+    // runs one block per class, in more than one wave)
+    const int64_t chains = (int64_t)fg * 256;
+    const int64_t classes = C / 8 > 32 ? C / 8 / 32 : 1, per_class = chains / 32 / classes;
+    const int64_t class_blocks = resident / classes > 0 ? resident / classes : 1;
+    const int64_t rounds = (per_class + kReduceWarps * class_blocks - 1) / (kReduceWarps * class_blocks);
+    const int blocks = (int)(classes * ((per_class + kReduceWarps * rounds - 1) / (kReduceWarps * rounds)));
+    kern<<<blocks, 256, slab, stream>>>(gp, xp, ap, scale, shift, mean, invstd, fx, fx + C, nvec, C, chains,
+                                        (int)rounds);
     if (check_launch("bn_bwd_reduce_fixed_kernel") != 0) return -100;
     return fix_done(stream, fix_flush(fx, s12, 2 * (int64_t)C, stream));
   }

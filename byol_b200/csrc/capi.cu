@@ -1,5 +1,5 @@
 // byol_b200 — C-ABI plumbing shared by every entry point: thread-local error string, launch checks, version, and the
-// host-side launch helpers (shared-memory opt-in, tensor maps, fixed-point scratch).
+// host-side launch helpers (shared-memory opt-in, resident grids, tensor maps, fixed-point scratch).
 #include <stdarg.h>
 #include <stdio.h>
 
@@ -64,6 +64,27 @@ int smem_opt_in(const void* kernel, int bytes, const char* what) {
   }
   have = bytes;
   return 0;
+}
+
+int resident_blocks(const void* kernel, int threads, int smem_bytes, const char* what) {
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, int> known;   // (kernel, device slot) -> blocks on the device
+  const std::lock_guard<std::mutex> lock(mu);
+  int& n = known.emplace(std::make_pair(kernel, device_slot()), 0).first->second;
+  if (n > 0) return n;
+  int per_sm = 0;
+  // not a stream operation: allowed while the calling stream is being captured (as in fix_scratch)
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, (size_t)smem_bytes);
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  if (e != cudaSuccess || per_sm <= 0) {
+    set_last_error("%s: no resident block of %d threads and %d bytes of shared memory (%s)", what, threads, smem_bytes,
+                   cudaGetErrorString(e));
+    return 0;
+  }
+  n = per_sm * device_sm_count();
+  return n;
 }
 
 int tmap_bf16(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims, const uint64_t* byte_strides,

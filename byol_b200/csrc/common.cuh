@@ -26,6 +26,10 @@ int device_sm_count();   // SM count of the current device (cached per device; 1
 // Lets `kernel` launch with `bytes` of dynamic shared memory on the current device.  The attribute is raised only
 // when a launch needs more than the kernel was granted there so far (48 KB need no opt-in).  0, or -2 on failure.
 int smem_opt_in(const void* kernel, int bytes, const char* what);
+// Blocks of `kernel` (`threads` per block, `smem_bytes` of dynamic shared memory) the current device holds at once:
+// the occupancy calculator's blocks per SM times the SM count, queried once per (kernel, device), so a kernel must
+// always be asked about with the same block shape.  0 on failure.
+int resident_blocks(const void* kernel, int threads, int smem_bytes, const char* what);
 
 // Tensor maps: every operand the kernels move by TMA is bf16, uninterleaved, promoted to L2 in 256-byte lines and
 // not OOB-filled (out-of-bounds elements load as zero).  dims[0] is the contiguous dimension; byte_strides holds the
