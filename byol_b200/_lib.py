@@ -68,6 +68,9 @@ _SIGNATURES = {
     "byol_loss_fwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
     "byol_loss_bwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                       c_void_p],
+    "byol_loss_rows_fwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p],
+    "byol_loss_rows_bwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                           c_int, c_void_p],
     "byol_ema_update": [c_void_p, c_void_p, c_float, c_float, c_int64, c_void_p],
     "byol_lars_sgd_step": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                            c_void_p, c_void_p, c_int, c_void_p, c_float, c_float, c_float, c_int, c_void_p],

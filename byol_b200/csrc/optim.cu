@@ -102,6 +102,141 @@ __global__ void loss_bwd_kernel(const float* __restrict__ q1, const float* __res
 }
 
 // ---------------------------------------------------------------------------------------------
+// The BYOL paper's loss: per-sample L2-normalised predictions and targets.
+//   r(x) = max(sum x^2, eps)^(-1/2) (eps = 1e-12 under the square root), x^ = r(x) x,
+//   l(q, z) = sum_d (q^_d - z^_d)^2,  L = (1/B) sum_i [ l(q1_i, z2_i) + l(q2_i, z1_i) ].
+// A row whose sum of squares is NaN or +inf (a NaN or inf element, or a finite row whose squares overflow) gets
+// r = NaN, so its loss and its gradient are NaN instead of those of a zero row.
+// Every fp32 operation is written as an intrinsic or fmaf, so the compiler contracts nothing and the arithmetic is
+// exactly what the source says.
+// ---------------------------------------------------------------------------------------------
+constexpr float kPaperLossEps = 1e-12f;
+constexpr int kRowsPerBlock = 8;   // one warp per sample, 256 threads
+
+__device__ __forceinline__ float add_squares(const float4 v, float s) {
+  s = fmaf(v.x, v.x, s);
+  s = fmaf(v.y, v.y, s);
+  s = fmaf(v.z, v.z, s);
+  return fmaf(v.w, v.w, s);
+}
+
+__device__ __forceinline__ float row_rnorm(float s) {
+  return s < INFINITY ? __fdiv_rn(1.f, __fsqrt_rn(fmaxf(s, kPaperLossEps))) : __int_as_float(0x7fffffff);
+}
+
+// u = q^ - z^ for one element; l += u^2, p += q^ u
+__device__ __forceinline__ void pair_terms(float q, float z, float rq, float rz, float& l, float& p) {
+  const float qh = __fmul_rn(rq, q);
+  const float u = __fsub_rn(qh, __fmul_rn(rz, z));
+  l = fmaf(u, u, l);
+  p = fmaf(qh, u, p);
+}
+
+__device__ __forceinline__ void pair_terms4(const float4 q, const float4 z, float rq, float rz, float& l, float& p) {
+  pair_terms(q.x, z.x, rq, rz, l, p);
+  pair_terms(q.y, z.y, rq, rz, l, p);
+  pair_terms(q.z, z.z, rq, rz, l, p);
+  pair_terms(q.w, z.w, rq, rz, l, p);
+}
+
+// Warp w of block b takes sample i = 8b + w, both of its pairs (q1_i, z2_i) and (q2_i, z1_i).  Lane l sums the float4s
+// l, l + 32, ... of each row in order (x, y, z, w by fmaf), then a butterfly over the 32 lanes.  Pass 1 gives the
+// sums of squares, pass 2 re-reads the rows (from L1) for l and q^.u.  saved[8 i ..] = r(q1), r(z2), c12, l12, r(q2),
+// r(z1), c21, l21 with c = q^.u when sum q^2 > eps and 0 when the row is clamped.  part[b] = the fp64 sum, in warp
+// order, of (double)l12 + (double)l21 over the block's samples.
+__global__ void __launch_bounds__(256)
+loss_rows_fwd_kernel(const float* __restrict__ q1, const float* __restrict__ q2, const float* __restrict__ z1,
+                     const float* __restrict__ z2, int rows, int d4, float* __restrict__ saved,
+                     double* __restrict__ part) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int row = blockIdx.x * kRowsPerBlock + warp;
+  double lrow = 0.0;
+  if (row < rows) {
+    const int64_t off = (int64_t)row * d4;
+    const float4* __restrict__ a4 = reinterpret_cast<const float4*>(q1) + off;
+    const float4* __restrict__ b4 = reinterpret_cast<const float4*>(z2) + off;
+    const float4* __restrict__ c4 = reinterpret_cast<const float4*>(q2) + off;
+    const float4* __restrict__ d4p = reinterpret_cast<const float4*>(z1) + off;
+    float sq1 = 0.f, sz2 = 0.f, sq2 = 0.f, sz1 = 0.f;
+    for (int j = lane; j < d4; j += 32) {
+      sq1 = add_squares(__ldg(a4 + j), sq1);
+      sz2 = add_squares(__ldg(b4 + j), sz2);
+      sq2 = add_squares(__ldg(c4 + j), sq2);
+      sz1 = add_squares(__ldg(d4p + j), sz1);
+    }
+    sq1 = warp_sum(sq1); sz2 = warp_sum(sz2); sq2 = warp_sum(sq2); sz1 = warp_sum(sz1);
+    const float rq1 = row_rnorm(sq1), rz2 = row_rnorm(sz2), rq2 = row_rnorm(sq2), rz1 = row_rnorm(sz1);
+    float l12 = 0.f, p12 = 0.f, l21 = 0.f, p21 = 0.f;
+    for (int j = lane; j < d4; j += 32) {
+      pair_terms4(__ldg(a4 + j), __ldg(b4 + j), rq1, rz2, l12, p12);
+      pair_terms4(__ldg(c4 + j), __ldg(d4p + j), rq2, rz1, l21, p21);
+    }
+    l12 = warp_sum(l12); p12 = warp_sum(p12); l21 = warp_sum(l21); p21 = warp_sum(p21);
+    if (lane == 0) {
+      float4* s = reinterpret_cast<float4*>(saved + (int64_t)row * 8);
+      s[0] = make_float4(rq1, rz2, sq1 > kPaperLossEps ? p12 : 0.f, l12);
+      s[1] = make_float4(rq2, rz1, sq2 > kPaperLossEps ? p21 : 0.f, l21);
+    }
+    lrow = (double)l12 + (double)l21;
+  }
+  __shared__ double sh[kRowsPerBlock];
+  if (lane == 0) sh[warp] = lrow;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+#pragma unroll
+    for (int w = 0; w < kRowsPerBlock; ++w) s += sh[w];
+    part[blockIdx.x] = s;
+  }
+}
+
+// loss = (float)(S / rows), S the fp64 sum of the nb block slots: lane l adds slots l, l + 32, ... in order (and zeroes
+// them: they live in the stream's scratch, which its users leave zeroed), then a butterfly over the lanes.
+__global__ void loss_rows_finalize_kernel(double* __restrict__ part, int nb, int rows, float* __restrict__ loss) {
+  const int lane = threadIdx.x;
+  double s = 0.0;
+  for (int b = lane; b < nb; b += 32) {
+    s += part[b];
+    part[b] = 0.0;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) loss[0] = (float)(s / (double)rows);
+}
+
+// dq = a * (u - c q^) per element, a = fl(fl(2 go / rows) * r(q)), u = q^ - z^ recomputed from q, z and the saved
+// r(q), r(z); the inner term is one fmaf(-c, q^, u).  One pass over q and z, no atomics.
+__device__ __forceinline__ float pair_grad(float q, float z, float rq, float rz, float c, float a) {
+  const float qh = __fmul_rn(rq, q);
+  const float u = __fsub_rn(qh, __fmul_rn(rz, z));
+  return __fmul_rn(a, fmaf(-c, qh, u));
+}
+
+__device__ __forceinline__ float4 pair_grad4(const float4 q, const float4 z, float rq, float rz, float c, float a) {
+  return make_float4(pair_grad(q.x, z.x, rq, rz, c, a), pair_grad(q.y, z.y, rq, rz, c, a),
+                     pair_grad(q.z, z.z, rq, rz, c, a), pair_grad(q.w, z.w, rq, rz, c, a));
+}
+
+__global__ void __launch_bounds__(256)
+loss_rows_bwd_kernel(const float* __restrict__ q1, const float* __restrict__ q2, const float* __restrict__ z1,
+                     const float* __restrict__ z2, const float* __restrict__ saved,
+                     const float* __restrict__ grad_out, float* __restrict__ dq1, float* __restrict__ dq2,
+                     int64_t n4, int d4, int rows) {
+  const float go = grad_out != nullptr ? grad_out[0] : 1.f;
+  const float k = __fdiv_rn(__fmul_rn(go, 2.f), (float)rows);
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+    const float4* s = reinterpret_cast<const float4*>(saved + (i / d4) * 8);
+    const float4 s12 = __ldg(s), s21 = __ldg(s + 1);
+    reinterpret_cast<float4*>(dq1)[i] = pair_grad4(__ldg(reinterpret_cast<const float4*>(q1) + i),
+                                                   __ldg(reinterpret_cast<const float4*>(z2) + i), s12.x, s12.y, s12.z,
+                                                   __fmul_rn(k, s12.x));
+    reinterpret_cast<float4*>(dq2)[i] = pair_grad4(__ldg(reinterpret_cast<const float4*>(q2) + i),
+                                                   __ldg(reinterpret_cast<const float4*>(z1) + i), s21.x, s21.y, s21.z,
+                                                   __fmul_rn(k, s21.x));
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // EMA:  mean[i] = fl(fl(a*x[i]) + fl(d*mean[i]))   a = fp32(1-decay), d = fp32(decay)
 // float4-vectorised; 12 B/param of HBM traffic.
 // ---------------------------------------------------------------------------------------------
@@ -459,6 +594,45 @@ extern "C" int byol_loss_bwd(const float* q1, const float* q2, const float* z1, 
   loss_bwd_kernel<<<grid_for(n / 4, 256, 132 * 4), 256, 0, stream>>>(q1, q2, z1, z2, saved, grad_out, dq1, dq2,
                                                                     n / 4, rows);
   return check_launch("loss_bwd_kernel");
+}
+
+static inline bool aligned16_host(const void* p) { return ((uintptr_t)p & 15u) == 0; }
+
+// The paper's loss.  q1,q2,z1,z2: [rows, dim] fp32 contiguous, 16-byte aligned, dim a positive multiple of 4.
+// loss: 1 float; saved: [rows, 8] floats (16-byte aligned) consumed by byol_loss_rows_bwd.  The per-block fp64 slots
+// (one per 8 rows) live in the stream's zeroed scratch, as byol_loss_fwd's do; the grid depends on rows alone.
+extern "C" int byol_loss_rows_fwd(const float* q1, const float* q2, const float* z1, const float* z2, int rows,
+                                  int dim, float* loss, float* saved, cudaStream_t stream) {
+  BYOL_CHECK_ARG(q1 && q2 && z1 && z2 && loss && saved, "byol_loss_rows_fwd: null pointer");
+  BYOL_CHECK_ARG(rows > 0 && dim > 0 && dim % 4 == 0,
+                 "byol_loss_rows_fwd: need rows >= 1 and dim a positive multiple of 4 (rows=%d dim=%d)", rows, dim);
+  BYOL_CHECK_ARG(aligned16_host(q1) && aligned16_host(q2) && aligned16_host(z1) && aligned16_host(z2) &&
+                     aligned16_host(saved),
+                 "byol_loss_rows_fwd: q1, q2, z1, z2 and saved must be 16-byte aligned");
+  const int nb = (rows + kRowsPerBlock - 1) / kRowsPerBlock;
+  static_assert(sizeof(Fix128) == 3 * sizeof(double), "the block slots are carved from the Fix128 scratch");
+  Fix128* scratch = fix_scratch(stream, (nb + 2) / 3);
+  if (scratch == nullptr) return -2;
+  double* part = reinterpret_cast<double*>(scratch);
+  loss_rows_fwd_kernel<<<nb, 32 * kRowsPerBlock, 0, stream>>>(q1, q2, z1, z2, rows, dim / 4, saved, part);
+  loss_rows_finalize_kernel<<<1, 32, 0, stream>>>(part, nb, rows, loss);
+  return fix_done(stream, check_launch("loss_rows_fwd kernels"));
+}
+
+// dq1, dq2: [rows, dim] fp32 (16-byte aligned); grad_out: 1 float or null (1).
+extern "C" int byol_loss_rows_bwd(const float* q1, const float* q2, const float* z1, const float* z2,
+                                  const float* saved, const float* grad_out, float* dq1, float* dq2, int rows, int dim,
+                                  cudaStream_t stream) {
+  BYOL_CHECK_ARG(q1 && q2 && z1 && z2 && saved && dq1 && dq2, "byol_loss_rows_bwd: null pointer");
+  BYOL_CHECK_ARG(rows > 0 && dim > 0 && dim % 4 == 0,
+                 "byol_loss_rows_bwd: need rows >= 1 and dim a positive multiple of 4 (rows=%d dim=%d)", rows, dim);
+  BYOL_CHECK_ARG(aligned16_host(q1) && aligned16_host(q2) && aligned16_host(z1) && aligned16_host(z2) &&
+                     aligned16_host(saved) && aligned16_host(dq1) && aligned16_host(dq2),
+                 "byol_loss_rows_bwd: every array must be 16-byte aligned");
+  const int64_t n4 = (int64_t)rows * (dim / 4);
+  loss_rows_bwd_kernel<<<grid_for(n4, 256, 132 * 4), 256, 0, stream>>>(q1, q2, z1, z2, saved, grad_out, dq1, dq2,
+                                                                       n4, dim / 4, rows);
+  return check_launch("loss_rows_bwd_kernel");
 }
 
 // mean = fl(fl(one_minus_decay*x) + fl(decay*mean)), elementwise over n fp32 values

@@ -553,6 +553,35 @@ def loss_bwd(q1, q2, z1, z2, saved, grad_out, dq1, dq2):
     return dq1, dq2
 
 
+def _loss_rows_shape(q1, q2, z1, z2):
+    for t, nm in ((q1, "q1"), (q2, "q2"), (z1, "z1"), (z2, "z2")):
+        _chk(t, F32, nm)
+    if q1.dim() != 2 or any(t.shape != q1.shape for t in (q2, z1, z2)):
+        raise ValueError("the paper's loss needs four [rows, dim] tensors of one shape")
+    return q1.shape
+
+
+def loss_rows_fwd(q1, q2, z1, z2, loss, saved):
+    """The BYOL paper's loss of fp32 [rows, dim] predictions q and targets z (dim a multiple of 4): loss (fp32 [1]) =
+    mean over rows of |q1^ - z2^|^2 + |q2^ - z1^|^2, per-row L2-normalised; saved: fp32 [rows, 8] for the backward."""
+    rows, dim = _loss_rows_shape(q1, q2, z1, z2)
+    _chk(loss, F32, "loss"); _chk(saved, F32, "saved")
+    if saved.numel() != 8 * rows:
+        raise ValueError("saved must hold 8 floats per row")
+    check(lib.byol_loss_rows_fwd(_ptr(q1), _ptr(q2), _ptr(z1), _ptr(z2), rows, dim, _ptr(loss), _ptr(saved),
+                                 _stream()), "byol_loss_rows_fwd", kernels=2)
+    return loss
+
+
+def loss_rows_bwd(q1, q2, z1, z2, saved, grad_out, dq1, dq2):
+    """dq1, dq2 of loss_rows_fwd's loss, scaled by grad_out (fp32 [1], or None: 1)."""
+    rows, dim = _loss_rows_shape(q1, q2, z1, z2)
+    _chk(saved, F32, "saved"); _chk(grad_out, F32, "grad_out"); _chk(dq1, F32, "dq1"); _chk(dq2, F32, "dq2")
+    check(lib.byol_loss_rows_bwd(_ptr(q1), _ptr(q2), _ptr(z1), _ptr(z2), _ptr(saved), _ptr(grad_out), _ptr(dq1),
+                                 _ptr(dq2), rows, dim, _stream()), "byol_loss_rows_bwd")
+    return dq1, dq2
+
+
 def ema_update(x, mean, one_minus_decay, decay):
     """mean <- fl(fl(a*x) + fl(d*mean)) in place; a, d already rounded to fp32 by the caller."""
     _chk(x, F32, "x"); _chk(mean, F32, "mean")

@@ -13,7 +13,7 @@ import torch
 import torch.nn as nn
 
 from .lars import LARS  # noqa: F401 (re-exported)
-from .objective import cross_entropy_topk, loss_function
+from .objective import check_variant, cross_entropy_topk, loss_function
 
 
 def add_weight_decay(model, weight_decay=1e-5, skip_list=()):
@@ -76,13 +76,16 @@ def topk(output, target, topk=(1,)):
         return [out[1:2] if k == 1 else out[2:3] for k in topk]
 
 
-def train_step(model, optimizer, augmentation1, augmentation2, labels):
-    """One optimisation step exactly as the reference's loop body (main.py:589-624) orders it."""
+def train_step(model, optimizer, augmentation1, augmentation2, labels, loss_variant="reference"):
+    """One optimisation step exactly as the reference's loop body (main.py:589-624) orders it.  loss_variant selects
+    the BYOL objective (objective.loss_function's variant: "reference" or the paper's "byol")."""
+    check_variant(loss_variant)
     output_dict = model(augmentation1, augmentation2)
     byol_loss = loss_function(online_prediction1=output_dict['online_prediction1'],
                               online_prediction2=output_dict['online_prediction2'],
                               target_projection1=output_dict['target_projection1'],
-                              target_projection2=output_dict['target_projection2'])
+                              target_projection2=output_dict['target_projection2'],
+                              variant=loss_variant)
     # F.cross_entropy + metrics.topk on cat([labels, labels]) (main.py:591,596-598) in one kernel: row r of the
     # [2b, classes] logits uses labels[r % b], so the concatenated label vector is never materialised
     classifier_loss, acc1, acc5 = cross_entropy_topk(output_dict['linear_preds'], labels)

@@ -177,6 +177,18 @@ int byol_loss_fwd(const float* q1, const float* q2, const float* z1, const float
 int byol_loss_bwd(const float* q1, const float* q2, const float* z1, const float* z2, const float* saved,
                   const float* grad_out, float* dq1, float* dq2, int rows, int dim, byol_stream_t stream);
 
+/* ---- the BYOL paper's loss: per-row L2-normalised predictions and targets, one warp per sample ----
+ * r(x) = max(sum x^2, 1e-12)^(-1/2), x^ = r(x) x; loss = (1/rows) sum_i |q1^_i - z2^_i|^2 + |q2^_i - z1^_i|^2.
+ * q1, q2, z1, z2: [rows, dim] fp32 contiguous and 16-byte aligned, dim a positive multiple of 4.  loss: 1 float;
+ * saved: [rows, 8] floats (16-byte aligned) = r(q1), r(z2), c12, l12, r(q2), r(z1), c21, l21 per row (c = q^.u, or
+ * 0 for a clamped row; l the row's pair loss), consumed by byol_loss_rows_bwd.  A row with a NaN or inf element, or
+ * whose sum of squares overflows, has r = NaN.  Deterministic: the grid depends on rows only.
+ * dq = grad_out * 2/rows * r(q) * (u - c q^), u = q^ - z^ (grad_out may be null: 1).  No gradient reaches z. */
+int byol_loss_rows_fwd(const float* q1, const float* q2, const float* z1, const float* z2, int rows, int dim,
+                       float* loss, float* saved, byol_stream_t stream);
+int byol_loss_rows_bwd(const float* q1, const float* q2, const float* z1, const float* z2, const float* saved,
+                       const float* grad_out, float* dq1, float* dq2, int rows, int dim, byol_stream_t stream);
+
 /* ---- target network: replaces CosEMA.forward, main.py:159-162.  mean = fl(fl(a*x) + fl(d*mean)), bit-exact ---- */
 int byol_ema_update(const float* x, float* mean, float one_minus_decay, float decay, int64_t n,
                     byol_stream_t stream);
