@@ -543,7 +543,9 @@ extern "C" int byol_gn_bwd_reduce(const void* g, const void* x, const void* act,
   BYOL_CHECK_ARG(g && x && gamma && beta && stats && s12 && gn_shape_ok(N, HW, C), "byol_gn_bwd_reduce: bad args");
   BYOL_CHECK_ARG(mask_mode >= 0 && mask_mode <= 3 && (mask_mode < 2 || act), "byol_gn_bwd_reduce: bad mask_mode %d",
                  mask_mode);
-  BYOL_CHECK_ARG((dgamma == nullptr) == (dbeta == nullptr), "byol_gn_bwd_reduce: dgamma and dbeta go together");
+  // dgamma / dbeta are required: the kernel always accumulates the per-channel sums, and only their flush leaves the
+  // stream's scratch zeroed for a CUDA graph captured earlier on this stream (its replay does not clear the scratch)
+  BYOL_CHECK_ARG(dgamma && dbeta, "byol_gn_bwd_reduce: dgamma and dbeta are required");
   const GnGeom gm = gn_geom(HW, C);
   const int64_t ng2 = (int64_t)N * 2 * kGroups;
   const size_t red_bytes = (2 * kGroups + 2 * (size_t)C) * sizeof(Fix128);
@@ -558,13 +560,9 @@ extern "C" int byol_gn_bwd_reduce(const void* g, const void* x, const void* act,
                                                         stats, fx, fx + ng2, gm);
   if (check_launch("gn_bwd_reduce_kernel") != 0) return -100;
   if (fix_flush(fx, s12, ng2, stream) != 0) return -100;
-  if (dgamma != nullptr) {
-    if (fix_flush(fx + ng2, dbeta, C, stream) != 0) return -100;
-    if (fix_flush(fx + ng2 + C, dgamma, C, stream) != 0) return -100;
-    return fix_done(stream, 0);
-  }
-  // the channel sums are not wanted: the next fix_scratch on this stream zeroes them
-  return 0;
+  if (fix_flush(fx + ng2, dbeta, C, stream) != 0) return -100;
+  if (fix_flush(fx + ng2 + C, dgamma, C, stream) != 0) return -100;
+  return fix_done(stream, 0);
 }
 
 extern "C" int byol_gn_bwd_apply(const void* g, const void* x, const void* act, const float* gamma, const float* beta,

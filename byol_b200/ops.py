@@ -407,18 +407,75 @@ def col_sum(x2d, out):
 GN_GROUPS = 32
 
 
+def _chk_shape(t, dtype, shape, name):
+    """_chk, and t has exactly `shape` (nothing to check when t is None)."""
+    if t is None:
+        return
+    _chk(t, dtype, name)
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError("%s must have shape %s, got %s" % (name, tuple(shape), tuple(t.shape)))
+
+
+def _chk_bits(t, x, name):
+    """t (optional): contiguous CUDA uint8 mask bits of x, one bit per element of x."""
+    if t is None:
+        return
+    _chk(t, torch.uint8, name)
+    if t.numel() * 8 != x.numel():
+        raise ValueError("%s must hold %d mask bytes (one bit per element of x), got %d" % (name, x.numel() // 8,
+                                                                                           t.numel()))
+
+
+def _chk_gn(x, gamma, beta, stats, gamma_name="gamma", beta_name="beta", stats_name="stats"):
+    """x bf16 [N, ..., C]; gamma / beta fp32 [C]; stats fp32 [N, 32, 2].  Checked on the host only: these wrappers run
+    inside CUDA-graph capture, where a device sync is not allowed."""
+    _chk(x, BF16, "x")
+    if x.dim() < 2:
+        raise ValueError("x must be [N, ..., C], got shape %s" % (tuple(x.shape),))
+    n, c = x.shape[0], x.shape[-1]
+    for t, name in ((gamma, gamma_name), (beta, beta_name)):
+        if t is None:
+            raise ValueError("%s is required" % name)
+        _chk_shape(t, F32, (c,), name)
+    if stats is None:
+        raise ValueError("%s is required" % stats_name)
+    _chk_shape(stats, F32, (n, GN_GROUPS, 2), stats_name)
+    return n, c
+
+
+def _chk_act(act, x, mask_mode):
+    if mask_mode not in (0, 1, 2, 3):
+        raise ValueError("mask_mode must be 0, 1, 2 or 3, got %r" % (mask_mode,))
+    if mask_mode >= 2 and act is None:
+        raise ValueError("mask_mode %d needs act" % mask_mode)
+    if mask_mode == 3:
+        _chk_bits(act, x, "act")
+    elif mask_mode == 2:
+        _chk_shape(act, BF16, x.shape, "act")
+
+
+def _chk_ws(desc, num_rows, stats):
+    """desc: contiguous CUDA int64 [units, 5]; stats fp32 [num_rows, 2]."""
+    _chk(desc, torch.int64, "desc")
+    if desc.dim() != 2 or desc.shape[1] != 5 or desc.shape[0] < 1:
+        raise ValueError("desc must be [units, 5] with at least one unit, got shape %s" % (tuple(desc.shape),))
+    if int(num_rows) <= 0:
+        raise ValueError("num_rows must be positive, got %d" % int(num_rows))
+    _chk_shape(stats, F32, (int(num_rows), 2), "stats")
+
+
 def ws_fwd(flat, desc, num_rows, w_out, stats):
     """Standardise every weight row listed in `desc` (device int64 [units, 5] = src offset in flat, offset in w_out,
     Cout, fan-in, first row): w_out[row] = (w - mean) / sqrt(var + 1e-5) (biased variance); stats fp32 [rows, 2] =
     (mean, rstd)."""
-    _chk(flat, F32, "flat"); _chk(w_out, F32, "w_out"); _chk(stats, F32, "stats")
+    _chk(flat, F32, "flat"); _chk(w_out, F32, "w_out"); _chk_ws(desc, num_rows, stats)
     check(lib.byol_ws_fwd(_ptr(flat), _ptr(desc), desc.shape[0], int(num_rows), _ptr(w_out), _ptr(stats), _stream()),
           "byol_ws_fwd")
 
 
 def ws_bwd(dwhat, what, stats, desc, num_rows, grad):
     """grad[row] (flat fp32, at the row's src offset) += rstd * (dw^ - mean(dw^) - w^ * mean(dw^ * w^))."""
-    _chk(dwhat, F32, "dwhat"); _chk(what, F32, "what"); _chk(stats, F32, "stats"); _chk(grad, F32, "grad")
+    _chk(dwhat, F32, "dwhat"); _chk(what, F32, "what"); _chk(grad, F32, "grad"); _chk_ws(desc, num_rows, stats)
     check(lib.byol_ws_bwd(_ptr(dwhat), _ptr(what), _ptr(stats), _ptr(desc), desc.shape[0], int(num_rows), _ptr(grad),
                           _stream()), "byol_ws_bwd")
 
@@ -426,8 +483,9 @@ def ws_bwd(dwhat, what, stats, desc, num_rows, grad):
 def gn_stats(y, eps, out=None, sums64=None):
     """y bf16 [N, H, W, C] -> fp32 [N, 32, 2] (mean, rstd) per (image, group); sums64 (fp64 [N, 32, 2], optional)
     receives the sums and sums of squares."""
-    _chk(y, BF16, "y"); _chk(sums64, F64, "sums64")
+    _chk(y, BF16, "y")
     n, c = y.shape[0], y.shape[-1]
+    _chk_shape(out, F32, (n, GN_GROUPS, 2), "out"); _chk_shape(sums64, F64, (n, GN_GROUPS, 2), "sums64")
     if out is None:
         out = torch.empty((n, GN_GROUPS, 2), dtype=F32, device=y.device)
     check(lib.byol_gn_stats(_ptr(y), _ptr(out), _ptr(sums64), n, y.numel() // (n * c), c, float(eps), _stream()),
@@ -438,11 +496,15 @@ def gn_stats(y, eps, out=None, sums64=None):
 def gn_apply(x, gamma, beta, stats, relu, resid=None, rgn=None, out=None, mask_out=None):
     """act(x*scale + shift (+ resid | + GroupNorm(resid))) of bf16 [N, H, W, C] with scale = gamma*rstd, shift =
     beta - mean*scale per (image, channel); rgn = (gamma, beta, stats) of a GroupNorm-applied residual."""
-    _chk(x, BF16, "x"); _chk(resid, BF16, "resid"); _chk(mask_out, torch.uint8, "mask_out")
-    n, c = x.shape[0], x.shape[-1]
+    n, c = _chk_gn(x, gamma, beta, stats)
+    _chk_shape(resid, BF16, x.shape, "resid"); _chk_shape(out, BF16, x.shape, "out"); _chk_bits(mask_out, x, "mask_out")
+    rg, rb, rs = rgn if rgn is not None else (None, None, None)
+    if rgn is not None:
+        if resid is None:
+            raise ValueError("rgn needs resid")
+        _chk_gn(resid, rg, rb, rs, "rgamma", "rbeta", "rstats")
     if out is None:
         out = torch.empty_like(x)
-    rg, rb, rs = rgn if rgn is not None else (None, None, None)
     check(lib.byol_gn_apply(_ptr(x), _ptr(gamma), _ptr(beta), _ptr(stats), _ptr(resid), _ptr(rg), _ptr(rb), _ptr(rs),
                             _ptr(out), _ptr(mask_out), n, x.numel() // (n * c), c, int(relu), _stream()),
           "byol_gn_apply")
@@ -451,7 +513,7 @@ def gn_apply(x, gamma, beta, stats, relu, resid=None, rgn=None, out=None, mask_o
 
 def gn_relu_maxpool_fwd(x, gamma, beta, stats, k=3, s=2, p=1, want_idx=True):
     """maxpool(relu(GroupNorm(x))) in one pass (stem); bit-identical to gn_apply(relu) + maxpool_fwd."""
-    _chk(x, BF16, "x")
+    _chk_gn(x, gamma, beta, stats)
     n, h, w, c = x.shape
     ho, wo = conv_out_size(h, k, s, p), conv_out_size(w, k, s, p)
     y = torch.empty((n, ho, wo, c), dtype=BF16, device=x.device)
@@ -461,22 +523,30 @@ def gn_relu_maxpool_fwd(x, gamma, beta, stats, k=3, s=2, p=1, want_idx=True):
     return y, idx
 
 
-def gn_bwd_reduce(g, x, gamma, beta, stats, s12, mask_mode, act=None, dgamma=None, dbeta=None):
-    """s12 (zeroed fp32 [N, 32, 2]) += per (image, group) [sum gamma*dz, sum gamma*dz*xhat]; dgamma / dbeta += the
-    per-channel sums dz*xhat / dz.  mask_mode as bn_bwd_reduce."""
-    _chk(g, BF16, "g"); _chk(x, BF16, "x"); _chk(act, torch.uint8 if mask_mode == 3 else BF16, "act")
-    _chk(s12, F32, "s12")
-    n, c = x.shape[0], x.shape[-1]
+def gn_bwd_reduce(g, x, gamma, beta, stats, s12, mask_mode, dgamma, dbeta, act=None):
+    """s12 (zeroed fp32 [N, 32, 2]) += per (image, group) [sum gamma*dz, sum gamma*dz*xhat]; dgamma / dbeta (fp32 [C],
+    required) += the per-channel sums dz*xhat / dz.  mask_mode as bn_bwd_reduce."""
+    n, c = _chk_gn(x, gamma, beta, stats)
+    _chk_shape(g, BF16, x.shape, "g"); _chk_act(act, x, mask_mode)
+    for t, name in ((s12, "s12"), (dgamma, "dgamma"), (dbeta, "dbeta")):
+        if t is None:
+            raise ValueError("%s is required" % name)
+    _chk_shape(s12, F32, (n, GN_GROUPS, 2), "s12")
+    _chk_shape(dgamma, F32, (c,), "dgamma"); _chk_shape(dbeta, F32, (c,), "dbeta")
     check(lib.byol_gn_bwd_reduce(_ptr(g), _ptr(x), _ptr(act), _ptr(gamma), _ptr(beta), _ptr(stats), _ptr(s12),
                                  _ptr(dgamma), _ptr(dbeta), n, x.numel() // (n * c), c, mask_mode, _stream()),
-          "byol_gn_bwd_reduce", kernels=2 if dgamma is None else 4)
+          "byol_gn_bwd_reduce", kernels=4)
     return s12
 
 
 def gn_bwd_apply(g, x, gamma, beta, stats, s12, mask_mode, act=None, dy=None, dz_out=None):
     """dy = rstd*(gamma*dz - s1/m - xhat*s2/m) per (image, group), m = H*W*C/32; dz_out (optional) receives dz."""
-    _chk(g, BF16, "g"); _chk(x, BF16, "x"); _chk(act, torch.uint8 if mask_mode == 3 else BF16, "act")
-    n, c = x.shape[0], x.shape[-1]
+    n, c = _chk_gn(x, gamma, beta, stats)
+    _chk_shape(g, BF16, x.shape, "g"); _chk_act(act, x, mask_mode)
+    if s12 is None:
+        raise ValueError("s12 is required")
+    _chk_shape(s12, F32, (n, GN_GROUPS, 2), "s12")
+    _chk_shape(dy, BF16, x.shape, "dy"); _chk_shape(dz_out, BF16, x.shape, "dz_out")
     if dy is None:
         dy = torch.empty_like(x)
     check(lib.byol_gn_bwd_apply(_ptr(g), _ptr(x), _ptr(act), _ptr(gamma), _ptr(beta), _ptr(stats), _ptr(s12), _ptr(dy),

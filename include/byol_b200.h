@@ -116,8 +116,8 @@ int byol_gn_apply(const void* x, const float* gamma, const float* beta, const fl
 /* stem fusion: y = maxpool(relu(gn(x))); values and argmax indices equal byol_gn_apply + byol_maxpool_fwd */
 int byol_gn_relu_maxpool_fwd(const void* x, const float* gamma, const float* beta, const float* stats, void* y,
                              void* idx, int N, int H, int W, int C, int k, int s, int p, byol_stream_t stream);
-/* s12 (zeroed fp32 [N][32][2]) += per (image, group) (sum gamma*dz, sum gamma*dz*xhat); dgamma / dbeta (optional,
- * together) += per-channel sum dz*xhat / sum dz; mask_mode as byol_bn_bwd_reduce */
+/* s12 (zeroed fp32 [N][32][2]) += per (image, group) (sum gamma*dz, sum gamma*dz*xhat); dgamma / dbeta (required)
+ * += per-channel sum dz*xhat / sum dz; mask_mode as byol_bn_bwd_reduce */
 int byol_gn_bwd_reduce(const void* g, const void* x, const void* act, const float* gamma, const float* beta,
                        const float* stats, float* s12, float* dgamma, float* dbeta, int N, int HW, int C, int mask_mode,
                        byol_stream_t stream);

@@ -284,6 +284,67 @@ def bn_bwd_reduce_f32_case(dev, exact, g, m, c, mask_mode):
     return run, ref
 
 
+def gn_stats_case(dev, exact, g, n, h, w, c, big=False):
+    """GroupNorm statistics: fp64 (sum, sum of squares) per (image, group) in sums64 and (mean, rstd); big: every
+    value +-8192, so the sums of squares pass 2^45 (2^26 per value)"""
+    from byol_b200 import ops
+    from tests.util import gn_finalize_restated
+    y = _vals((n, h, w, c), exact, g, 3)
+    if big:
+        y = torch.where(torch.rand((n, h, w, c), generator=g) < 0.5, 8192.0, -8192.0)
+    yd = y.to(dev, BF)
+    cnt = h * w * (c // 32)
+
+    def run():
+        sums = torch.zeros((n, 32, 2), dtype=F64, device=dev)
+        st = ops.gn_stats(yd, 1e-5, sums64=sums)
+        return [st, sums]
+
+    def ref(o):
+        v = y.double().reshape(n, -1, 32, c // 32)
+        sums = torch.stack([v.sum((1, 3)), (v * v).sum((1, 3))], -1)
+        st = torch.from_numpy(gn_finalize_restated(sums.numpy(), float(cnt), 1e-5)).double()
+        return [("sums64", o[1], sums), ("stats", o[0], st)]
+    return run, ref
+
+
+def gn_bwd_reduce_case(dev, exact, g, n, h, w, c, mask_mode, big=False):
+    """GroupNorm-backward sums: s12 [n, 32, 2] += (sum gamma*dz, sum gamma*dz*xhat) per (image, group), dbeta / dgamma
+    [c] += sum dz / sum dz*xhat per channel; big: dz = xhat = +-8192, so the channel sums pass 2^45"""
+    from byol_b200 import ops
+    gy, x = _vals((n, h, w, c), exact, g, 3), _vals((n, h, w, c), exact, g, 3)
+    if big:
+        gy = torch.full((n, h, w, c), 8192.0)
+        x = torch.where(torch.rand((n, h, w, c), generator=g) < 0.95, 8192.0, -8192.0)
+    if exact:
+        gamma = torch.pow(2.0, torch.randint(-1, 2, (c,), generator=g).float())
+        mean = torch.randint(-2, 3, (n, 32), generator=g).float() * (not big)
+        rstd = torch.pow(2.0, torch.randint(-1, 2, (n, 32), generator=g).float()) if not big else torch.ones(n, 32)
+    else:
+        gamma, mean, rstd = torch.rand(c, generator=g) + 0.5, torch.randn(n, 32, generator=g) * 0.1, \
+            torch.rand(n, 32, generator=g) + 0.5
+    act = _vals((n, h, w, c), exact, g, 2) if mask_mode == 2 else None
+    st = torch.stack([mean, rstd], -1).to(dev)
+    gd, xd, gmd, bd = gy.to(dev, BF), x.to(dev, BF), gamma.to(dev), torch.zeros(c, device=dev)
+    actd = act.to(dev, BF) if act is not None else None
+
+    def run():
+        s12, dg, db = torch.zeros((n, 32, 2), device=dev), torch.zeros(c, device=dev), torch.zeros(c, device=dev)
+        ops.gn_bwd_reduce(gd, xd, gmd, bd, st, s12, mask_mode, dgamma=dg, dbeta=db, act=actd)
+        return [s12, dg, db]
+
+    def ref(o):
+        grp = torch.arange(c) // (c // 32)
+        dz = gy.double() * ((act > 0).double() if act is not None else 1.0)
+        xh = (x.double() - mean.double()[:, grp].view(n, 1, 1, c)) * rstd.double()[:, grp].view(n, 1, 1, c)
+        gdz = gamma.double() * dz
+        s1 = gdz.reshape(n, -1, 32, c // 32).sum((1, 3))
+        s2 = (gdz * xh).reshape(n, -1, 32, c // 32).sum((1, 3))
+        return [("s12", o[0], torch.stack([s1, s2], -1)), ("dgamma", o[1], (dz * xh).sum((0, 1, 2))),
+                ("dbeta", o[2], dz.sum((0, 1, 2)))]
+    return run, ref
+
+
 def augment_case(dev, exact, g, n, hs, ws, r):
     from byol_b200.augment import TwoViewAugment
     imgs = torch.rand(n, 3, hs, ws, generator=g).to(dev)
@@ -333,6 +394,14 @@ EXACT = {
     "bn_bwd_reduce_f32_m1_c300": (bn_bwd_reduce_f32_case, dict(m=2999, c=300, mask_mode=1)),
     "bn_bwd_reduce_f32_m3_c264": (bn_bwd_reduce_f32_case, dict(m=5003, c=264, mask_mode=3)),
     "bn_bwd_reduce_f32_m3_c64": (bn_bwd_reduce_f32_case, dict(m=REAL_M + 37 * 8, c=64, mask_mode=3)),
+    # GroupNorm: C/8 dividing 256 (a thread stays on one vector) and not (it changes vector every iteration), the
+    # 224 px stem map (13 blocks per image, the last one short), and totals past 2^45
+    "gn_stats_stem224": (gn_stats_case, dict(n=3, h=112, w=112, c=64)),
+    "gn_stats_c96": (gn_stats_case, dict(n=3, h=30, w=26, c=96)),
+    "gn_stats_past_2^45": (gn_stats_case, dict(n=1, h=1024, w=512, c=64, big=True)),
+    "gn_bwd_reduce_stem224": (gn_bwd_reduce_case, dict(n=3, h=112, w=112, c=64, mask_mode=0)),
+    "gn_bwd_reduce_c96": (gn_bwd_reduce_case, dict(n=3, h=30, w=26, c=96, mask_mode=2)),
+    "gn_bwd_reduce_past_2^45": (gn_bwd_reduce_case, dict(n=3, h=512, w=512, c=64, mask_mode=0, big=True)),
 }
 
 # smaller shapes for the run-to-run checks (four launches each, plus a graph capture)
@@ -355,6 +424,10 @@ BITS = {
     "loss_fwd": (loss_case, dict(rows=512, dim=256)),
     "stats_f32": (stats_f32_case, dict(m=50000, c=64)),
     "augment": (augment_case, dict(n=8, hs=96, ws=128, r=64)),
+    "gn_stats": (gn_stats_case, dict(n=3, h=112, w=112, c=64)),
+    "gn_stats_c96": (gn_stats_case, dict(n=3, h=30, w=26, c=96)),
+    "gn_bwd_reduce": (gn_bwd_reduce_case, dict(n=3, h=112, w=112, c=64, mask_mode=0)),
+    "gn_bwd_reduce_c96": (gn_bwd_reduce_case, dict(n=3, h=30, w=26, c=96, mask_mode=2)),
 }
 
 
@@ -640,3 +713,39 @@ def test_two_streams_flush_into_one_destination(cuda):
     torch.cuda.synchronize()
     assert torch.equal(ab[0], ba[0]) and torch.equal(ab[1], ba[1])
     assert torch.equal(st, ab[0]) and torch.equal(dw, ab[1])
+
+
+def test_gradient_less_gn_bwd_reduce_cannot_dirty_a_captured_scratch(cuda):
+    """gn_bwd_reduce always accumulates its per-channel sums in the stream's scratch; only their flush into dgamma /
+    dbeta leaves those slots at zero.  A graph captured earlier on the stream holds no memset (its scratch was clean
+    and large enough at capture), so a call that left the channel sums behind would corrupt the replay of a captured
+    gn_stats.  The C entry point refuses a call without dgamma / dbeta before it takes the scratch: the replay keeps
+    the eager bits."""
+    from byol_b200 import ops
+    gen = _gen(11)
+    n, h, w, c = 4, 8, 8, 64
+    y = (torch.randn((n, h, w, c), generator=gen) * 2 + 0.5).to(cuda, BF)
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        ops.gn_stats(y, 1e-5)                          # the stream's scratch exists and is clean before the capture
+    torch.cuda.synchronize()
+    sums = torch.zeros((n, 32, 2), dtype=F64, device=cuda)
+    g = torch.cuda.CUDAGraph()
+    with _capture(g, s):
+        st = ops.gn_stats(y, 1e-5, sums64=sums)
+    with torch.cuda.stream(s):
+        eager_sums = torch.zeros_like(sums)
+        eager = ops.gn_stats(y, 1e-5, sums64=eager_sums)
+        x1, g1 = y[:1], (torch.randn((1, h, w, c), generator=gen)).to(cuda, BF)
+        gamma, beta = torch.ones(c, device=cuda), torch.zeros(c, device=cuda)
+        st1, s12 = eager[:1].contiguous(), torch.zeros((1, 32, 2), device=cuda)
+        rc = ops.lib.byol_gn_bwd_reduce(g1.data_ptr(), x1.data_ptr(), None, gamma.data_ptr(), beta.data_ptr(),
+                                        st1.data_ptr(), s12.data_ptr(), None, None, 1, h * w, c, 0, s.cuda_stream)
+    torch.cuda.synchronize()
+    g.replay()
+    torch.cuda.synchronize()
+    bad = int((sums != eager_sums).any(-1).sum())
+    assert torch.equal(sums, eager_sums) and torch.equal(st, eager), \
+        "the replayed gn_stats read leftover sums in %d of %d (image, group) slots" % (bad, n * 32)
+    assert rc != 0, "byol_gn_bwd_reduce without dgamma / dbeta must be refused"

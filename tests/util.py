@@ -63,6 +63,30 @@ def fma32(a, b, c):
     return s.astype(np.float32)
 
 
+def gn_finalize_restated(sums, count, eps):
+    """csrc/groupnorm.cu gn_finalize_kernel as compiled, from fp64 (sum, sum of squares) [..., 2]: mean = s / count and
+    q / count correctly rounded fp64 divisions, var = q/count - mean*mean contracted to one DFMA (rounded once), clamped
+    at 0, rstd = 1.0 / sqrt(var + eps) (fp64 IEEE sqrt and division, eps the fp32 value widened); both rounded once to
+    fp32.  Returns fp32 [..., 2] (mean, rstd)."""
+    sums = np.asarray(sums, dtype=np.float64)
+    s, q = sums[..., 0].reshape(-1), sums[..., 1].reshape(-1)
+    eps = float(np.float32(eps))
+    out = np.empty((s.size, 2), dtype=np.float32)
+    for i in range(s.size):
+        mean = s[i] / count
+        qc = q[i] / count
+        if np.isfinite(mean) and np.isfinite(qc):
+            var = float(Fraction(qc) - Fraction(mean) * Fraction(mean))
+        else:
+            with np.errstate(invalid="ignore"):
+                var = qc - mean * mean
+        var = 0.0 if var < 0.0 else var
+        out[i, 0] = np.float32(mean)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            out[i, 1] = np.float32(1.0 / np.sqrt(np.float64(var) + eps))
+    return out.reshape(sums.shape[:-1] + (2,))
+
+
 def pack_bits(keep):
     """bool [..., C] -> uint8 bits, element i of the flat index space in bit i % 8 of byte i // 8 (bn_apply's mask)."""
     k = keep.reshape(-1, 8).to(torch.int32) * (2 ** torch.arange(8, dtype=torch.int32, device=keep.device))
