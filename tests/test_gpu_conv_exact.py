@@ -17,7 +17,9 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from tests.util import gen as _gen, ints as _ints, pack_bits as _pack, report_mismatch
+from tests.exact import (Case, byol_train_step, check_in_fresh_process, check_row_launches, conv64, dgrad64, expect,
+                         nchw, nhwc, recording, replay, rounded_like, row_case, run_and_check, wgrad64)
+from tests.util import ints as _ints, pack_bits as _pack
 
 pytestmark = pytest.mark.gpu
 BF = torch.bfloat16
@@ -38,57 +40,20 @@ def _colstats(y2d):
     return torch.cat([y.sum(0), (y * y).sum(0)])
 
 
-def _nchw(t):
-    return t.permute(0, 3, 1, 2)
-
-
-def _nhwc(t):
-    return t.permute(0, 2, 3, 1)
-
-
-def _conv64(x, w, s, p, groups=1):
-    with torch.backends.cudnn.flags(enabled=False):
-        return _nhwc(F.conv2d(_nchw(x), w, None, s, p, 1, groups))
-
-
-def _dgrad64(dy, w, h, wd, s, p, groups=1):
-    n, cin = dy.shape[0], w.shape[1] * groups
-    with torch.backends.cudnn.flags(enabled=False):
-        return _nhwc(torch.nn.grad.conv2d_input((n, cin, h, wd), w, _nchw(dy), s, p, 1, groups))
-
-
-def _wgrad64(x, dy, wshape, s, p, groups=1):
-    with torch.backends.cudnn.flags(enabled=False):
-        return torch.nn.grad.conv2d_weight(_nchw(x), wshape, _nchw(dy), s, p, 1, groups)
-
-
-def _want(got, ref64):
-    """The float64 reference rounded once to the kernel's output dtype."""
-    if got.dtype == torch.bool:
-        return ref64.bool()
-    return ref64.float() if got.dtype == torch.float32 else ref64.float().to(BF)
+def _bad_parities(got, want):
+    """NHWC: which (h, w) parities hold the bad pixels."""
+    if got.dim() != 4:
+        return ""
+    bad = (got.float() != want.float()).any(-1)
+    hh = torch.arange(bad.shape[1], device=bad.device).view(1, -1, 1) % 2
+    ww = torch.arange(bad.shape[2], device=bad.device).view(1, 1, -1) % 2
+    per = {"%d%d" % (a, b): int((bad & (hh == a) & (ww == b)).sum()) for a in (0, 1) for b in (0, 1)}
+    return " | bad pixels by (h %% 2, w %% 2): %s of %d each" % (per, bad.numel() // 4)
 
 
 def _expect(name, got, ref64):
-    want = _want(got, ref64).reshape(got.shape)
-    if torch.equal(got, want):
-        return
-    _, msg = report_mismatch(name, got.float(), want.float(), 0.0, 0.0)
-    if got.dim() == 4:      # NHWC: which (h, w) parities hold the bad pixels
-        bad = (got.float() != want.float()).any(-1)
-        hh = torch.arange(bad.shape[1], device=bad.device).view(1, -1, 1) % 2
-        ww = torch.arange(bad.shape[2], device=bad.device).view(1, 1, -1) % 2
-        per = {"%d%d" % (a, b): int((bad & (hh == a) & (ww == b)).sum()) for a in (0, 1) for b in (0, 1)}
-        msg += " | bad pixels by (h %% 2, w %% 2): %s of %d each" % (per, bad.numel() // 4)
-    raise AssertionError(msg)
-
-
-class Case:
-    """run() launches the kernel(s) on fresh outputs and returns them; check(outs) compares them with float64;
-    route: the kernel the host is expected to pick (ROUTE_KERNEL), parity: whether parity mode is expected."""
-
-    def __init__(self, run, check, route, parity=False):
-        self.run, self.check, self.route, self.parity = run, check, route, parity
+    """torch.equal: a NaN output fails even where the reference is NaN."""
+    expect(name, got, ref64, equal=torch.equal, note=_bad_parities)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -178,7 +143,7 @@ def fprop_case(dev, g, n, h, w, c, cout, k, s, p, bias=False, resid=False, stats
 
     def check(outs):
         y, st = outs
-        ref = _conv64(x, wt, s, p, c // cin)
+        ref = conv64(x, wt, s, p, c // cin)
         if bias:
             ref = ref + b
         if resid:
@@ -187,7 +152,7 @@ def fprop_case(dev, g, n, h, w, c, cout, k, s, p, bias=False, resid=False, stats
             ref = torch.relu(ref)
         _expect("y", y, ref.reshape(y.shape))
         if stats:
-            _expect("stats", st, _colstats(_want(y, ref).reshape(-1, cout)))
+            _expect("stats", st, _colstats(rounded_like(y, ref).reshape(-1, cout)))
 
     route, parity = igemm_route(False, n, h, w, c, ho, wo, cout, k, s, p, resid=resid, bias=bias, stats=stats,
                                 relu=relu, out_fp32=out_fp32, gather=gather, grouped=bool(cg))
@@ -224,7 +189,7 @@ def dgrad_case(dev, g, n, h, w, cin, cout, k, s, p, resid=None, gather=False, cg
                                resid_up=resid == "up")]
 
     def check(outs):
-        ref = _dgrad64(dy, wt, h, w, s, p, cout // wcin if cg else 1)
+        ref = dgrad64(dy, wt, h, w, s, p, cout // wcin if cg else 1)
         if resid == "up":
             ref[:, ::2, ::2, :] += r
         elif resid == "mask":
@@ -262,9 +227,9 @@ def wgrad_case(dev, g, n, h, w, c, cin_real, cout, k, s, p, ldy=None, gather=Fal
     def check(outs):
         buf = outs[0]
         if grouped:
-            ref = _wgrad64(x, dy, dw0.shape, s, p, c // cin_real)
+            ref = wgrad64(x, dy, dw0.shape, s, p, c // cin_real)
         else:
-            ref = _wgrad64(x[..., :cin_real], dy, dw0.shape, s, p)
+            ref = wgrad64(x[..., :cin_real], dy, dw0.shape, s, p)
         _expect("dw", buf[guard:guard + numel].view(dw0.shape), ref + dw0)
         margins = torch.cat([buf[:guard], buf[guard + numel:]])
         assert bool((margins == 7.0).all()), "wgrad wrote outside dw"
@@ -284,10 +249,10 @@ def stem_fprop_case(dev, g, n, h, w, stats=False):
 
     def check(outs):
         with torch.backends.cudnn.flags(enabled=False):
-            ref = _nhwc(F.conv2d(x, wt, None, 2, 3))
+            ref = nhwc(F.conv2d(x, wt, None, 2, 3))
         _expect("y", outs[0], ref)
         if stats:
-            _expect("stats", outs[1], _colstats(_want(outs[0], ref).reshape(-1, 64)))
+            _expect("stats", outs[1], _colstats(rounded_like(outs[0], ref).reshape(-1, 64)))
     return Case(run, check, "stem")
 
 
@@ -305,7 +270,7 @@ def stem_wgrad_case(dev, g, n, h, w, cin):
 
     def check(outs):
         with torch.backends.cudnn.flags(enabled=False):
-            ref = torch.nn.grad.conv2d_weight(x, dw0.shape, _nchw(dy), 2, 3)
+            ref = torch.nn.grad.conv2d_weight(x, dw0.shape, nchw(dy), 2, 3)
         _expect("dw", outs[0], ref + dw0)
     return Case(run, check, "stem")
 
@@ -417,50 +382,38 @@ ROWS = {
 }
 
 
-def _build(name, dev):
-    _, builder, kw = ROWS[name]
-    return builder(dev, _gen(dev, sum(map(ord, name))), **kw)
+def _build(dev, name):
+    return row_case(dev, name, *ROWS[name][1:])
 
 
 @pytest.mark.parametrize("name", list(ROWS))
 def test_route_exact(cuda, name):
-    case = _build(name, cuda)
-    outs = case.run()
-    torch.cuda.synchronize()
-    case.check(outs)
+    run_and_check(_build(cuda, name))
 
 
-def _kernel_names(run):
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        run()
-        torch.cuda.synchronize()
-    return [e.name.replace(" ", "") for e in prof.events() if "kernel" in e.name]
+def _check_launches():
+    cases = {name: _build(torch.device("cuda:0"), name) for name in ROWS}
+
+    def complaints(name, launched):
+        case, want = cases[name], ROWS[name][0]
+        parity = want == "parity" or want.endswith("_parity")
+        route = "gather" if want == "parity" else want[:-len("_parity")] if parity else want
+        wrong = []
+        if (case.route, case.parity) != (route, parity):
+            wrong.append("%s: the host predicate gives %s%s, the row is meant for %s" % (
+                name, case.route, " (parity)" if case.parity else "", want))
+        if not any(re.search(ROUTE_KERNEL[route], k) for k in launched):
+            wrong.append("%s: expected %s, launched %s" % (name, ROUTE_KERNEL[route], sorted(set(launched))))
+        return wrong
+    check_row_launches({name: case.run for name, case in cases.items()}, complaints)
 
 
 def test_routes_launch_their_kernels(cuda):
     """Each row runs the kernel it is meant for.  Parity mode and the gathered operand share conv_igemm_kernel: for
-    those rows the restated host predicate (igemm_route, after conv_igemm_impl) decides."""
-    cases = {name: _build(name, cuda) for name in ROWS}
-    for case in cases.values():          # first launches (shared-memory opt-in, scratch) outside the profiler
-        case.run()
-    torch.cuda.synchronize()
-    wrong = []
-    seen_any = False
-    for name, case in cases.items():
-        want = ROWS[name][0]
-        parity = want == "parity" or want.endswith("_parity")
-        route = "gather" if want == "parity" else want[:-len("_parity")] if parity else want
-        if (case.route, case.parity) != (route, parity):
-            wrong.append("%s: the host predicate gives %s%s, the row is meant for %s" % (
-                name, case.route, " (parity)" if case.parity else "", want))
-        names = _kernel_names(case.run)
-        seen_any = seen_any or bool(names)
-        if names and not any(re.search(ROUTE_KERNEL[route], k) for k in names):
-            wrong.append("%s: expected %s, launched %s" % (name, ROUTE_KERNEL[route], sorted(set(names))))
-    if not seen_any:
-        pytest.skip("torch.profiler recorded no CUDA kernel events on this system")
-    assert not wrong, "\n".join(wrong)
+    those rows the restated host predicate (igemm_route, after conv_igemm_impl) decides.  Checked in a fresh Python
+    process: one that has already held many profiler sessions (the rest of the GPU suite) can drop CUDA kernel
+    events."""
+    check_in_fresh_process(__name__)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -492,31 +445,6 @@ def _recorders(calls):
         calls.add(("stem_conv_wgrad", xs4.shape[0], h, w, dw.shape[1]))
     return dict(conv_fprop=conv_fprop, conv_dgrad=conv_dgrad, conv_wgrad=conv_wgrad,
                 stem_conv_fprop=stem_conv_fprop, stem_conv_wgrad=stem_conv_wgrad)
-
-
-def _record_step(monkeypatch, dev, arch, rep, b, r):
-    from byol_b200 import ops, wiring
-    from byol_b200.model import BYOL
-    calls = set()
-    with monkeypatch.context() as mp:
-        for name, rec in _recorders(calls).items():
-            orig = getattr(ops, name)
-
-            def wrapped(*a, _orig=orig, _rec=rec, **k):
-                _rec(*a, **k)
-                return _orig(*a, **k)
-            mp.setattr(ops, name, wrapped)
-        torch.manual_seed(5)
-        model = BYOL(rep, 256, 1000, 10, arch=arch).to(dev).train()
-        model._engine.use_graphs = False
-        g = torch.Generator().manual_seed(6)
-        a1, a2 = torch.rand(b, 3, r, r, generator=g).to(dev), torch.rand(b, 3, r, r, generator=g).to(dev)
-        lab = torch.randint(0, 1000, (b,), generator=g).to(dev)
-        opt = wiring.build_optimizer(model, global_batch_size=256)
-        wiring.train_step(model, opt, a1, a2, lab)
-        torch.cuda.synchronize()
-    del model, opt
-    return calls
 
 
 def _replay_case(dev, g, sig, cg_by_c):
@@ -560,11 +488,12 @@ def _dgrad_sig_route(sig):
                        resid=resid is not None, mask=mask, up=up, gather=gather, grouped=len(ws) == 3)
 
 
-def test_replay_engine_calls_exactly(cuda, monkeypatch):
+def test_replay_engine_calls_exactly(cuda):
     calls = set()
-    for arch, rep, b, r in NETS:
-        calls |= _record_step(monkeypatch, cuda, arch, rep, b, r)
-        torch.cuda.empty_cache()
+    with recording(_recorders(calls)):
+        for arch, rep, b, r in NETS:
+            byol_train_step(cuda, arch, rep, b, r)
+            torch.cuda.empty_cache()
     dgrads = [sig for sig in calls if sig[0] == "conv_dgrad"]
     resid_routes = {_dgrad_sig_route(sig) for sig in dgrads if sig[9] is not None}
     # the replay must keep covering the residual epilogues where the backward pass joins its branches
@@ -575,15 +504,4 @@ def test_replay_engine_calls_exactly(cuda, monkeypatch):
     assert any(sig[12] for sig in dgrads), "no resid_up dgrad recorded"
     cg_by_c = {sig[1][3]: sig[3][1] for sig in calls
                if sig[0] == "conv_wgrad" and sig[3][1] < sig[1][3] and sig[1][3] % 64 == 0}
-    failures = []
-    for i, sig in enumerate(sorted(calls, key=repr)):
-        case = _replay_case(cuda, _gen(cuda, 1000 + i), sig, cg_by_c)
-        outs = case.run()
-        torch.cuda.synchronize()
-        try:
-            case.check(outs)
-        except AssertionError as e:
-            failures.append("%s: %s" % (sig, e))
-        del outs, case
-    print("replayed %d distinct calls" % len(calls))
-    assert not failures, "%d of %d replayed calls differ:\n%s" % (len(failures), len(calls), "\n".join(failures))
+    replay(cuda, calls, lambda dev, g, sig: _replay_case(dev, g, sig, cg_by_c), 1000)

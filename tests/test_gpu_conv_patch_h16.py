@@ -8,7 +8,9 @@ import re
 import pytest
 import torch
 
-from tests.test_gpu_conv_exact import _gen, _kernel_names, dgrad_case, fprop_case
+from tests.exact import check_in_fresh_process, check_row_launches, row_case, run_and_check
+from tests.test_gpu_conv_exact import dgrad_case, fprop_case
+from tests.util import gen
 
 pytestmark = pytest.mark.gpu
 
@@ -35,26 +37,23 @@ CASES = {
 
 def _case(dev, name):
     fprop, n, h, w, c, ndim = CASES[name]
-    g = _gen(dev, sum(map(ord, name)))
     if fprop:
-        return fprop_case(dev, g, n, h, w, c, ndim, 3, 1, 1, stats=True)
-    return dgrad_case(dev, g, n, h, w, ndim, c, 3, 1, 1)
+        return row_case(dev, name, fprop_case, dict(n=n, h=h, w=w, c=c, cout=ndim, k=3, s=1, p=1, stats=True))
+    return row_case(dev, name, dgrad_case, dict(n=n, h=h, w=w, cin=ndim, cout=c, k=3, s=1, p=1))
 
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_patch_h16_exact(cuda, name):
     case = _case(cuda, name)
     assert case.route == "patch"
-    outs = case.run()
-    torch.cuda.synchronize()
-    case.check(outs)
+    run_and_check(case)
 
 
 @pytest.mark.parametrize("c, ndim, hw", [(64, 64, 56), (128, 128, 28), (256, 256, 14), (64, 192, 30)])
 def test_patch_h16_stats_run_to_run(cuda, c, ndim, hw):
     """Statistics of real-valued data (inexact fp32 partial sums) are the same bits on every run."""
     from byol_b200 import ops
-    g = _gen(cuda, c + ndim + hw)
+    g = gen(cuda, c + ndim + hw)
     x = torch.randn(6, hw, hw, c, device=cuda, generator=g).to(torch.bfloat16)
     w_f, _ = ops.prep_weight(torch.randn(ndim, c, 3, 3, device=cuda, generator=g) / (3 * c ** 0.5), want_dgrad=False)
     runs = []
@@ -74,7 +73,7 @@ def test_patch_h16_matches_fp32_tile_kernel(cuda, c, ndim, h, w):
     64-column pair tiles, reached here through an all-zero residual: the same outputs, and the same statistics,
     which the 128-column tiles sum in the pair kernel's grouping."""
     from byol_b200 import ops
-    g = _gen(cuda, c + ndim + h)
+    g = gen(cuda, c + ndim + h)
     x = torch.randn(23, h, w, c, device=cuda, generator=g).to(torch.bfloat16)
     w_f, _ = ops.prep_weight(torch.randn(ndim, c, 3, 3, device=cuda, generator=g) / (3 * c ** 0.5), want_dgrad=False)
     zero = torch.zeros(23, h, w, ndim, device=cuda, dtype=torch.bfloat16)
@@ -121,18 +120,19 @@ def _launch(dev, fprop, n, h, w, c, ndim, stats=False, resid=False, relu=False, 
     return lambda: ops.conv_dgrad(x, wd, h, w, 3, 3, 1, 1, resid=r)
 
 
-def test_patch_variant_launched(cuda):
-    runs = {name: _launch(cuda, **kw) for name, (_, kw) in LAUNCHES.items()}
-    for run in runs.values():     # first launches (shared-memory opt-in, scratch) outside the profiler
-        run()
-    torch.cuda.synchronize()
-    wrong, seen_any = [], False
-    for name, run in runs.items():
-        names = [k for k in _kernel_names(run) if "conv3x3_patch_kernel" in k]
-        seen_any = seen_any or bool(_kernel_names(run))
+def _check_launches():
+    dev = torch.device("cuda:0")
+
+    def complaints(name, launched):
         want = LAUNCHES[name][0]
+        names = [k for k in launched if "conv3x3_patch_kernel" in k]
         if not any(re.search(re.escape(want), k) for k in names):
-            wrong.append("%s: expected %s, launched %s" % (name, want, sorted(set(names))))
-    if not seen_any:
-        pytest.skip("torch.profiler recorded no CUDA kernel events on this system")
-    assert not wrong, "\n".join(wrong)
+            return ["%s: expected %s, launched %s" % (name, want, sorted(set(names)))]
+        return []
+    check_row_launches({name: _launch(dev, **kw) for name, (_, kw) in LAUNCHES.items()}, complaints)
+
+
+def test_patch_variant_launched(cuda):
+    """Each kind of call launches its variant.  Checked in a fresh Python process: one that has already held many
+    profiler sessions (the rest of the GPU suite) can drop CUDA kernel events."""
+    check_in_fresh_process(__name__)

@@ -15,18 +15,16 @@
   options only; byol_avgpool_fwd at the ops.lib level, where the engine calls it) and replays every distinct call with
   exact operands.
 """
-import os
 import re
-import subprocess
-import sys
-from fractions import Fraction
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-from tests.util import _fma32, fma32, gen, ints, pack_bits, pow2, report_mismatch, unpack_bits
+from tests.exact import (Case, byol_train_step, check_in_fresh_process, check_row_launches, expect, expect_same,
+                         recording, replay, row_case, run_and_check)
+from tests.util import _fma32, fma32, fma64, gen, ints, pack_bits, pow2, unpack_bits
 
 pytestmark = pytest.mark.gpu
 BF, F32, F64, U8 = torch.bfloat16, torch.float32, torch.float64, torch.uint8
@@ -35,7 +33,7 @@ BF, F32, F64, U8 = torch.bfloat16, torch.float32, torch.float64, torch.uint8
 # ------------------------------------------------------------------------------------------------------------------
 # operands and comparison
 # ------------------------------------------------------------------------------------------------------------------
-def _acts(shape, dev, g, amp=4, big=0.05):
+def acts(shape, dev, g, amp=4, big=0.05):
     """fp64 integers in [-amp, amp]; a fraction `big` of them even integers of either sign in [256, 510] (exact in
     bf16, while their sums with small integers are not: the bf16 output rounding is exercised)."""
     v = ints(shape, dev, g, amp)
@@ -53,47 +51,6 @@ def _fine(shape, dev, g, amp=4):
 
 def _pos2(n, dev, g):
     return pow2(n, dev, g)
-
-
-def _want(got, ref64):
-    if got.dtype in (torch.bool, U8):
-        return ref64.to(got.dtype)
-    return ref64.float() if got.dtype == F32 else ref64.float().to(BF)
-
-
-def _same(a, b):
-    """torch.equal with NaN == NaN."""
-    if a.shape != b.shape or a.dtype != b.dtype:
-        return False
-    if not a.is_floating_point():
-        return torch.equal(a, b)
-    na, nb = torch.isnan(a), torch.isnan(b)
-    return torch.equal(na, nb) and torch.equal(torch.where(na, 0, a), torch.where(nb, 0, b))
-
-
-def _expect(name, got, ref64):
-    """got == ref64 rounded once to got's dtype."""
-    want = _want(got, ref64.reshape(got.shape))
-    if _same(got, want):
-        return
-    _, msg = report_mismatch(name, got.float().reshape(-1, got.shape[-1]), want.float().reshape(-1, got.shape[-1]),
-                             0.0, 0.0)
-    raise AssertionError(msg)
-
-
-def _expect_same(name, got, want):
-    if not _same(got, want):
-        _, msg = report_mismatch(name, got.float().reshape(-1, got.shape[-1]), want.float().reshape(-1, got.shape[-1]),
-                                 0.0, 0.0)
-        raise AssertionError(msg)
-
-
-class Case:
-    """run() launches the kernel under test on fresh outputs and returns them; check(outs) compares them with the
-    reference; route: the ROUTE_KERNEL key the restated host predicate picks."""
-
-    def __init__(self, run, check, route):
-        self.run, self.check, self.route = run, check, route
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -162,8 +119,8 @@ FAMILY = [_K + r"bn_apply(_fixed)?_kernel", _K + r"bn_bwd_apply(_fixed)?_kernel"
 def bn_apply_case(dev, g, m, c, resid=None, relu=False, mask=False, out=True, out_f32=False):
     """y = act(x*scale + shift (+ r | r*rscale + rshift)); resid None / "plain" / "affine"; any of y, y_f32, mask."""
     from byol_b200 import ops
-    x, sc, sh = _acts((m, c), dev, g), pow2(c, dev, g, signed=True), ints((c,), dev, g, 3)
-    r = _acts((m, c), dev, g) if resid else None
+    x, sc, sh = acts((m, c), dev, g), pow2(c, dev, g, signed=True), ints((c,), dev, g, 3)
+    r = acts((m, c), dev, g) if resid else None
     rs, rb = (pow2(c, dev, g, signed=True), ints((c,), dev, g, 3)) if resid == "affine" else (None, None)
     xd, rd = x.to(BF), (r.to(BF) if resid else None)
     f = [t.float() if t is not None else None for t in (sc, sh, rs, rb)]
@@ -183,9 +140,9 @@ def bn_apply_case(dev, g, m, c, resid=None, relu=False, mask=False, out=True, ou
         if relu:
             ref = torch.relu(ref)
         if out:
-            _expect("y", y, ref)
+            expect("y", y, ref)
         if out_f32:
-            _expect("y_f32", y32, ref)
+            expect("y_f32", y32, ref)
         if mask:
             assert torch.equal(unpack_bits(mo, (m, c)), ref > 0), "mask_out differs"
 
@@ -195,7 +152,7 @@ def bn_apply_case(dev, g, m, c, resid=None, relu=False, mask=False, out=True, ou
 
 
 def _bwd_operands(dev, g, m, c, mask_mode):
-    x, gr = _acts((m, c), dev, g), _acts((m, c), dev, g, 3)
+    x, gr = acts((m, c), dev, g), acts((m, c), dev, g, 3)
     mean, invstd, gamma = ints((c,), dev, g, 3), _pos2(c, dev, g), pow2(c, dev, g, signed=True)
     scale, shift = pow2(c, dev, g, signed=True), ints((c,), dev, g, 2)
     act = keep = None
@@ -240,12 +197,12 @@ def bn_bwd_apply_case(dev, g, m, c, mask_mode, dz_out=False, grads=False, count=
     def check(outs):
         dy, dzo, dg, db = outs
         xhat = (x - mean) * invstd
-        _expect("dy", dy, gamma * invstd * (dz - s1 / count - xhat * s2 / count))
+        expect("dy", dy, gamma * invstd * (dz - s1 / count - xhat * s2 / count))
         if dz_out:
-            _expect("dz", dzo, dz)
+            expect("dz", dzo, dz)
         if grads:
-            _expect("dgamma", dg, loc[0][c:] + loc[1][c:])
-            _expect("dbeta", db, loc[0][:c] + loc[1][:c])
+            expect("dgamma", dg, loc[0][c:] + loc[1][c:])
+            expect("dbeta", db, loc[0][:c] + loc[1][:c])
 
     fixed = fixed_grid(m * c // 8, c // 8) > 0
     return Case(run, check, ("bwd_apply_fixed%d" if fixed else "bwd_apply_generic%d") % mask_mode)
@@ -276,17 +233,13 @@ def bn_bwd_reduce_case(dev, g, m, c, mask_mode):
 
     def check(outs):
         dz = gr * keep if keep is not None else gr
-        _expect("s12", outs[0], torch.cat([dz.sum(0), (dz * (x - mean) * invstd).sum(0)]))
+        expect("s12", outs[0], torch.cat([dz.sum(0), (dz * (x - mean) * invstd).sum(0)]))
 
     fixed = fixed_grid(m * c // 8, c // 8) > 0
     return Case(run, check, ("reduce_fixed%d" if fixed else "reduce_rows%d") % mask_mode)
 
 
 # --- statistics -> coefficients: numpy restatement of the compiled arithmetic ------------------------------------
-def _fma64(a, b, c):
-    return np.array([float(Fraction(float(x)) * Fraction(float(y)) + Fraction(float(z))) for x, y, z in zip(a, b, c)])
-
-
 def finalize_restated(stats, count, gammas, betas, rm, rv, momentum, eps):
     """bn_finalize_lanes_kernel as compiled (fp64 statistics, fp32 coefficients; nvcc contracts
     q/n - mean^2, beta - mean*scale and both running-statistic updates into FMAs)."""
@@ -298,7 +251,7 @@ def finalize_restated(stats, count, gammas, betas, rm, rv, momentum, eps):
     for l in range(len(gammas)):
         st = stats[l * 2 * C:(l + 1) * 2 * C].astype(np.float64)
         mean = st[:C] / count
-        var = np.maximum(_fma64(-mean, mean, st[C:] / count), 0.0)
+        var = np.maximum(fma64(-mean, mean, st[C:] / count), 0.0)
         invstd = (1.0 / np.sqrt(var + np.float64(eps32))).astype(np.float32)
         sc = gammas[l] * invstd
         mean32 = mean.astype(np.float32)
@@ -382,10 +335,10 @@ def finalize_f64_restated(stats, count, gammas, betas, rm, rv, momentum, eps):
     for l in range(len(gammas)):
         st = stats[l * 2 * C:(l + 1) * 2 * C]
         mean = st[:C] / count
-        var = np.maximum(_fma64(-mean, mean, st[C:] / count), 0.0)
+        var = np.maximum(fma64(-mean, mean, st[C:] / count), 0.0)
         invstd = (1.0 / np.sqrt(var + np.float64(np.float32(eps)))).astype(np.float32)
         sc = gammas[l] * invstd
-        shift = _fma64(-mean, sc.astype(np.float64), betas[l].astype(np.float64)).astype(np.float32)
+        shift = fma64(-mean, sc.astype(np.float64), betas[l].astype(np.float64)).astype(np.float32)
         mean32 = mean.astype(np.float32)
         unb = var * count / (count - 1.0) if count > 1 else var
         rm = fma32(rm, one_m, mom * mean32)
@@ -423,7 +376,7 @@ def finalize_f64_case(dev, g, c, lanes, count, running=True, negvar=False, momen
                                                rv0.cpu().numpy(), momentum, eps)
         if negvar:
             m64 = st[:c] / cnt
-            assert (_fma64(-m64[:5], m64[:5], st[c:c + 5] / cnt) < 0).all(), "no negative variance to clamp"
+            assert (fma64(-m64[:5], m64[:5], st[c:c + 5] / cnt) < 0).all(), "no negative variance to clamp"
         checks = [("coeffs", co, want)] + ([("running_mean", rm, wrm), ("running_var", rv, wrv)] if running else [])
         for name, a, b in checks:
             bad = a.view(np.uint32) != b.view(np.uint32)
@@ -470,13 +423,13 @@ def _with_edges(x, k, s, p):
     return x
 
 
-def _aten_pool(x64, k, s, p):
+def aten_pool(x64, k, s, p):
     """float64 NHWC -> (values NHWC, flat input index h*W + w NHWC) of torch.nn.functional.max_pool2d."""
     y, i = F.max_pool2d(x64.permute(0, 3, 1, 2), k, s, p, return_indices=True)
     return y.permute(0, 2, 3, 1), i.permute(0, 2, 3, 1)
 
 
-def _flat_index(idx, w, k, s, p):
+def flat_index(idx, w, k, s, p):
     """window position (kh*k + kw) -> flat input index ih*W + iw, as ATen reports it."""
     n, ho, wo, c = idx.shape
     i = idx.long()
@@ -498,9 +451,9 @@ def maxpool_case(dev, g, n, h, w, c, k, s, p, edges=False, fp32=False):
 
     def check(outs):
         y, idx = outs
-        ry, ri = _aten_pool(x, k, s, p)
-        _expect("y", y, ry)
-        fi = _flat_index(idx, w, k, s, p)
+        ry, ri = aten_pool(x, k, s, p)
+        expect("y", y, ry)
+        fi = flat_index(idx, w, k, s, p)
         bad = fi != ri
         assert not bad.any(), "argmax differs at %d of %d outputs (first %s: %d vs ATen %d)" % (
             int(bad.sum()), bad.numel(), bad.nonzero()[0].tolist(), int(fi[bad][0]), int(ri[bad][0]))
@@ -512,7 +465,7 @@ def bnpool_case(dev, g, n, h, w, c, k, s, p, want_idx):
     """bn_relu_maxpool_fwd == bn_apply(relu) then maxpool_fwd, values and argmax bit for bit; values also against
     float64 (scales of both signs: many windows are all zeros after the ReLU)."""
     from byol_b200 import ops
-    x, sc, sh = _acts((n, h, w, c), dev, g), pow2(c, dev, g, signed=True), ints((c,), dev, g, 3)
+    x, sc, sh = acts((n, h, w, c), dev, g), pow2(c, dev, g, signed=True), ints((c,), dev, g, 3)
     x[-1, 1, 1, 3] = float("nan")         # NaN * scale + shift -> fmaxf(NaN, 0) = 0 on both paths
     xd, scf, shf = x.to(BF), sc.float(), sh.float()
 
@@ -523,11 +476,11 @@ def bnpool_case(dev, g, n, h, w, c, k, s, p, want_idx):
         y, idx = outs
         a = ops.bn_apply(xd.view(-1, c), scf, shf, True).view(n, h, w, c)
         y2, i2 = ops.maxpool_fwd(a, k, s, p)
-        _expect_same("y vs bn_apply + maxpool_fwd", y, y2)
+        expect_same("y vs bn_apply + maxpool_fwd", y, y2)
         if want_idx:
             assert torch.equal(idx, i2), "argmax differs from bn_apply + maxpool_fwd"
         a64 = torch.relu(torch.nan_to_num(x * sc + sh, nan=0.0)).float().to(BF).to(F64)
-        _expect("y", y, _aten_pool(a64, k, s, p)[0])
+        expect("y", y, aten_pool(a64, k, s, p)[0])
 
     return Case(run, check, "bnpool_idx" if want_idx else "bnpool_noidx")
 
@@ -550,11 +503,11 @@ def pool_bwd_case(dev, g, n, h, w, c, k, s, p, fp32=False):
         return [(ops.maxpool_bwd_f32 if fp32 else ops.maxpool_bwd)(dyd, idx, h, w, k, s, p)]
 
     def check(outs):
-        fi = _flat_index(idx, w, k, s, p).permute(0, 3, 1, 2).reshape(n, c, -1)
+        fi = flat_index(idx, w, k, s, p).permute(0, 3, 1, 2).reshape(n, c, -1)
         assert bool(((fi >= 0) & (fi < h * w)).all()), "a saved argmax points outside the image"
         ref = torch.zeros((n, c, h * w), dtype=F64, device=dev)
         ref.scatter_add_(2, fi, dy.permute(0, 3, 1, 2).reshape(n, c, -1))
-        _expect("dx", outs[0], ref.view(n, c, h, w).permute(0, 2, 3, 1))
+        expect("dx", outs[0], ref.view(n, c, h, w).permute(0, 2, 3, 1))
 
     if fp32:
         return Case(run, check, "maxpool_bwd_f32")
@@ -569,7 +522,7 @@ def _times_inv(v32, hw):
 def avgpool_case(dev, g, n, h, w, c, want_f32=True, want_bf16=True):
     """avgpool_fwd: fp32 sums of bf16 integers (exact), times fl(1/HW) -> fp32 RN(sum * RN(1/HW)), bf16 of that."""
     from byol_b200 import ops
-    x = _acts((n, h, w, c), dev, g)
+    x = acts((n, h, w, c), dev, g)
     xd = x.to(BF)
 
     def run():
@@ -582,9 +535,9 @@ def avgpool_case(dev, g, n, h, w, c, want_f32=True, want_bf16=True):
         if (h * w) & (h * w - 1) == 0:
             assert torch.equal(want.to(F64), sm / (h * w))        # a power of two: the average itself
         if want_f32:
-            _expect_same("y_f32", yf, want)
+            expect_same("y_f32", yf, want)
         if want_bf16:
-            _expect_same("y_bf16", yb, want.to(BF))
+            expect_same("y_bf16", yb, want.to(BF))
 
     return Case(run, check, "avgpool_fwd")
 
@@ -592,7 +545,7 @@ def avgpool_case(dev, g, n, h, w, c, want_f32=True, want_bf16=True):
 def avgpool_bwd_case(dev, g, n, h, w, c, ga=True, gb=True):
     """avgpool_bwd: dx = bf16(RN((g_a + g_b) * RN(1/HW))), g_a bf16, g_b fp32, either absent."""
     from byol_b200 import ops
-    a, b = _acts((n, c), dev, g), ints((n, c), dev, g, 5)
+    a, b = acts((n, c), dev, g), ints((n, c), dev, g, 5)
     ad, bf = (a.to(BF) if ga else None), (b.float() if gb else None)
 
     def run():
@@ -601,7 +554,7 @@ def avgpool_bwd_case(dev, g, n, h, w, c, ga=True, gb=True):
     def check(outs):
         v = (a if ga else 0) + (b if gb else 0)
         want = _times_inv(v.float(), h * w).to(BF)
-        _expect_same("dx", outs[0], want.view(n, 1, 1, c).expand(n, h, w, c).contiguous())
+        expect_same("dx", outs[0], want.view(n, 1, 1, c).expand(n, h, w, c).contiguous())
 
     return Case(run, check, "avgpool_bwd")
 
@@ -609,7 +562,7 @@ def avgpool_bwd_case(dev, g, n, h, w, c, ga=True, gb=True):
 def avgpool_f32_case(dev, g, n, h, w, c):
     """avgpool_f32: fp32 sum (exact for integers) divided by HW -> RN(sum / HW)."""
     from byol_b200 import ops
-    x = _acts((n, h, w, c), dev, g)
+    x = acts((n, h, w, c), dev, g)
     xf = x.float()
 
     def run():
@@ -617,21 +570,21 @@ def avgpool_f32_case(dev, g, n, h, w, c):
 
     def check(outs):
         want = x.sum((1, 2)).float().cpu() / float(h * w)       # IEEE fp32 division
-        _expect_same("y", outs[0].cpu(), want)
+        expect_same("y", outs[0].cpu(), want)
 
     return Case(run, check, "avgpool_f32")
 
 
 def avgpool_bwd_f32_case(dev, g, n, h, w, c, ga=True, gb=True):
     from byol_b200 import ops
-    a, b = _acts((n, c), dev, g).float(), ints((n, c), dev, g, 5).float()
+    a, b = acts((n, c), dev, g).float(), ints((n, c), dev, g, 5).float()
 
     def run():
         return [ops.avgpool_bwd_f32(a if ga else None, b if gb else None, n, h, w, c)]
 
     def check(outs):
         v = ((a if ga else 0) + (b if gb else 0)).cpu() / float(h * w)
-        _expect_same("dx", outs[0].cpu(), v.view(n, 1, 1, c).expand(n, h, w, c).contiguous())
+        expect_same("dx", outs[0].cpu(), v.view(n, 1, 1, c).expand(n, h, w, c).contiguous())
 
     return Case(run, check, "avgpool_bwd_f32")
 
@@ -737,14 +690,14 @@ def stem4_case(dev, g, n, cin, h, w):
 
 def subsample2_case(dev, g, n, h, w, c):
     from byol_b200 import ops
-    x = _acts((n, h, w, c), dev, g)
+    x = acts((n, h, w, c), dev, g)
     xd = x.to(BF)
 
     def run():
         return [ops.subsample2(xd)]
 
     def check(outs):
-        _expect("y", outs[0], x[:, ::2, ::2, :])
+        expect("y", outs[0], x[:, ::2, ::2, :])
 
     return Case(run, check, "subsample2")
 
@@ -774,7 +727,7 @@ def _check_plane_stack(name, got, x, pattern):
     where the pattern holds all three planes, they sum back to every finite x with |x| >= 2^-110 (or 0)."""
     pl = _split3(x)
     for j, a in enumerate(pattern):
-        _expect_same("%s plane %d" % (name, j), got[:, j].contiguous(), pl[a])
+        expect_same("%s plane %d" % (name, j), got[:, j].contiguous(), pl[a])
     if 2 in pattern:
         back = sum(got[:, pattern.index(a)].double() for a in range(3))
         keep = torch.isfinite(x) & ((x.abs() >= EXACT_FROM) | (x == 0))
@@ -814,7 +767,7 @@ def split_planes_case(dev, g, m, c, T, cpad=None, ldx=None, copy=False, guard=25
         assert _is_pos_zero(got[..., c:]), "split_planes: padding channels not +0"
         guards = [buf[:guard], buf[guard + m * T * cpad:]]
         if copy:
-            _expect_same("copy", cbuf[guard:guard + m * c].view(m, c), _split3(x)[0])
+            expect_same("copy", cbuf[guard:guard + m * c].view(m, c), _split3(x)[0])
             guards += [cbuf[:guard], cbuf[guard + m * c:]]
         assert all(bool(torch.isnan(t).all()) for t in guards), "split_planes wrote outside its outputs"
 
@@ -898,11 +851,11 @@ def apply_f32_case(dev, g, m, c, T, out32=True, planes=True, copy=False, mask=Fa
         ref32 = ref.float()
         assert torch.equal(ref32.double(), ref), "operands not exact in fp32"
         if out32:
-            _expect("out32", o32, ref)
+            expect("out32", o32, ref)
         if planes:
             _check_planes("planes", pl, ref32, T)
         if copy:
-            _expect_same("copy", cp, ref32.to(BF))
+            expect_same("copy", cp, ref32.to(BF))
         if mask:
             assert torch.equal(unpack_bits(mk, (m, c)), ref > 0), "mask differs"
 
@@ -939,13 +892,13 @@ def bwd_apply_f32_case(dev, g, m, c, mask_mode, T, want_f32=True, want_planes=Tr
         ref = gamma * invstd * (dzr - s12[:c] / count - (y - mean) * invstd * s12[c:] / count)
         assert torch.equal(ref.float().double(), ref), "operands not exact in fp32"
         if want_f32:
-            _expect("dy32", d32, ref)
+            expect("dy32", d32, ref)
         if want_planes:
             _check_planes("dy planes", pl, ref.float(), T)
         if want_dz:
-            _expect("dz", dz, dzr)
-        _expect("dgamma", dg, loc[0][c:] + loc[1][c:])
-        _expect("dbeta", db, loc[0][:c] + loc[1][:c])
+            expect("dz", dz, dzr)
+        expect("dgamma", dg, loc[0][c:] + loc[1][c:])
+        expect("dbeta", db, loc[0][:c] + loc[1][:c])
 
     return Case(run, check, "bwd_apply_f32_%d" % mask_mode)
 
@@ -1072,68 +1025,39 @@ ROWS["bwd_apply_f32_planes_only"] = ("bwd_apply_f32_3", bwd_apply_f32_case, dict
                                                                                  want_f32=False, want_dz=False))
 
 
-def _build(name, dev):
-    _, builder, kw = ROWS[name]
-    return builder(dev, gen(dev, sum(map(ord, name))), **kw)
+def _build(dev, name):
+    return row_case(dev, name, *ROWS[name][1:])
 
 
 @pytest.mark.parametrize("name", list(ROWS))
 def test_row_exact(cuda, name):
-    case = _build(name, cuda)
-    outs = case.run()
-    torch.cuda.synchronize()
-    case.check(outs)
-
-
-def _kernel_names(run):
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        run()
-        torch.cuda.synchronize()
-    return [e.name.replace(" ", "") for e in prof.events() if "kernel" in e.name]
+    run_and_check(_build(cuda, name))
 
 
 def _check_launches():
-    cases = {name: _build(name, torch.device("cuda:0")) for name in ROWS}
-    for case in cases.values():
-        case.run()
-    torch.cuda.synchronize()
-    wrong, seen_any = [], False
-    for name, case in cases.items():
-        want = ROWS[name][0]
+    cases = {name: _build(torch.device("cuda:0"), name) for name in ROWS}
+
+    def complaints(name, launched):
+        case, want = cases[name], ROWS[name][0]
+        wrong = []
         if case.route != want:
             wrong.append("%s: the restated host predicate gives %s, the row is meant for %s" % (name, case.route, want))
-        names = _kernel_names(case.run)
-        seen_any = seen_any or bool(names)
-        if not names:
-            continue
-        if not any(re.search(ROUTE_KERNEL[want], k) for k in names):
-            wrong.append("%s: expected %s, launched %s" % (name, ROUTE_KERNEL[want], sorted(set(names))))
+        if not any(re.search(ROUTE_KERNEL[want], k) for k in launched):
+            wrong.append("%s: expected %s, launched %s" % (name, ROUTE_KERNEL[want], sorted(set(launched))))
         for fam in FAMILY:
             if re.search(fam, ROUTE_KERNEL[want].replace(_K, "")):
-                other = [k for k in names if re.search(fam, k) and not re.search(ROUTE_KERNEL[want], k)]
+                other = [k for k in launched if re.search(fam, k) and not re.search(ROUTE_KERNEL[want], k)]
                 if other:
                     wrong.append("%s: also launched %s" % (name, sorted(set(other))))
-    if not seen_any:
-        print("SKIP: torch.profiler recorded no CUDA kernel events on this system")
-        return
-    assert not wrong, "\n".join(wrong)
-    print("%d rows launched their kernels" % len(cases))
+        return wrong
+    check_row_launches({name: case.run for name, case in cases.items()}, complaints)
 
 
 def test_rows_launch_their_kernels(cuda):
     """Each row runs the kernel named for it (the restated host predicate agrees), and no other variant of it.
     Checked in a fresh Python process: one that has already held many profiler sessions (the rest of the GPU suite)
     can drop CUDA kernel events."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([root] + [p for p in [os.environ.get("PYTHONPATH")] if p]))
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
-        "-c", "from tests.test_gpu_elementwise_exact import _check_launches; _check_launches()"]
-    r = subprocess.run(cmd, cwd=root, env=env, capture_output=True, text=True, timeout=900)
-    print(r.stdout[-2000:])
-    assert r.returncode == 0, r.stderr[-4000:]
-    if r.stdout.startswith("SKIP"):
-        pytest.skip(r.stdout.strip())
+    check_in_fresh_process(__name__)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -1145,7 +1069,7 @@ def test_avgpool_roundings_of_the_two_paths(cuda):
     from byol_b200 import ops
     g = gen(cuda, 3)
     for hw in (1, 16, 49, 64, 144):
-        x = _acts((64, hw, 1, 256), cuda, g)
+        x = acts((64, hw, 1, 256), cuda, g)
         a = ops.avgpool_fwd(x.to(BF), True, False)[0]
         b = ops.avgpool_f32(x.float())
         ulps = _ulps(a.cpu().numpy(), b.cpu().numpy().astype(np.float64))
@@ -1268,38 +1192,12 @@ def _recorders(calls, ratios):
 
     def avgpool_bwd_f32(ga, gb, n, h, w, c):
         calls.add(("avgpool_bwd_f32", n, h, w, c, ga is not None, gb is not None))
-    return {k: v for k, v in locals().items() if callable(v) and k not in ("calls", "ratios")}
 
-
-def _record_step(monkeypatch, dev, arch, rep, b, r, precision, ratios):
-    from byol_b200 import ops, wiring
-    from byol_b200.model import BYOL
-    calls = set()
-    with monkeypatch.context() as mp:
-        for name, rec in _recorders(calls, ratios).items():
-            orig = getattr(ops, name)
-
-            def wrapped(*a, _orig=orig, _rec=rec, **k):
-                _rec(*a, **k)
-                return _orig(*a, **k)
-            mp.setattr(ops, name, wrapped)
-        lib_avgpool = ops.lib.byol_avgpool_fwd
-
-        def avgpool_fwd(x, yf, yb, n, hw, c, stream):
-            calls.add(("avgpool_fwd", n, hw, c, bool(yf), bool(yb)))
-            return lib_avgpool(x, yf, yb, n, hw, c, stream)
-        mp.setattr(ops.lib, "byol_avgpool_fwd", avgpool_fwd)
-        torch.manual_seed(5)
-        model = BYOL(rep, 256, 1000, 10, arch=arch, precision=precision, backward_precision=precision).to(dev).train()
-        model._engine.use_graphs = False
-        g = torch.Generator().manual_seed(6)
-        a1, a2 = torch.rand(b, 3, r, r, generator=g).to(dev), torch.rand(b, 3, r, r, generator=g).to(dev)
-        lab = torch.randint(0, 1000, (b,), generator=g).to(dev)
-        opt = wiring.build_optimizer(model, global_batch_size=256)
-        wiring.train_step(model, opt, a1, a2, lab)
-        torch.cuda.synchronize()
-    del model, opt
-    return calls
+    def lib_avgpool_fwd(x, yf, yb, n, hw, c, stream):       # the engine calls the library entry directly
+        calls.add(("avgpool_fwd", n, hw, c, bool(yf), bool(yb)))
+    recs = {k: v for k, v in locals().items() if callable(v) and k not in ("calls", "ratios", "lib_avgpool_fwd")}
+    recs["lib.byol_avgpool_fwd"] = lib_avgpool_fwd
+    return recs
 
 
 def _replay_case(dev, g, sig):
@@ -1365,11 +1263,12 @@ NETS = [("resnet18", 512, 8, 224, "bf16"), ("resnet:bottleneck:2,1,1,1", 2048, 8
         ("resnext:32x4:1,1,1,1", 2048, 2, 112, "bf16"), ("resnet18", 512, 4, 64, "fp32")]
 
 
-def test_replay_engine_calls_exactly(cuda, monkeypatch):
+def test_replay_engine_calls_exactly(cuda):
     calls, ratios = set(), []
-    for arch, rep, b, r, precision in NETS:
-        calls |= _record_step(monkeypatch, cuda, arch, rep, b, r, precision, ratios)
-        torch.cuda.empty_cache()
+    with recording(_recorders(calls, ratios)):
+        for arch, rep, b, r, precision in NETS:
+            byol_train_step(cuda, arch, rep, b, r, precision=precision, backward_precision=precision)
+            torch.cuda.empty_cache()
     ops_seen = {sig[0] for sig in calls}
     pools = {sig[5] for sig in calls if sig[0] == "bn_relu_maxpool_fwd"}
     assert pools == {True, False}, "the stem pool with and without argmax must both be recorded, got %s" % pools
@@ -1378,17 +1277,6 @@ def test_replay_engine_calls_exactly(cuda, monkeypatch):
     assert {1, 3} <= modes, "bn_bwd_apply mask modes recorded: %s" % sorted(modes)
     for op in ("bn_apply_f32", "bn_bwd_apply_f32", "maxpool_f32", "maxpool_bwd_f32", "avgpool_f32"):
         assert op in ops_seen, "no %s call recorded from the fp32 path" % op
-    failures = []
-    for i, sig in enumerate(sorted(calls, key=repr)):
-        case = _replay_case(cuda, gen(cuda, 2000 + i), sig)
-        outs = case.run()
-        torch.cuda.synchronize()
-        try:
-            case.check(outs)
-        except AssertionError as e:
-            failures.append("%s: %s" % (sig, e))
-        del outs, case
-    print("replayed %d distinct calls (%s)" % (len(calls), ", ".join(sorted(ops_seen))))
     print("largest |mean| / sqrt(var + eps) of a BatchNorm input in these steps: %.1f" % max(ratios))
     assert max(ratios) < 50, "a BatchNorm input approaches the variance-cancellation range of bn_finalize"
-    assert not failures, "%d of %d replayed calls differ:\n%s" % (len(failures), len(calls), "\n".join(failures))
+    replay(cuda, calls, _replay_case, 2000, " (%s)" % ", ".join(sorted(ops_seen)))

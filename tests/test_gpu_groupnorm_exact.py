@@ -22,17 +22,16 @@ kernel variant.
   torch.profiler, in a fresh process, that each row launches exactly its kernels.
 * Non-finite inputs, batch independence per kernel, and a replay of the engine's own calls with exact operands.
 """
-import os
 import re
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 
-from tests.test_gpu_elementwise_exact import Case, _acts, _aten_pool, _expect, _expect_same, _flat_index, _fma64, _same
-from tests.util import fma32, gen, gn_finalize_restated, ints, pack_bits, pow2, unpack_bits
+from tests.exact import (Case, byol_model, byol_train_step, check_in_fresh_process, check_row_launches, expect,
+                         expect_same, kernel_names, recording, replay, row_case, run_and_check, same)
+from tests.test_gpu_elementwise_exact import acts, aten_pool, flat_index
+from tests.util import fma32, fma64, gen, gn_finalize_restated, ints, pack_bits, pow2, unpack_bits
 
 pytestmark = pytest.mark.gpu
 BF, F32, F64, U8 = torch.bfloat16, torch.float32, torch.float64, torch.uint8
@@ -113,8 +112,8 @@ def stats_pm_case(dev, g, n, h, w, c):
 
     def check(outs):
         st, sums = outs
-        _expect_same("sums64", sums, _group_sums(y, c))
-        _expect("stats", st, torch.stack([mu, 1.0 / a], -1))
+        expect_same("sums64", sums, _group_sums(y, c))
+        expect("stats", st, torch.stack([mu, 1.0 / a], -1))
 
     return Case(run, check, "stats")
 
@@ -136,10 +135,10 @@ def stats_rand_case(dev, g, n, h, w, c):
     def check(outs):
         st, sums = outs
         want_sums = _group_sums(y, c)
-        _expect_same("sums64", sums, want_sums)
+        expect_same("sums64", sums, want_sums)
         cnt = h * w * (c // GROUPS)
         want = torch.from_numpy(gn_finalize_restated(want_sums.cpu().numpy(), float(cnt), 1e-5)).to(dev)
-        _expect_same("stats vs restated gn_finalize", st, want)
+        expect_same("stats vs restated gn_finalize", st, want)
         s64 = want_sums.cpu()
         mean = s64[..., 0] / cnt
         var = (s64[..., 1] / cnt - mean * mean).clamp_min(0)
@@ -157,10 +156,10 @@ def stats_rand_case(dev, g, n, h, w, c):
 def apply_case(dev, g, n, h, w, c, resid=None, relu=False, mask=False):
     """y = act(x*scale + shift (+ r | + r*rscale + rshift)) and its mask bits; resid None / "plain" / "gn"."""
     from byol_b200 import ops
-    x = _acts((n, h, w, c), dev, g)
+    x = acts((n, h, w, c), dev, g)
     gam, bet = pow2(c, dev, g, signed=True), ints((c,), dev, g, 3)
     mean, rstd, st = _stats(n, dev, g)
-    r = _acts((n, h, w, c), dev, g) if resid else None
+    r = acts((n, h, w, c), dev, g) if resid else None
     rgn = None
     if resid == "gn":
         rgam, rbet = pow2(c, dev, g, signed=True), ints((c,), dev, g, 3)
@@ -185,7 +184,7 @@ def apply_case(dev, g, n, h, w, c, resid=None, relu=False, mask=False):
             ref = ref + r
         if relu:
             ref = torch.relu(ref)
-        _expect("y", y, ref)
+        expect("y", y, ref)
         if mask:
             assert torch.equal(unpack_bits(mo, ref.shape), ref > 0), "mask_out differs"
 
@@ -197,7 +196,7 @@ def pool_case(dev, g, n, h, w, c, k=3, s=2, p=1, want_idx=True):
     first maximum in scan order).  Scales of both signs and one forced all-negative block give windows that are all
     zero after the ReLU (their argmax: the first in-image position)."""
     from byol_b200 import ops
-    x = _acts((n, h, w, c), dev, g)
+    x = acts((n, h, w, c), dev, g)
     gam, bet = pow2(c, dev, g, signed=True), ints((c,), dev, g, 3)
     mean, rstd, _ = _stats(n, dev, g)
     x[0, :, :, :8] = 0.0
@@ -213,11 +212,11 @@ def pool_case(dev, g, n, h, w, c, k=3, s=2, p=1, want_idx=True):
         y, idx = outs
         sc, sh = _affine(gam, bet, mean, rstd, c)
         a64 = torch.relu(x * sc + sh).float().to(BF).to(F64)
-        ry, ri = _aten_pool(a64, k, s, p)
+        ry, ri = aten_pool(a64, k, s, p)
         assert bool((ry[0, :, :, :8] == 0).all()), "the forced all-zero windows are missing"
-        _expect("y", y, ry)
+        expect("y", y, ry)
         if want_idx:
-            fi = _flat_index(idx, w, k, s, p)
+            fi = flat_index(idx, w, k, s, p)
             bad = fi != ri
             assert not bad.any(), "argmax differs at %d of %d outputs (first %s: %d vs ATen %d)" % (
                 int(bad.sum()), bad.numel(), bad.nonzero()[0].tolist(), int(fi[bad][0]), int(ri[bad][0]))
@@ -231,7 +230,7 @@ def pool_case(dev, g, n, h, w, c, k=3, s=2, p=1, want_idx=True):
 # backward
 # ------------------------------------------------------------------------------------------------------------------
 def _bwd_operands(dev, g, n, h, w, c, mask_mode):
-    x, gr = _acts((n, h, w, c), dev, g), _acts((n, h, w, c), dev, g, 3)
+    x, gr = acts((n, h, w, c), dev, g), acts((n, h, w, c), dev, g, 3)
     gam, bet = pow2(c, dev, g, signed=True), ints((c,), dev, g, 3)
     mean, rstd, st = _stats(n, dev, g)
     act, keep = None, None
@@ -239,7 +238,7 @@ def _bwd_operands(dev, g, n, h, w, c, mask_mode):
         sc, sh = _affine(gam, bet, mean, rstd, c)
         keep = x * sc + sh > 0
     elif mask_mode == 2:
-        a = _acts((n, h, w, c), dev, g)
+        a = acts((n, h, w, c), dev, g)
         keep, act = a > 0, a.to(BF)
     elif mask_mode == 3:
         keep = torch.rand((n, h, w, c), generator=g, device=dev) > 0.4
@@ -272,7 +271,7 @@ def reduce_case(dev, g, n, h, w, c, mask_mode):
                                        ("dbeta", db, db0, db64)):
             # fl32(init + fl32(exact)) with one rounding of the fp32 sum (an fp64 sum of the two could round twice)
             want = fma32(init.cpu().numpy(), np.float32(1), exact.float().cpu().numpy())
-            _expect_same(name, got, torch.from_numpy(want).to(dev).view(got.shape))
+            expect_same(name, got, torch.from_numpy(want).to(dev).view(got.shape))
 
     return Case(run, check, "reduce%d" % mask_mode)
 
@@ -302,19 +301,19 @@ def bwd_apply_case(dev, g, n, h, w, c, mask_mode, dz_out=False):
         rs = _chan(o["rstd"], c)
         ref = rs * (gam * o["dz"] - s1 / m - o["xh"] * s2 / m)
         if dyadic:
-            _expect("dy", dy, ref)
+            expect("dy", dy, ref)
         else:
             f = lambda t: t.float()
             inv_m = torch.tensor(float(np.float32(1.0 / m)), dtype=F32, device=dev)
             m1, m2 = f(s1) * inv_m, f(s2) * inv_m
             xh32 = (f(o["x"]) - f(_chan(o["mean"], c))) * f(rs)
             o32 = f(rs) * ((f(gam) * f(o["dz"]) - m1) - xh32 * m2)
-            _expect_same("dy vs the fp32 restatement", dy, o32.to(BF))
+            expect_same("dy vs the fp32 restatement", dy, o32.to(BF))
             bound = 2.0 ** -21 * rs.abs() * ((gam * o["dz"]).abs() + (s1 / m).abs() + (o["xh"] * s2 / m).abs())
             err = (o32.double() - ref).abs()
             assert bool((err <= bound).all()), "fp32 restatement beyond its bound by %g" % float((err - bound).max())
         if dz_out:
-            _expect("dz_out", dz, o["dz"])
+            expect("dz_out", dz, o["dz"])
         else:
             assert dz is None
 
@@ -357,7 +356,7 @@ def _strided(w, step):
 
 
 def _fma_rows(a, b, c):
-    return _fma64(a.reshape(-1), b.reshape(-1), c.reshape(-1)).reshape(a.shape)
+    return fma64(a.reshape(-1), b.reshape(-1), c.reshape(-1)).reshape(a.shape)
 
 
 def ws_fwd_restated(w):
@@ -517,9 +516,8 @@ ROWS["ws_fwd_one_unit"] = ("ws_fwd", ws_case, dict(units=[(3, 2048)]))
 ROWS["ws_bwd_one_unit"] = ("ws_bwd", ws_case, dict(units=[(3, 2048)], bwd=True))
 
 
-def _build(name, dev):
-    _, builder, kw = ROWS[name]
-    return builder(dev, gen(dev, sum(map(ord, name))), **kw)
+def _build(dev, name):
+    return row_case(dev, name, *ROWS[name][1:])
 
 
 def test_shapes_sit_at_their_geometry_edges():
@@ -533,59 +531,38 @@ def test_shapes_sit_at_their_geometry_edges():
 
 @pytest.mark.parametrize("name", list(ROWS))
 def test_row_exact(cuda, name):
-    case = _build(name, cuda)
-    outs = case.run()
-    torch.cuda.synchronize()
-    case.check(outs)
+    run_and_check(_build(cuda, name))
 
 
 def _byol_kernels(run):
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        run()
-        torch.cuda.synchronize()
+    """The sorted GroupNorm / WS / fix_flush kernels one run() launches, with their template argument."""
     names = []
-    for e in prof.events():
-        m = re.search(r"\b((?:gn|ws)_\w+?_kernel|fix_flush_kernel)(<\d+>)?\(", e.name.replace(" ", ""))
+    for k in kernel_names(run):
+        m = re.search(r"\b((?:gn|ws)_\w+?_kernel|fix_flush_kernel)(<\d+>)?\(", k)
         if m:
             names.append(m.group(1) + (m.group(2) or ""))
-    return sorted(names), bool(prof.events())
+    return sorted(names)
 
 
 def _check_launches():
-    cases = {name: _build(name, torch.device("cuda:0")) for name in ROWS}
-    for case in cases.values():
-        case.run()
-    torch.cuda.synchronize()
-    wrong, seen_any = [], False
-    for name, case in cases.items():
-        want = ROWS[name][0]
+    cases = {name: _build(torch.device("cuda:0"), name) for name in ROWS}
+
+    def complaints(name, launched):
+        case, want = cases[name], ROWS[name][0]
+        wrong = []
         if case.route != want:
             wrong.append("%s: the case says %s, the row is meant for %s" % (name, case.route, want))
-        names, _ = _byol_kernels(case.run)
-        seen_any = seen_any or bool(names)
-        if names and names != sorted(ROUTE_KERNELS[want]):
-            wrong.append("%s: expected %s, launched %s" % (name, sorted(ROUTE_KERNELS[want]), names))
-    if not seen_any:
-        print("SKIP: torch.profiler recorded no CUDA kernel events on this system")
-        return
-    assert not wrong, "\n".join(wrong)
-    print("%d rows launched their kernels" % len(cases))
+        if launched != sorted(ROUTE_KERNELS[want]):
+            wrong.append("%s: expected %s, launched %s" % (name, sorted(ROUTE_KERNELS[want]), launched))
+        return wrong
+    check_row_launches({name: case.run for name, case in cases.items()}, complaints, _byol_kernels)
 
 
 def test_rows_launch_their_kernels(cuda):
     """Each row launches exactly its kernels: gn_stats_kernel + gn_finalize_kernel, the <MASK> / <RESID>
     instantiation named for it, gn_bwd_reduce with its three fix_flush_kernels (s12, dbeta, dgamma).  Checked in a
     fresh Python process (a process that has held many profiler sessions can drop CUDA kernel events)."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([root] + [p for p in [os.environ.get("PYTHONPATH")] if p]))
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
-        "-c", "from tests.test_gpu_groupnorm_exact import _check_launches; _check_launches()"]
-    r = subprocess.run(cmd, cwd=root, env=env, capture_output=True, text=True, timeout=900)
-    print(r.stdout[-2000:])
-    assert r.returncode == 0, r.stderr[-4000:]
-    if r.stdout.startswith("SKIP"):
-        pytest.skip(r.stdout.strip())
+    check_in_fresh_process(__name__)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -623,15 +600,15 @@ def test_non_finite_inputs(cuda):
     good = [k for k in range(GROUPS) if k not in bad and k != 20]
     assert torch.isnan(st[1, bad, 1]).all(), "rstd of the groups holding NaN / Inf must be NaN"
     assert torch.isnan(st[1, [0, 15], 0]).all() and st[1, 5, 0] == float("inf") and st[1, 10, 0] == float("-inf")
-    assert _same(st[1, good], st0[1, good]) and _same(st[0], st0[0]), "the statistics of finite groups changed"
+    assert same(st[1, good], st0[1, good]) and same(st[0], st0[0]), "the statistics of finite groups changed"
     keep = unpack_bits(mo, y.shape)
     chans = torch.cat([torch.arange(k * 2, k * 2 + 2) for k in bad]).to(cuda)
     assert (y[1][..., chans] == 0).all() and not keep[1][..., chans].any()
     assert torch.isnan(yl[1][..., chans].float()).all()
     other = torch.tensor([ch for ch in range(c) if ch // 2 not in bad], device=cuda)
-    assert _same(y[1][..., other], y0[1][..., other]) and torch.equal(keep[1][..., other],
+    assert same(y[1][..., other], y0[1][..., other]) and torch.equal(keep[1][..., other],
                                                                        unpack_bits(m0, y0.shape)[1][..., other])
-    assert _same(y[0], y0[0]) and _same(yl[0], l0[0])
+    assert same(y[0], y0[0]) and same(yl[0], l0[0])
     assert torch.isfinite(sums[2]).all() and torch.isfinite(st[2]).all(), "sums near the bf16 maximum overflowed"
     assert float(sums[2, 20, 1]) == float(big) ** 2 * h * w * 2
 
@@ -670,7 +647,7 @@ def test_batch_independence_per_kernel(cuda, shape):
         torch.cuda.synchronize()
         for label, a, b in zip(("stats", "sums64", "y", "pool", "pool idx", "s12", "dy"), alone, full):
             if a is not None:
-                assert _same(a[0], b[i]), "%s of image %d differs alone and in the batch" % (label, i)
+                assert same(a[0], b[i]), "%s of image %d differs alone and in the batch" % (label, i)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -770,41 +747,27 @@ def _recorders(calls, descs):
     return {k: v for k, v in locals().items() if callable(v) and not k.startswith("_")}
 
 
-def _record(monkeypatch, dev, arch, b, r, what):
-    from byol_b200 import ops, wiring
+def _record(dev, arch, b, r, what):
+    """The signatures of one source's calls: a BYOL step, a fine-tune step or representations() of one image."""
     from byol_b200.finetune import FineTune
-    from byol_b200.model import BYOL
     calls, descs = set(), []
-    with monkeypatch.context() as mp:
-        for name, rec in _recorders(calls, descs).items():
-            orig = getattr(ops, name)
-
-            def wrapped(*a, _orig=orig, _rec=rec, **k):
-                _rec(*a, **k)
-                return _orig(*a, **k)
-            mp.setattr(ops, name, wrapped)
-        torch.manual_seed(5)
-        model = BYOL(512 if arch == "resnet18" else 2048, 64, 10, 10, arch=arch, head_latent_size=128,
-                     norm="group_ws").to(dev).train()
-        model._engine.use_graphs = False
-        g = torch.Generator().manual_seed(6)
-        a1, a2 = torch.rand(b, 3, r, r, generator=g).to(dev), torch.rand(b, 3, r, r, generator=g).to(dev)
-        lab = torch.randint(0, 10, (b,), generator=g).to(dev)
+    model_kw = dict(classes=10, projection=64, head_latent_size=128, norm="group_ws")
+    with recording(_recorders(calls, descs)):
         if what == "byol":
-            opt = wiring.build_optimizer(model, global_batch_size=256)
-            wiring.train_step(model, opt, a1, a2, lab)
-        elif what == "finetune":
-            FineTune(model, 5, 0.1, seed=2).step(a1, lab % 5, 1.0)
+            byol_train_step(dev, arch, 512 if arch == "resnet18" else 2048, b, r, **model_kw)
         else:
-            model.representations(a1[:1])
-        torch.cuda.synchronize()
+            model, a1, _, lab = byol_model(dev, arch, 512 if arch == "resnet18" else 2048, b, r, **model_kw)
+            if what == "finetune":
+                FineTune(model, 5, 0.1, seed=2).step(a1, lab % 5, 1.0)
+            else:
+                model.representations(a1[:1])
+            torch.cuda.synchronize()
     out = set()
     for sig in calls:
         if sig[0] in ("ws_fwd", "ws_bwd"):
             d = descs[sig[1]].cpu().tolist()
             sig = (sig[0], tuple((row[2], row[3]) for row in d), sig[2])
         out.add(sig)
-    del model
     return out
 
 
@@ -839,13 +802,13 @@ SOURCES = [("resnet18", 4, 64, "byol"), ("resnet:bottleneck:1,1,1,1", 4, 64, "by
            ("resnet:bottleneck:1,1,1,1", 1, 64, "representations")]
 
 
-def test_replay_engine_calls_exactly(cuda, monkeypatch):
+def test_replay_engine_calls_exactly(cuda):
     """Every distinct GroupNorm / weight-standardisation call of a BYOL step (ResNet-18, a bottleneck net and a
     ResNeXt net at 64 px, ResNet-18 at 72 px: maps of 36, 18, 9, 5 and 3), a fine-tune step and representations() of
     one image, replayed with exact operands (or against the restatement where m or the fan-in is not dyadic)."""
     calls = set()
     for arch, b, r, what in SOURCES:
-        calls |= _record(monkeypatch, cuda, arch, b, r, what)
+        calls |= _record(cuda, arch, b, r, what)
         torch.cuda.empty_cache()
     modes = {sig[2] for sig in calls if sig[0] == "gn_bwd_apply"}
     assert {1, 3} <= modes, "gn_bwd_apply mask modes recorded: %s" % sorted(modes)
@@ -855,15 +818,4 @@ def test_replay_engine_calls_exactly(cuda, monkeypatch):
     assert any(sig[0] == "ws_bwd" for sig in calls) and any(sig[0] == "gn_bwd_reduce" for sig in calls)
     maps = {sig[1][1] for sig in calls if sig[0].startswith("gn_")}
     assert {36, 18, 9, 5, 3} <= maps, "map sizes recorded: %s" % sorted(maps)
-    failures = []
-    for i, sig in enumerate(sorted(calls, key=repr)):
-        case = _replay_case(cuda, gen(cuda, 3000 + i), sig)
-        outs = case.run()
-        torch.cuda.synchronize()
-        try:
-            case.check(outs)
-        except AssertionError as e:
-            failures.append("%s: %s" % (sig, e))
-        del outs, case
-    print("replayed %d distinct calls" % len(calls))
-    assert not failures, "%d of %d replayed calls differ:\n%s" % (len(failures), len(calls), "\n".join(failures))
+    replay(cuda, calls, _replay_case, 3000)

@@ -33,17 +33,15 @@ float64, on every branch inside their kernels.
   shapes and options of every loss, cross-entropy and LARS call (for LARS each tensor's length and 16-byte phases),
   and every distinct call is replayed with exact operands.
 """
-import os
-import re
-import subprocess
-import sys
 from fractions import Fraction
 
 import numpy as np
 import pytest
 import torch
 
-from tests.util import _rn32, fma32, gen, ints, report_mismatch
+from tests.exact import (Case, bits_same, byol_kernel_sequence, byol_train_step, check_in_fresh_process, expect_bits,
+                         expect_within, NO_EVENTS, recording, replay, row_case, run_and_check)
+from tests.util import _rn32, fma32, gen, ints
 
 pytestmark = pytest.mark.gpu
 F32, F64, I64 = torch.float32, torch.float64, torch.int64
@@ -59,55 +57,8 @@ CE_TOL = 2.0 ** -16       # row loss / lse: of 1 + |max| + |x_label|; dlogits: |
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# comparison helpers
+# operands
 # ------------------------------------------------------------------------------------------------------------------
-def _bits_same(got, want):
-    """got (torch) == want (numpy fp32 or torch) bit for bit (every NaN matches every NaN)."""
-    g = got.detach().float().cpu().numpy().reshape(-1)
-    w = want.detach().float().cpu().numpy() if torch.is_tensor(want) else np.asarray(want, dtype=np.float32)
-    w = w.reshape(-1)
-    if g.shape != w.shape:
-        return False
-    gn, wn = np.isnan(g), np.isnan(w)
-    return bool(np.array_equal(gn, wn) and np.array_equal(np.where(gn, 0, g).view(np.uint32),
-                                                          np.where(wn, 0, w).view(np.uint32)))
-
-
-def _expect_bits(name, got, want):
-    if _bits_same(got, want):
-        return
-    g = got.detach().float().cpu().reshape(1, -1)
-    w = want.detach().float().cpu().reshape(1, -1) if torch.is_tensor(want) else \
-        torch.from_numpy(np.asarray(want, dtype=np.float32).reshape(1, -1).copy())
-    _, msg = report_mismatch(name, g, w, 0.0, 0.0)
-    raise AssertionError(msg + " (bits)")
-
-
-def _expect_within(name, got, ref64, tol):
-    """|got - ref64| <= tol where ref64 is finite; non-finite entries must match in kind (NaN, +inf, -inf)."""
-    g = np.asarray(got.detach().cpu().double().numpy() if torch.is_tensor(got) else got, dtype=np.float64).reshape(-1)
-    r, tol = np.asarray(ref64, dtype=np.float64).reshape(-1), np.broadcast_to(np.asarray(tol, np.float64), g.shape)
-    fin, inf = np.isfinite(r), np.isinf(r)
-    same_kind = np.array_equal(np.isnan(g), np.isnan(r)) and np.array_equal(g[inf], r[inf]) and \
-        bool(np.isfinite(g[fin]).all())
-    err = np.where(fin, np.abs(g - np.where(fin, r, 0)), 0)
-    bad = fin & ~(err <= tol)
-    print("%s: max |err| / bound %.3g over %d finite values" % (name, float((err / np.maximum(tol, 1e-300))[fin].max())
-                                                                if fin.any() else 0.0, int(fin.sum())))
-    assert same_kind, "%s: non-finite entries differ from float64" % name
-    assert not bad.any(), "%s: %d of %d beyond the float64 bound (first %s: got %r, ref %r)" % (
-        name, int(bad.sum()), bad.size, np.nonzero(bad)[0][:8].tolist(), g[bad][:4].tolist(), r[bad][:4].tolist())
-
-
-class Case:
-    """run() launches the kernels under test on fresh outputs and returns them; check(outs) compares them with the
-    restatement and with float64; launches: the byol:: kernels run() launches, in order; branch: the restated
-    predicates."""
-
-    def __init__(self, run, check, launches, branch):
-        self.run, self.check, self.launches, self.branch = run, check, launches, branch
-
-
 def _grid(shape, dev, g, amp, k):
     """fp32 integers in [-amp, amp] times 2^-k (exact)."""
     return (ints(shape, dev, g, amp) * 2.0 ** -k).float()
@@ -183,27 +134,27 @@ def loss_case(dev, g, rows, dim, go=0.75):
         np_ = [x.cpu().numpy() for x in ops_]
         loss, saved, r1, r2, (a1, b1, a2, b2) = loss_restated(sums, rows, 1.0 if go is None else go,
                                                               np_[0], np_[1], np_[2], np_[3])
-        _expect_bits("loss", out[0:1], [loss])
-        _expect_bits("saved", out[1:7], saved)
-        _expect_bits("dq1", dq1, r1)
-        _expect_bits("dq2", dq2, r2)
+        expect_bits("loss", out[0:1], [loss])
+        expect_bits("saved", out[1:7], saved)
+        expect_bits("dq1", dq1, r1)
+        expect_bits("dq2", dq2, r2)
         # float64 evaluation of objective.py (regression_loss of whole-matrix norms, symmetric, mean over rows)
         s = [float(x) for x in sums]
         n = [s[0] ** 0.5, s[1] ** 0.5, s[2] ** 0.5, s[3] ** 0.5]
         c12, c21 = -2 * s[4] / (n[0] * n[3]), -2 * s[5] / (n[1] * n[2])
-        _expect_within("loss vs float64", out[0:1], [(c12 + c21) / rows],
-                       LOSS_ULPS * 2.0 ** -24 * (abs(c12) + abs(c21)) / rows)
-        _expect_within("saved vs float64", out[1:7], n + s[4:], LOSS_ULPS * 2.0 ** -24 * np.abs(n + s[4:]))
+        expect_within("loss vs float64", out[0:1], [(c12 + c21) / rows],
+                      LOSS_ULPS * 2.0 ** -24 * (abs(c12) + abs(c21)) / rows)
+        expect_within("saved vs float64", out[1:7], n + s[4:], LOSS_ULPS * 2.0 ** -24 * np.abs(n + s[4:]))
         gv = 1.0 if go is None else float(f32(go))
         kk = gv * -2 / rows
         for name, got, q, z, nq, nz, sqz in (("dq1", dq1, x64[0], x64[3], n[0], n[3], s[4]),
                                             ("dq2", dq2, x64[1], x64[2], n[1], n[2], s[5])):
             ta, tb = kk / (nq * nz) * z, -kk * sqz / (nq ** 3 * nz) * q
-            _expect_within(name + " vs float64", got.reshape(-1), (ta + tb).reshape(-1).cpu().numpy(),
-                           DQ_ULPS * 2.0 ** -24 * (ta.abs() + tb.abs()).reshape(-1).cpu().numpy())
+            expect_within(name + " vs float64", got.reshape(-1), (ta + tb).reshape(-1).cpu().numpy(),
+                          DQ_ULPS * 2.0 ** -24 * (ta.abs() + tb.abs()).reshape(-1).cpu().numpy())
 
-    return Case(run, check, ["loss_fwd_partial_kernel", "loss_finalize_kernel", "loss_bwd_kernel"],
-                dict(br, grad_out=go is not None))
+    return Case(run, check, launches=["loss_fwd_partial_kernel", "loss_finalize_kernel", "loss_bwd_kernel"],
+                branch=dict(br, grad_out=go is not None))
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -377,21 +328,21 @@ def lars_case(dev, g, ts, momentum=0.9, eps=0.0, trust=0.001, first_step=False, 
             if mom and s > 0:
                 # the carried buffer is the one the previous step wrote
                 for i in range(len(ts)):
-                    _expect_bits("step %d momentum in, tensor %d" % (s, i), ms[i], hist[s - 1][4][i])
+                    expect_bits("step %d momentum in, tensor %d" % (s, i), ms[i], hist[s - 1][4][i])
             want_p, want_m = lars_restated(np_p, np_g, np_m, ts, momentum or 0.0, eps, trust, first_step)
             ref = lars_float64(np_p, np_g, m64, ts, momentum or 0.0, eps, trust, first_step, mag)
             for i, t in enumerate(ts):
-                _expect_bits("step %d p[%d] (n=%d)" % (s, i, t.n), got_p[i], want_p[i])
+                expect_bits("step %d p[%d] (n=%d)" % (s, i, t.n), got_p[i], want_p[i])
                 if mom:
-                    _expect_bits("step %d m[%d] (n=%d)" % (s, i, t.n), got_m[i], want_m[i])
+                    expect_bits("step %d m[%d] (n=%d)" % (s, i, t.n), got_m[i], want_m[i])
                 p64, mag_b = ref[i]
                 if not t.n:
                     continue
-                _expect_within("step %d p[%d] vs float64" % (s, i), got_p[i], p64,
-                               LARS_ULPS * 2.0 ** -24 * np.nan_to_num(np.abs(p64) + float(f32(t.lr)) * mag_b))
+                expect_within("step %d p[%d] vs float64" % (s, i), got_p[i], p64,
+                              LARS_ULPS * 2.0 ** -24 * np.nan_to_num(np.abs(p64) + float(f32(t.lr)) * mag_b))
                 if mom:
-                    _expect_within("step %d m[%d] vs float64" % (s, i), got_m[i], m64[i],
-                                   LARS_ULPS * 2.0 ** -24 * np.nan_to_num(mag[i]))
+                    expect_within("step %d m[%d] vs float64" % (s, i), got_m[i], m64[i],
+                                  LARS_ULPS * 2.0 ** -24 * np.nan_to_num(mag[i]))
         # nothing outside the tensors was written
         for r, buf in enumerate(bufs):
             keep = torch.ones_like(buf, dtype=torch.bool)
@@ -400,8 +351,8 @@ def lars_case(dev, g, ts, momentum=0.9, eps=0.0, trust=0.001, first_step=False, 
             if r < 2 or mom:
                 assert bool((buf[keep] == SENTINEL).all()), "LARS wrote outside its tensors (buffer %d)" % r
 
-    return Case(run, check, ["lars_norms_kernel", "lars_update_kernel"] * steps,
-                dict(lars_branch(ts, mom), momentum=mom, first_step=bool(first_step)))
+    return Case(run, check, launches=["lars_norms_kernel", "lars_update_kernel"] * steps,
+                branch=dict(lars_branch(ts, mom), momentum=mom, first_step=bool(first_step)))
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -473,8 +424,8 @@ def ce_case(dev, g, R, C, LR=None, ld=None, edits=None, labels=None, go=0.37):
         fl, it, out2, lse2, d, d2 = outs
         loss, lse, rank, mx, xl, labr, ok = ce_reference(x32, labn, R, C)
         # two launches, the same bits; the ticket is reset
-        assert _bits_same(out2, fl[2 * R:].cpu().numpy()) and _bits_same(lse2, fl[:R].cpu().numpy())
-        assert _bits_same(d, d2.cpu().numpy()), "two backward launches differ"
+        assert bits_same(out2, fl[2 * R:].cpu().numpy()) and bits_same(lse2, fl[:R].cpu().numpy())
+        assert bits_same(d, d2.cpu().numpy()), "two backward launches differ"
         assert int(it[R]) == 0, "ticket not reset"
         got_rank = it[:R].cpu().numpy().astype(np.int64)
         got_rank = np.where(got_rank == 0x7fffffff, MISS, got_rank)
@@ -483,8 +434,8 @@ def ce_case(dev, g, R, C, LR=None, ld=None, edits=None, labels=None, go=0.37):
                                                                       rank[bad][:8].tolist())
         tol = CE_TOL * (1 + np.abs(np.nan_to_num(mx, posinf=0, neginf=0)) + np.abs(np.nan_to_num(xl, posinf=0,
                                                                                                 neginf=0)))
-        _expect_within("row_loss", fl[R:2 * R], loss, tol)
-        _expect_within("row_lse", fl[:R], lse, tol)
+        expect_within("row_loss", fl[R:2 * R], loss, tol)
+        expect_within("row_lse", fl[:R], lse, tol)
         # the mean: exactly the kernel's fp64 reduction of its own row losses (thread i: rows i, i + 256, ...; then
         # the shared-memory tree), and within the row bounds of float64
         rl = fl[R:2 * R].cpu().numpy().astype(np.float64)
@@ -498,11 +449,11 @@ def ce_case(dev, g, R, C, LR=None, ld=None, edits=None, labels=None, go=0.37):
                 part[:o] = part[:o] + part[o:2 * o]
                 o >>= 1
             mean = f32(part[0] / R)
-        _expect_bits("mean loss (row reduction)", fl[2 * R:2 * R + 1], [mean])
-        _expect_within("mean loss vs float64", fl[2 * R:2 * R + 1], [loss.mean()], [tol.mean()])
+        expect_bits("mean loss (row reduction)", fl[2 * R:2 * R + 1], [mean])
+        expect_within("mean loss vs float64", fl[2 * R:2 * R + 1], [loss.mean()], [tol.mean()])
         hits1, hits5 = int((rank < 1).sum()), int((rank < 5).sum())
-        _expect_bits("top1", fl[2 * R + 1:2 * R + 2], [f32(100) * f32(hits1) / f32(R)])
-        _expect_bits("top5", fl[2 * R + 2:2 * R + 3], [f32(100) * f32(hits5) / f32(R)])
+        expect_bits("top1", fl[2 * R + 1:2 * R + 2], [f32(100) * f32(hits1) / f32(R)])
+        expect_bits("top5", fl[2 * R + 2:2 * R + 3], [f32(100) * f32(hits5) / f32(R)])
         # dlogits = go / R * (softmax - onehot); a label outside [0, C) has no one-hot term
         k = float(f32(go) / f32(R))
         with np.errstate(invalid="ignore", over="ignore"):
@@ -513,9 +464,10 @@ def ce_case(dev, g, R, C, LR=None, ld=None, edits=None, labels=None, go=0.37):
             ref = k * (p - onehot)
             fin = lambda v: np.abs(np.nan_to_num(v, posinf=0, neginf=0))
             dtol = abs(k) * (CE_TOL * np.nan_to_num(p, nan=0) * (1 + fin(mx)[:, None] + fin(x)) + 2.0 ** -23)
-        _expect_within("dlogits", d.reshape(-1), ref.reshape(-1), dtol.reshape(-1))
+        expect_within("dlogits", d.reshape(-1), ref.reshape(-1), dtol.reshape(-1))
 
-    return Case(run, check, ["ce_topk_fwd_kernel"] * 2 + ["ce_bwd_kernel"] * 2, ce_branch(x32, labn, R, C, ld))
+    return Case(run, check, launches=["ce_topk_fwd_kernel"] * 2 + ["ce_bwd_kernel"] * 2,
+                branch=ce_branch(x32, labn, R, C, ld))
 
 
 def _nan_label(x, lab):
@@ -642,9 +594,8 @@ def _ce_rows():
 ROWS = {**_loss_rows(), **_lars_rows(), **_ce_rows()}
 
 
-def _build(name, dev):
-    builder, kw, _ = ROWS[name]
-    return builder(dev, gen(dev, sum(map(ord, name))), **kw)
+def _build(dev, name):
+    return row_case(dev, name, *ROWS[name][:2])
 
 
 def _check_branch(name, case):
@@ -655,31 +606,22 @@ def _check_branch(name, case):
 
 @pytest.mark.parametrize("name", list(ROWS))
 def test_row_exact(cuda, name):
-    case = _build(name, cuda)
+    case = _build(cuda, name)
     _check_branch(name, case)
-    outs = case.run()
-    torch.cuda.synchronize()
-    case.check(outs)
+    run_and_check(case)
 
 
 def _check_launches():
     """All rows in one profiler session, one after the other with a device synchronisation between them: the byol::
     kernels in device-time order must be the rows' launch lists one after the other."""
-    from torch.profiler import ProfilerActivity, profile
-    dev = torch.device("cuda:0")
-    cases = {name: _build(name, dev) for name in ROWS}
+    cases = {name: _build(torch.device("cuda:0"), name) for name in ROWS}
     for case in cases.values():
         case.run()
     torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for case in cases.values():
-            case.run()
-            torch.cuda.synchronize()
-    events = sorted((e for e in prof.events() if "byol::" in e.name), key=lambda e: e.time_range.start)
-    if not events:
-        print("SKIP: torch.profiler recorded no CUDA kernel events on this system")
+    got = byol_kernel_sequence([case.run for case in cases.values()])
+    if not got:
+        print(NO_EVENTS)
         return
-    got = [re.sub(r"^byol::([A-Za-z0-9_]+).*$", r"\1", e.name) for e in events]
     at = 0
     for name, case in cases.items():
         seen = got[at:at + len(case.launches)]
@@ -693,15 +635,7 @@ def test_rows_launch_their_kernels(cuda):
     """Every row launches exactly its kernels: loss_fwd_partial + loss_finalize + loss_bwd, lars_norms + lars_update
     per step, ce_topk_fwd twice + ce_bwd twice, and no other byol:: kernel.  Checked in a fresh Python process: one
     that has already held many profiler sessions (the rest of the GPU suite) can drop CUDA kernel events."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([root] + [p for p in [os.environ.get("PYTHONPATH")] if p]))
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
-        "-c", "from tests.test_gpu_optim_exact import _check_launches; _check_launches()"]
-    r = subprocess.run(cmd, cwd=root, env=env, capture_output=True, text=True, timeout=900)
-    print(r.stdout[-2000:])
-    assert r.returncode == 0, r.stderr[-4000:]
-    if r.stdout.startswith("SKIP"):
-        pytest.skip(r.stdout.strip())
+    check_in_fresh_process(__name__)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -735,7 +669,7 @@ def test_loss_is_scale_invariant(cuda):
             scaled = torch.cat([out[0:1], out[1:5] * 2.0 ** e, out[5:7] * 4.0 ** e]).cpu()
             if base is None:
                 base = scaled
-            _expect_bits("%dx256 loss and saved, inputs scaled by 2^-%d" % (rows, e), scaled, base)
+            expect_bits("%dx256 loss and saved, inputs scaled by 2^-%d" % (rows, e), scaled, base)
     print("loss bit-identical under scaling by 2^0 .. 2^-%d at 8x256 and 512x256" % SCALE_E)
 
 
@@ -753,11 +687,8 @@ def _lars_signature(table, trust, eps, momentum, first_step):
     return ("lars", ts, mp is not None, float(f32(trust)), float(f32(eps)), float(f32(momentum)), bool(first_step))
 
 
-def _record_step(monkeypatch, dev, arch, rep, classes, b, r, precision, rms):
-    from byol_b200 import ops, wiring
-    from byol_b200.model import BYOL
-    calls = set()
-
+def _recorders(calls, rms):
+    """ops function name -> recorder noting the call's shapes and options (for LARS: lengths and 16-byte phases)."""
     def loss_fwd(q1, q2, z1, z2, workspace, loss, saved):
         calls.add(("loss", q1.shape[0], q1.shape[1]))
         for nm, t in (("q", q1), ("q", q2), ("z", z1), ("z", z2)):
@@ -774,28 +705,7 @@ def _record_step(monkeypatch, dev, arch, rep, classes, b, r, precision, rms):
 
     def lars_sgd_step(table, trust_coef, eps, momentum, first_step):
         calls.add(_lars_signature(table, trust_coef, eps, momentum, first_step))
-
-    with monkeypatch.context() as mp:
-        for name, rec in (("loss_fwd", loss_fwd), ("loss_bwd", loss_bwd), ("ce_topk_fwd", ce_topk_fwd),
-                          ("ce_bwd", ce_bwd), ("lars_sgd_step", lars_sgd_step)):
-            orig = getattr(ops, name)
-
-            def wrapped(*a, _orig=orig, _rec=rec, **k):
-                _rec(*a, **k)
-                return _orig(*a, **k)
-            mp.setattr(ops, name, wrapped)
-        torch.manual_seed(5)
-        model = BYOL(rep, 256, classes, 10, arch=arch, precision=precision, backward_precision=precision)
-        model = model.to(dev).train()
-        model._engine.use_graphs = False
-        g = torch.Generator().manual_seed(6)
-        a1, a2 = torch.rand(b, 3, r, r, generator=g).to(dev), torch.rand(b, 3, r, r, generator=g).to(dev)
-        lab = torch.randint(0, classes, (b,), generator=g).to(dev)
-        opt = wiring.build_optimizer(model, global_batch_size=256)
-        wiring.train_step(model, opt, a1, a2, lab)
-        torch.cuda.synchronize()
-    del model, opt
-    return calls
+    return {k: v for k, v in locals().items() if callable(v)}
 
 
 def _replay_case(dev, g, sig):
@@ -822,11 +732,12 @@ NETS = [("resnet18", 512, 1000, 8, 64, "bf16"), ("resnet:bottleneck:1,1,1,1", 20
         ("resnet18", 512, 10, 4, 64, "fp32")]
 
 
-def test_replay_engine_calls_exactly(cuda, monkeypatch):
+def test_replay_engine_calls_exactly(cuda):
     calls, rms = set(), {"q": [], "z": []}
-    for arch, rep, classes, b, r, precision in NETS:
-        calls |= _record_step(monkeypatch, cuda, arch, rep, classes, b, r, precision, rms)
-        torch.cuda.empty_cache()
+    with recording(_recorders(calls, rms)):
+        for arch, rep, classes, b, r, precision in NETS:
+            byol_train_step(cuda, arch, rep, b, r, classes, precision=precision, backward_precision=precision)
+            torch.cuda.empty_cache()
     kinds = {sig[0] for sig in calls}
     assert kinds == {"loss", "loss_bwd", "ce", "ce_bwd", "lars"}, kinds
     phases = {(t[1], t[2], t[3]) for sig in calls if sig[0] == "lars" for t in sig[1]}
@@ -835,15 +746,4 @@ def test_replay_engine_calls_exactly(cuda, monkeypatch):
         min(rms["q"]), max(rms["q"]), min(rms["z"]), max(rms["z"])))
     assert min(rms["q"] + rms["z"]) >= 2.0 ** -SCALE_E, "loss operands below the range test_loss_is_scale_invariant " \
         "asserts"
-    failures = []
-    for i, sig in enumerate(sorted(calls, key=repr)):
-        case = _replay_case(cuda, gen(cuda, 3000 + i), sig)
-        outs = case.run()
-        torch.cuda.synchronize()
-        try:
-            case.check(outs)
-        except AssertionError as e:
-            failures.append("%s: %s" % (str(sig)[:200], e))
-        del outs, case
-    print("replayed %d distinct calls" % len(calls))
-    assert not failures, "%d of %d replayed calls differ:\n%s" % (len(failures), len(calls), "\n".join(failures))
+    replay(cuda, calls, _replay_case, 3000)

@@ -22,17 +22,12 @@ dL/dq = (go / B) 2 r(q) (u - delta (q^.u) q^).  A row whose sum of squares is Na
   l_i (T + 6), T = the float4s per lane; dq within DQ_ULPS of |a| (|q^| + |z^| + |q^| (T + 9)).
 * Row scale invariance, batch-split independence, float64 autograd, run to run and two training-step comparisons.
 """
-import os
-import re
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-from tests.test_gpu_optim_exact import _expect_bits, _expect_within
+from tests.exact import NO_EVENTS, byol_kernel_sequence, check_in_fresh_process, expect_bits, expect_within
 from tests.util import fma32, gen, ints
 
 pytestmark = pytest.mark.gpu
@@ -149,17 +144,17 @@ def check_against_float64(name, loss, saved, dq1, dq2, q1, q2, z1, z2, go, b=Non
     L, pairs = float64_reference(q1, q2, z1, z2, go, b)
     mag = sum((np.abs(p["u"]) * (np.abs(p["qh"]) + np.abs(p["zh"]))).sum(1) + p["l"] * (t + 6) for p in pairs)
     with np.errstate(invalid="ignore"):
-        _expect_within(name + " loss vs float64", loss, [L], LOSS_ULPS * 2.0 ** -24 * mag.mean())
+        expect_within(name + " loss vs float64", loss, [L], LOSS_ULPS * 2.0 ** -24 * mag.mean())
     sv = saved.detach().cpu().numpy()
     for j, p in enumerate(pairs):
-        _expect_within(name + " r(q) vs float64", sv[:, 4 * j], p["r"], 4 * 2.0 ** -24 * np.abs(p["r"]))
-        _expect_within(name + " r(z) vs float64", sv[:, 4 * j + 1], p["rz"], 4 * 2.0 ** -24 * np.abs(p["rz"]))
+        expect_within(name + " r(q) vs float64", sv[:, 4 * j], p["r"], 4 * 2.0 ** -24 * np.abs(p["r"]))
+        expect_within(name + " r(z) vs float64", sv[:, 4 * j + 1], p["rz"], 4 * 2.0 ** -24 * np.abs(p["rz"]))
     for j, (got, p) in enumerate(((dq1, pairs[0]), (dq2, pairs[1]))):
         qh = np.abs(p["qh"])
         with np.errstate(invalid="ignore"):
             tol = DQ_ULPS * 2.0 ** -24 * np.abs(p["a"])[:, None] * (qh + np.abs(p["zh"]) + qh * (t + 9))
-        _expect_within("%s dq%d vs float64" % (name, j + 1), got.reshape(-1), p["dq"].reshape(-1),
-                       np.nan_to_num(tol.reshape(-1)))
+        expect_within("%s dq%d vs float64" % (name, j + 1), got.reshape(-1), p["dq"].reshape(-1),
+                      np.nan_to_num(tol.reshape(-1)))
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -218,10 +213,10 @@ def test_exact_against_restatement(cuda, b, d, go, edits):
     gv = 1.0 if go is None else go
     r_loss, r_saved, r_dq1, r_dq2 = restated(*np_, gv)
     name = "B=%d D=%d go=%s%s" % (b, d, go, " edited" if edits else "")
-    _expect_bits(name + " loss", loss, [r_loss])
-    _expect_bits(name + " saved", saved, r_saved)
-    _expect_bits(name + " dq1", dq1, r_dq1)
-    _expect_bits(name + " dq2", dq2, r_dq2)
+    expect_bits(name + " loss", loss, [r_loss])
+    expect_bits(name + " saved", saved, r_saved)
+    expect_bits(name + " dq1", dq1, r_dq1)
+    expect_bits(name + " dq2", dq2, r_dq2)
     if edits:
         assert torch.isnan(loss).all()
         for j, dq in enumerate((dq1, dq2)):
@@ -268,12 +263,12 @@ def test_row_scale_invariance(cuda):
         xs[2][j] *= 2.0 ** -k         # z1 row j (target of q2 row j)
         xs[1][j] *= 2.0 ** k          # q2 row j
         loss, _, dq1, dq2 = run_loss(*xs, 0.75)
-        _expect_bits("loss, rows scaled by 2^%d" % k, loss, l0)
+        expect_bits("loss, rows scaled by 2^%d" % k, loss, l0)
         want1, want2 = d10.clone(), d20.clone()
         want1[i] *= 2.0 ** -k
         want2[j] *= 2.0 ** -k
-        _expect_bits("dq1, rows scaled by 2^%d" % k, dq1, want1)
-        _expect_bits("dq2, rows scaled by 2^%d" % k, dq2, want2)
+        expect_bits("dq1, rows scaled by 2^%d" % k, dq1, want1)
+        expect_bits("dq2, rows scaled by 2^%d" % k, dq2, want2)
     print("loss bits and dq scaling exact for k in [-20, 20]")
 
 
@@ -285,9 +280,9 @@ def test_batch_split_independence(cuda):
     loss, saved, dq1, dq2 = run_loss(*xs, 1.0)
     halves = [run_loss(*[x[h * 256:(h + 1) * 256].contiguous() for x in xs], 1.0) for h in (0, 1)]
     torch.cuda.synchronize()
-    _expect_bits("dq1 of the batch vs its halves", dq1, torch.cat([h[2] for h in halves]) * 0.5)
-    _expect_bits("dq2 of the batch vs its halves", dq2, torch.cat([h[3] for h in halves]) * 0.5)
-    _expect_bits("saved of the batch vs its halves", saved, torch.cat([h[1] for h in halves]))
+    expect_bits("dq1 of the batch vs its halves", dq1, torch.cat([h[2] for h in halves]) * 0.5)
+    expect_bits("dq2 of the batch vs its halves", dq2, torch.cat([h[3] for h in halves]) * 0.5)
+    expect_bits("saved of the batch vs its halves", saved, torch.cat([h[1] for h in halves]))
     np_ = [x.cpu().numpy() for x in xs]
     L, pairs = float64_reference(*np_, 1.0)
     mag = sum((np.abs(p["u"]) * (np.abs(p["qh"]) + np.abs(p["zh"]))).sum(1) + p["l"] * 8 for p in pairs)
@@ -325,7 +320,7 @@ def test_run_to_run(cuda):
     xs = _randn_operands(cuda, 6, 4096, 256)
     a, b = run_loss(*xs, 0.5), run_loss(*xs, 0.5)
     for name, x, y in zip(("loss", "saved", "dq1", "dq2"), a, b):
-        _expect_bits("run to run " + name, x, y)
+        expect_bits("run to run " + name, x, y)
 
 
 def test_bad_arguments(cuda):
@@ -356,7 +351,6 @@ VARIANT_KERNELS = {"byol": ["loss_rows_fwd_kernel", "loss_rows_finalize_kernel",
 
 
 def _check_launches():
-    from torch.profiler import ProfilerActivity, profile
     from byol_b200.objective import loss_function
     dev = torch.device("cuda:0")
     xs = _randn_operands(dev, 7, 512, 256)
@@ -368,14 +362,10 @@ def _check_launches():
     for v in VARIANT_KERNELS:
         call(v)
     order = ["byol", "reference", "byol"]
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for v in order:
-            call(v)
-    events = sorted((e for e in prof.events() if "byol::" in e.name), key=lambda e: e.time_range.start)
-    if not events:
-        print("SKIP: torch.profiler recorded no CUDA kernel events on this system")
+    got = byol_kernel_sequence([lambda v=v: call(v) for v in order])
+    if not got:
+        print(NO_EVENTS)
         return
-    got = [re.sub(r"^byol::([A-Za-z0-9_]+).*$", r"\1", e.name) for e in events]
     want = [k for v in order for k in VARIANT_KERNELS[v]]
     assert got == want, "launched %s, expected %s" % (got, want)
     print("both variants launched exactly their kernels: %s" % got)
@@ -384,15 +374,7 @@ def _check_launches():
 def test_variants_launch_their_kernels(cuda):
     """variant="byol" launches the three loss_rows kernels and nothing else; the default launches the reference
     loss's three.  In a fresh Python process, as tests/test_gpu_optim_exact.py does."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([root] + [p for p in [os.environ.get("PYTHONPATH")] if p]))
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
-        "-c", "from tests.test_gpu_paper_loss import _check_launches; _check_launches()"]
-    r = subprocess.run(cmd, cwd=root, env=env, capture_output=True, text=True, timeout=900)
-    print(r.stdout[-2000:])
-    assert r.returncode == 0, r.stderr[-4000:]
-    if r.stdout.startswith("SKIP"):
-        pytest.skip(r.stdout.strip())
+    check_in_fresh_process(__name__)
 
 
 # ------------------------------------------------------------------------------------------------------------------

@@ -15,18 +15,17 @@
 * Replay.  One eager step each of ResNet-18 and a bottleneck net at precision = backward_precision = "fp32", and of
   ResNet-18 at precision "bf16x2", records the split path's calls, and every distinct call is replayed.
 """
-import os
 import re
-import subprocess
-import sys
 
 import pytest
 import torch
 
-from tests.test_gpu_conv_exact import Case, _conv64, _dgrad64, _gen, _wgrad64, igemm_route
-from tests.test_gpu_elementwise_exact import (_same, nchw_to_planes_case, prep_weight_dgrad_planes_case,
+from tests.exact import (Case, byol_train_step, check_in_fresh_process, check_row_launches, conv64, dgrad64, expect,
+                         recording, replay, row_case, run_and_check, wgrad64)
+from tests.test_gpu_conv_exact import igemm_route
+from tests.test_gpu_elementwise_exact import (nchw_to_planes_case, prep_weight_dgrad_planes_case,
                                               prep_weight_planes_case, split_planes_case)
-from tests.util import ints, report_mismatch
+from tests.util import ints
 
 pytestmark = pytest.mark.gpu
 BF, F32, F64 = torch.bfloat16, torch.float32, torch.float64
@@ -88,13 +87,12 @@ def _assert_exact(name, mag):
     assert top < 2 ** 24, "%s: operands not exact: a sum of |products| reaches %.3g units of 2^-6" % (name, top)
 
 
+def _nan_counts(got, want):
+    return " | NaN: %d got, %d expected" % (int(torch.isnan(got).sum()), int(torch.isnan(want).sum()))
+
+
 def _expect(name, got, ref64):
-    want = ref64.reshape(got.shape).float()
-    if _same(got, want):
-        return
-    _, msg = report_mismatch(name, got.reshape(-1, got.shape[-1]), want.reshape(-1, got.shape[-1]), 0.0, 0.0)
-    nan_got, nan_want = int(torch.isnan(got).sum()), int(torch.isnan(want).sum())
-    raise AssertionError("%s | NaN: %d got, %d expected" % (msg, nan_got, nan_want))
+    expect(name, got, ref64, note=_nan_counts)
 
 
 def _poison(planes):
@@ -155,8 +153,8 @@ def fprop_case(dev, g, T, n, h, w, c, cout, k, s, p, bias=False, linear=False, n
         return [ops.conv_fprop(xd, wf, k, k, s, p, bias=bf, out_fp32=True)]
 
     def check(outs):
-        ref = _terms(T, lambda a, bb: _conv64(xp[a], wq[bb], s, p))
-        mag = _terms(T, lambda a, bb: _conv64(_fin_abs(xp[a]), wq[bb].abs(), s, p))
+        ref = _terms(T, lambda a, bb: conv64(xp[a], wq[bb], s, p))
+        mag = _terms(T, lambda a, bb: conv64(_fin_abs(xp[a]), wq[bb].abs(), s, p))
         if bias:
             ref, mag = ref + b, mag + b.abs()
         _assert_exact("y", mag)
@@ -187,8 +185,8 @@ def dgrad_case(dev, g, T, n, h, w, cin, cout, k, s, p, resid=False, linear=False
         return [ops.conv_dgrad_planes(dyd, wd, h, w, k, k, s, p, T, resid=rf)]
 
     def check(outs):
-        ref = _terms(T, lambda a, b: _dgrad64(dyp[a], wq[b], h, w, s, p))
-        mag = _terms(T, lambda a, b: _dgrad64(_fin_abs(dyp[a]), wq[b].abs(), h, w, s, p))
+        ref = _terms(T, lambda a, b: dgrad64(dyp[a], wq[b], h, w, s, p))
+        mag = _terms(T, lambda a, b: dgrad64(_fin_abs(dyp[a]), wq[b].abs(), h, w, s, p))
         if resid:
             ref, mag = ref + r, mag + r.abs()
         _assert_exact("dx", mag)
@@ -233,8 +231,8 @@ def wgrad_case(dev, g, T, n, h, w, c, cin_real, cout, k, s, p, ldy=None, nonfini
 
     def check(outs):
         buf = outs[0]
-        ref = _terms(T, lambda a, b: _wgrad64(xp[b][..., :cin_real], dyp[a], dw0.shape, s, p)) + dw0
-        mag = _terms(T, lambda a, b: _wgrad64(_fin_abs(xp[b][..., :cin_real]), dyp[a].abs(), dw0.shape, s, p))
+        ref = _terms(T, lambda a, b: wgrad64(xp[b][..., :cin_real], dyp[a], dw0.shape, s, p)) + dw0
+        mag = _terms(T, lambda a, b: wgrad64(_fin_abs(xp[b][..., :cin_real]), dyp[a].abs(), dw0.shape, s, p))
         _assert_exact("dw", mag + dw0.abs())
         _expect("dw", buf[guard:guard + numel].view(dw0.shape), ref)
         margins = torch.cat([buf[:guard], buf[guard + numel:]])
@@ -329,62 +327,31 @@ ROWS["wgrad_nonfinite_t6"] = (W, dict(T=6, n=2, h=10, w=10, c=64, cin_real=64, c
 ROWS["near_flt_max_t6"] = (near_max_case, dict(m=64, k=64, n=64))
 
 
-def _build(name, dev):
-    builder, kw = ROWS[name]
-    return builder(dev, _gen(dev, sum(map(ord, name))), **kw)
+def _build(dev, name):
+    return row_case(dev, name, *ROWS[name])
 
 
 @pytest.mark.parametrize("name", list(ROWS))
 def test_plane_row_exact(cuda, name):
-    case = _build(name, cuda)
-    outs = case.run()
-    torch.cuda.synchronize()
-    case.check(outs)
-
-
-def _kernel_names(run):
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        run()
-        torch.cuda.synchronize()
-    return [e.name.replace(" ", "") for e in prof.events() if "kernel" in e.name]
+    run_and_check(_build(cuda, name))
 
 
 def _check_launches():
-    dev = torch.device("cuda:0")
-    cases = {name: _build(name, dev) for name in ROWS}
-    for case in cases.values():          # first launches (shared-memory opt-in, scratch) outside the profiler
-        case.run()
-    torch.cuda.synchronize()
-    wrong, seen_any = [], False
-    for name, case in cases.items():
-        names = _kernel_names(case.run)
-        seen_any = seen_any or bool(names)
-        if not names:
-            continue
-        convs = sorted({k for k in names if re.search(r"conv_(igemm|wgrad)_kernel|conv3x3|gemm_fused|stem_", k)})
-        if not convs or not all(re.search(case.route, k) for k in convs):
-            wrong.append("%s: expected %s, launched %s" % (name, case.route, convs))
-    if not seen_any:
-        print("SKIP: torch.profiler recorded no CUDA kernel events on this system")
-        return
-    assert not wrong, "\n".join(wrong)
-    print("%d rows launched their kernels" % len(cases))
+    cases = {name: _build(torch.device("cuda:0"), name) for name in ROWS}
+
+    def complaints(name, launched):
+        convs = sorted({k for k in launched if re.search(r"conv_(igemm|wgrad)_kernel|conv3x3|gemm_fused|stem_", k)})
+        if not convs or not all(re.search(cases[name].route, k) for k in convs):
+            return ["%s: expected %s, launched %s" % (name, cases[name].route, convs)]
+        return []
+    check_row_launches({name: case.run for name, case in cases.items()}, complaints)
 
 
 def test_plane_rows_launch_their_kernels(cuda):
     """Each row launches the conv_igemm_kernel / conv_wgrad_kernel variant its restated host predicate names, and no
     other variant of either.  Checked in a fresh Python process: one that has already held many profiler sessions
     (the rest of the GPU suite) can drop CUDA kernel events."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([root] + [p for p in [os.environ.get("PYTHONPATH")] if p]))
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
-        "-c", "from tests.test_gpu_split_exact import _check_launches; _check_launches()"]
-    r = subprocess.run(cmd, cwd=root, env=env, capture_output=True, text=True, timeout=900)
-    print(r.stdout[-2000:])
-    assert r.returncode == 0, r.stderr[-4000:]
-    if r.stdout.startswith("SKIP"):
-        pytest.skip(r.stdout.strip())
+    check_in_fresh_process(__name__)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -420,33 +387,6 @@ def _recorders(calls, T):
     def prep_weight_dgrad_planes(w, T_, out):
         calls.add(("prep_weight_dgrad_planes", T_, w.shape[0], w.shape[1], w.numel() // (w.shape[0] * w.shape[1])))
     return {k: v for k, v in locals().items() if callable(v)}
-
-
-def _record_step(monkeypatch, dev, arch, rep, classes, b, r, precision, backward_precision):
-    from byol_b200 import ops, wiring
-    from byol_b200.model import BYOL
-    T = {"bf16x2": 3, "fp32": 6}[precision]
-    calls = set()
-    with monkeypatch.context() as mp:
-        for name, rec in _recorders(calls, T).items():
-            orig = getattr(ops, name)
-
-            def wrapped(*a, _orig=orig, _rec=rec, **k):
-                _rec(*a, **k)
-                return _orig(*a, **k)
-            mp.setattr(ops, name, wrapped)
-        torch.manual_seed(5)
-        model = BYOL(rep, 256, classes, 10, arch=arch, precision=precision,
-                     backward_precision=backward_precision).to(dev).train()
-        model._engine.use_graphs = False
-        g = torch.Generator().manual_seed(6)
-        a1, a2 = torch.rand(b, 3, r, r, generator=g).to(dev), torch.rand(b, 3, r, r, generator=g).to(dev)
-        lab = torch.randint(0, classes, (b,), generator=g).to(dev)
-        opt = wiring.build_optimizer(model, global_batch_size=256)
-        wiring.train_step(model, opt, a1, a2, lab)
-        torch.cuda.synchronize()
-    del model, opt
-    return calls
 
 
 def _replay_case(dev, g, sig):
@@ -485,10 +425,11 @@ NETS = [("resnet18", 512, 10, 4, 64, "fp32", "fp32"), ("resnet:bottleneck:2,1,1,
         ("resnet18", 512, 1000, 4, 64, "bf16x2", "bf16")]
 
 
-def test_replay_split_calls_exactly(cuda, monkeypatch):
+def test_replay_split_calls_exactly(cuda):
     calls = set()
     for arch, rep, classes, b, r, precision, bwd in NETS:
-        calls |= _record_step(monkeypatch, cuda, arch, rep, classes, b, r, precision, bwd)
+        with recording(_recorders(calls, {"bf16x2": 3, "fp32": 6}[precision])):
+            byol_train_step(cuda, arch, rep, b, r, classes, precision=precision, backward_precision=bwd)
         torch.cuda.empty_cache()
     by_op = {}
     for sig in calls:
@@ -502,16 +443,5 @@ def test_replay_split_calls_exactly(cuda, monkeypatch):
     assert any(sig[3][3] // sig[1] > sig[4][0] for sig in by_op["conv_wgrad_planes"]), \
         "no pitched classifier wgrad recorded"
     assert {sig[1] for sig in calls} == {3, 6}, "T values recorded: %s" % sorted({sig[1] for sig in calls})
-    failures = []
-    for i, sig in enumerate(sorted(calls, key=repr)):
-        case = _replay_case(cuda, _gen(cuda, 3000 + i), sig)
-        outs = case.run()
-        torch.cuda.synchronize()
-        try:
-            case.check(outs)
-        except AssertionError as e:
-            failures.append("%s: %s" % (sig, e))
-        del outs, case
-    print("replayed %d distinct calls (%s)" % (len(calls), ", ".join("%s %d" % (op, len(v))
-                                                                     for op, v in sorted(by_op.items()))))
-    assert not failures, "%d of %d replayed calls differ:\n%s" % (len(failures), len(calls), "\n".join(failures))
+    replay(cuda, calls, _replay_case, 3000,
+           " (%s)" % ", ".join("%s %d" % (op, len(v)) for op, v in sorted(by_op.items())))

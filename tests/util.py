@@ -5,7 +5,8 @@ import numpy as np
 import torch
 
 
-# exact operands for the bit-for-bit kernel tests (test_gpu_conv_exact, test_gpu_elementwise_exact)
+# exact operands for the bit-for-bit kernel tests (the test_gpu_*_exact files and test_gpu_paper_loss; tests/exact.py
+# seeds their rows and replays with gen)
 def gen(dev, seed):
     return torch.Generator(device=dev).manual_seed(seed)
 
@@ -26,8 +27,8 @@ def pow2(n, dev, g, signed=False):
     return v
 
 
-# fp32 roundings for the numpy restatements of compiled kernel arithmetic (test_gpu_elementwise_exact,
-# test_gpu_optim_exact)
+# fp32 and fp64 roundings for the numpy restatements of compiled kernel arithmetic (test_gpu_elementwise_exact,
+# test_gpu_groupnorm_exact, test_gpu_optim_exact, test_gpu_paper_loss)
 def _rn32(fr):
     """Fraction -> the nearest fp32 (ties to even), without double rounding."""
     f = np.float32(float(fr))
@@ -61,6 +62,11 @@ def fma32(a, b, c):
         fix = np.isfinite(s) & (e != 0) & ~odd
         s = np.where(fix, np.nextafter(s, np.where(e > 0, np.inf, -np.inf)), s)
     return s.astype(np.float32)
+
+
+def fma64(a, b, c):
+    """fp64 fused multiply-add a*b + c, rounded once (elementwise over equal-length sequences)."""
+    return np.array([float(Fraction(float(x)) * Fraction(float(y)) + Fraction(float(z))) for x, y, z in zip(a, b, c)])
 
 
 def gn_finalize_restated(sums, count, eps):
